@@ -111,6 +111,7 @@ __device__ __forceinline__ void cov_to_weights(const float4 c, float &o0, float 
 struct ConeParams {
     float kappa;   // tan(acos(thresh)) = sqrt(1-t^2)/t
     float band;    // guard band per unit of S = |hx-ox|+|hy-oy|+cmax(tile) ; +inf => exact path only
+    float floor;   // lower bound of the guard band: flags every test with |h-c| <= 1e-6 (the reference's norm cut)
     float thresh;  // (float)inlier_thresh
 };
 

@@ -193,7 +193,7 @@ vote_kernel(const VoteK p)
         const float2 q = (h < a.hn) ? hyp[h] : make_float2(0.f, 0.f);
         float xc = q.x - ox, yc = q.y - oy;
         const float S = fabsf(xc) + fabsf(yc) + cmax;
-        float d = fmaxf(p.cone.band * S, 1e-30f);
+        float d = fmaxf(p.cone.band * S, p.cone.floor);    // the floor binds only for tiles narrower than ~0.4 px
         if (!(S <= 1e15f) || !(d < CUDART_INF_F)) { xc = 0.f; yc = 0.f; d = CUDART_INF_F; }   // exact path only
         hxc[j] = xc; hyc[j] = yc; dl[j] = d;
         neg[j] = 0;
@@ -275,6 +275,9 @@ vote_kernel(const VoteK p)
 // 2*(9+11*kappa)*u*S bounds twice the rounding error of m itself; 9*G*u*|h-c| is how far the reference's
 // fp32 cos can sit from the exact one, mapped into units of m; |h-c| <= S.  tools/band_check.c finds the
 // largest |m| of a fast/exact disagreement at 0.35x this bound (1e8 boundary samples).
+// The band never falls below floor = 2e-6*(kappa+1): the reference rejects every test with norm2 = |h-c| < 1e-6 whatever
+// the angle, and |m| <= (kappa+1)*|h-c| + err with err <= band*S/2.5 <= 0.4*floor, so every such test is flagged.  band*S
+// is below the floor only when S < ~0.4 px (t = 0.99), i.e. for tiles whose pixels (nearly) share one position.
 ConeParams make_cone(float thresh)
 {
     ConeParams c;
@@ -286,15 +289,18 @@ ConeParams make_cone(float thresh)
         const double band = 1.25 * ldexp(1.0, -24) * (18.0 + 22.0 * kappa + 9.0 * G);
         c.kappa = (float)kappa;
         c.band = nextafterf((float)band, INFINITY);
+        c.floor = nextafterf((float)(2e-6 * (kappa + 1.0)), INFINITY);
     } else {
         c.kappa = 0.f;
         c.band = INFINITY;   // threshold outside (0,1): exact path for every test
+        c.floor = INFINITY;
     }
     return c;
 }
 
-// 0 / 1 -> 512-pixel tile (the default); 2 / 3 -> 256 / 1024-pixel tile (tooling: tools/tune_vote.py).  Results do not
-// depend on it.  Atomic: may be flipped while other host threads launch.
+// 0 / 1 -> 1024-pixel tile (the default); 2 / 3 -> 256 / 512-pixel tile (tooling: tools/tune_vote.py).  Up to 256
+// hypotheses per keypoint the tile is always 512.  Results do not depend on it.  Atomic: may be flipped while other host
+// threads launch.
 static std::atomic<int> g_vote_variant{0};
 
 void set_vote_tuning(int variant) { g_vote_variant.store(variant, std::memory_order_relaxed); }
@@ -351,7 +357,8 @@ int refit_splits_for(int cap) { return (cap + RF_CHUNK - 1) / RF_CHUNK; }
 // The reference predicate for ONE hypothesis (the winner) against many pixels: same cone test and guard band as the
 // vote kernel, with the pixel itself as origin (d = RN(h-c) is the reference's own rounded difference) and without
 // normalising v:  m' = kappa*(v.d) - |v x d| = |v|*m,  flagged when m'^2 < (band*|d|_1)^2*|v|^2 (or anything unusual),
-// in which case the exact operation sequence decides.
+// in which case the exact operation sequence decides.  S = |d|_1 >= 2e-6 keeps |d|_2 >= 1.41e-6, clear of the reference's
+// norm2 < 1e-6 cut, which the cone test cannot see; closer hypotheses take the exact path.
 __device__ __forceinline__ bool vote_winner(float vx, float vy, float cx, float cy, float hx, float hy,
                                             const ConeParams &cone)
 {
@@ -360,7 +367,8 @@ __device__ __forceinline__ bool vote_winner(float vx, float vy, float cx, float 
     const float S = fabsf(dx) + fabsf(dy);
     const float m = cone.kappa * fmaf(vx, dx, vy * dy) - fabsf(fmaf(vx, dy, -(vy * dx)));
     const float thr = cone.band * S;
-    const bool safe = (n1sq > 1e-10f) && (n1sq < 1e8f) && (S <= 1e6f) && (m * m > thr * thr * n1sq * 1.0001f);
+    const bool safe = (n1sq > 1e-10f) && (n1sq < 1e8f) && (S >= 2e-6f) && (S <= 1e6f) &&
+                      (m * m > thr * thr * n1sq * 1.0001f);
     return safe ? (m > 0.f) : vote_exact(vx, vy, cx, cy, hx, hy, cone.thresh);
 }
 

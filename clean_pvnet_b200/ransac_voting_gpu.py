@@ -19,7 +19,8 @@ Extra keyword-only arguments (all optional; the reference call sites never pass 
     img_base   global index of image 0 (multi-GPU shards keep one philox stream)
     capacity   per-image pixel capacity of the workspace (default max_num + 8*sqrt(max_num) + 64;
                H*W whenever selection is supplied)
-    debug      also return the intermediates (tn, xy, dirs, hyp, counts, win)
+    debug      also return the intermediates (tn, xy, dirs, hyp, counts, win; for v3 also normal_eq, the refit's
+               float64 [B,K,5] normal equations (a00, a01, a11, b0, b1) summed over the winner's inliers)
 """
 import math
 import sys
@@ -38,6 +39,7 @@ _MASK_DTYPES = {
 
 _workspaces = {}
 _VALIDATE_CAPACITY = True      # tests switch it off to reach the device-side overflow report (PVB_ERR_CAPACITY)
+RF_CHUNK = 2048                # pixels per refit CTA (RF_CHUNK in csrc/vote.cu): one partial of the normal equations each
 
 
 def _workspace(device, nbytes):
@@ -115,8 +117,21 @@ def _make_desc(mask, vertex, hn, inlier_thresh, min_num, max_num, select_mode, s
     return d
 
 
-def _views(ws, d, lib):
-    """Cloned intermediates of the last call on this workspace (debug / tests)."""
+def _normal_eq(partial, tn, state, cap):
+    """The refit's normal equations per (image, keypoint), float64 [B,K,5] = (a00, a01, a11, b0, b1): the first
+    ceil(tn/RF_CHUNK) partials summed in split order, as the refit kernel's last CTA sums them (later splits hold data
+    of earlier calls).  Skipped images give zeros."""
+    nsplit = (tn.clamp(0, cap) + RF_CHUNK - 1) // RF_CHUNK
+    nsplit = torch.where(state == 0, nsplit, torch.zeros_like(nsplit))
+    acc = torch.zeros_like(partial[:, :, 0])
+    for sp in range(int(nsplit.max())):
+        use = (sp < nsplit)[:, None, None]
+        acc = acc + torch.where(use, partial[:, :, sp], torch.zeros_like(acc))
+    return acc
+
+
+def _views(ws, d, lib, refit=False):
+    """Cloned intermediates of the last call on this workspace (debug / tests); `refit`: the call ran the v3 refit."""
     L = _lib.PvbLayout()
     _lib.check(lib.pvb_workspace_layout(d, L))
     B, K, hn, cap = d.B, d.K, d.hn, L.capacity
@@ -137,6 +152,10 @@ def _views(ws, d, lib):
         win=view(L.win, B * K * 2, torch.float32).view(B, K, 2).clone(),
         capacity=cap,
     )
+    if refit:
+        assert L.refit_splits == (cap + RF_CHUNK - 1) // RF_CHUNK, "RF_CHUNK differs from csrc/vote.cu"
+        partial = view(L.refit_partial, B * K * L.refit_splits * 5, torch.float64).view(B, K, L.refit_splits, 5)
+        out["normal_eq"] = _normal_eq(partial, out["tn"], out["state"], cap)
     return out
 
 
@@ -238,7 +257,7 @@ def _run(op, mask, vertex, hn, inlier_thresh, min_num, max_num, mean=None, idxs=
         if debug:
             if B:
                 _lib.check(lib.pvb_read_status(d, ws.data_ptr(), stream))
-            info = _views(ws, d, lib) if B else {}
+            info = _views(ws, d, lib, refit=(op == "v3")) if B else {}
             info["seed"] = seed
             return out, info
     return out

@@ -290,7 +290,8 @@ PVB_API int pvb_profile_enable(int32_t every);
  *   gather_mode  access pattern of the gather kernel on an interleaved vertex tensor in device memory: 0 = auto = 1 =
  *                pixel-wise (one lane per pixel), 2 = row-wise (a warp reads whole 8*K-byte pixel rows; what in-place
  *                host reads always use)
- *   vote_variant pixel tile of the vote kernel: 0 = 1 = 512 pixels (default), 2 = 256, 3 = 1024 */
+ *   vote_variant pixel tile of the vote kernel above 256 hypotheses per keypoint: 0 = 1 = 1024 pixels (default),
+ *                2 = 256, 3 = 512; up to 256 hypotheses the tile is always 512 */
 PVB_API int pvb_set_tuning(int32_t gather_mode, int32_t vote_variant);
 PVB_API int pvb_profile_reset(void);
 PVB_API int pvb_profile_read(double *ms, int32_t n);

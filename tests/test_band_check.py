@@ -30,3 +30,14 @@ def test_no_unflagged_disagreement(band_check, thresh, local):
     ratio = float(re.search(r"analytic bound .* = ([0-9.]+)", r.stdout).group(1))
     assert mism > 1000            # the sampler really sits on the decision boundary
     assert ratio < 0.8            # worst disagreement stays well inside the analytic bound (band = 1.25 x bound)
+
+
+@pytest.mark.parametrize("thresh", ["0.99", "0.999", "0.5", "0.05"])
+def test_no_disagreement_next_to_pixels(band_check, thresh):
+    """Hypotheses within a few ulps of, or on, pixels at integer coordinates 0-15 (0 < |h-c| < 1e-6, the reference's
+    norm cut): the refit prefilter never decides one wrongly and a one-pixel vote tile flags every disagreement."""
+    r = subprocess.run([band_check, "0", thresh, "1"], stdout=subprocess.PIPE, text=True, timeout=120)
+    assert r.returncode == 0, r.stdout
+    m = re.search(r"near-pixel sweep: (\d+) tests, (\d+) rejected by the norm cut", r.stdout)
+    assert int(m.group(1)) == 256000
+    assert int(m.group(2)) > 100000          # the sweep really sits inside the norm cut

@@ -14,6 +14,8 @@ import numpy as np
 import pytest
 import torch
 
+from util import check_normal_eq, oracle_inliers
+
 pytestmark = pytest.mark.gpu
 
 
@@ -49,6 +51,7 @@ def test_cfg1_plumbing_case(pvb, oracle):
     assert np.array_equal(dbg["hyp"].cpu().numpy().view(np.uint32), odbg["hyp"].view(np.uint32))
     assert np.array_equal(dbg["counts"].cpu().numpy(), odbg["counts"])
     assert np.abs(out.cpu().numpy() - want).max() < 1e-4
+    check_normal_eq(dbg, 0.99, oracle_inliers(oracle))
     assert torch.equal(dbg["counts"][0], _counts_by_bytes(pvb, dbg, 0, 0.99))
     _, cov = pvb.estimate_voting_distribution_with_mean(mask, vertex, out, seed=12)
     _, wcov = oracle.estimate_voting_distribution_with_mean(mask.cpu().numpy(), vertex.cpu().numpy(), out.cpu().numpy(), seed=12)
@@ -98,6 +101,7 @@ def test_cfg5_stress_corners(pvb, oracle, K, hn, fill):
                                                    inlier_thresh=0.99, seed=51, debug=True)
         assert np.array_equal(odbg["counts"][0], dbg["counts"][0].cpu().numpy())
         assert np.abs(want[0] - out[0].cpu().numpy()).max() < 1e-4
+        check_normal_eq(dbg, 0.99, oracle_inliers(oracle))
     # image order / batch composition do not matter when the global image index is kept
     solo = pvb.ransac_voting_layer_v3(mask[1:2], vertex[1:2], hn, inlier_thresh=0.99, seed=51, img_base=1)
     assert torch.equal(solo[0], out[1])

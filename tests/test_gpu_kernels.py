@@ -130,8 +130,9 @@ def vote_variant():
     (1500, 2, 24, 20, 0.99), (2100, 3, 64, 21, 0.99), (3000, 2, 130, 22, 0.999), (1111, 2, 512, 23, 0.99),
     (2500, 1, 520, 24, 0.9), (1030, 2, 1100, 25, 0.99), (17, 1, 8, 26, 0.99), (1024, 1, 64, 27, 0.5)])
 def test_every_vote_kernel_matches_oracle(pvb, oracle, vote_variant, variant, tn, vn, hn, seed, thresh):
-    """Every launch shape of the vote kernel (pixel tile 512 / 256 / 1024; 1, 2 or 4 hypotheses per thread; 1, 2 or 4 warp
-    teams per CTA) at hypothesis counts on both sides of each switch-over, with partial slices and partial pixel tiles."""
+    """Every launch shape of the vote kernel (above 256 hypotheses, pixel tile 1024 / 256 / 512 for variants 1 / 2 / 3,
+    otherwise 512; 1, 2 or 4 hypotheses per thread; 1, 2 or 4 warp teams per CTA) at hypothesis counts on both sides of
+    each switch-over, with partial slices and partial pixel tiles."""
     direct, coords, idxs, _ = field_case(tn, vn, hn, seed)
     hyp = oracle.generate_hypothesis(direct, coords, idxs)
     want = oracle.vote_count(direct, coords, hyp, thresh)
@@ -171,6 +172,39 @@ def test_every_vote_kernel_adversarial(pvb, oracle, vote_variant, variant):
     vote_variant(variant)
     got = pvb.ransac_voting.vote_count(*cuda(direct, coords, hyp), 0.99).cpu().numpy()
     assert np.array_equal(got, want)
+
+
+def _ulp_ring(x, y):
+    """(x, y), and its float32 neighbours one ulp away in x, in y and in both."""
+    up, dn = np.float32(np.inf), np.float32(-np.inf)
+    xs = [np.float32(x), np.nextafter(np.float32(x), up), np.nextafter(np.float32(x), dn)]
+    ys = [np.float32(y), np.nextafter(np.float32(y), up), np.nextafter(np.float32(y), dn)]
+    return np.array([(a, b) for a in xs for b in ys], dtype=np.float32)
+
+
+@pytest.mark.parametrize("variant,hn,tile", [(1, 300, 1024), (2, 300, 256), (3, 300, 512), (1, 64, 512)])
+def test_vote_count_single_point_tiles(pvb, oracle, vote_variant, variant, hn, tile):
+    """tn = 2*tile + 1: the last tile holds one pixel, at small integer coordinates, and tile 1 has all its pixels at one
+    position.  Such tiles have a bounding box of ~0, so the guard band alone is tiny; hypotheses 1 ulp from those
+    positions (0 < |h-c| < 1e-6: the reference's norm cut) and exactly on them must still count as the reference does."""
+    rng = np.random.default_rng(variant * 1000 + hn)
+    tn, vn = 2 * tile + 1, 4
+    direct, coords, idxs, _ = field_case(tn, vn, hn, seed=variant)
+    hyp = oracle.generate_hypothesis(direct, coords, idxs)
+    coords[-1] = (3, 5)
+    coords[tile:2 * tile] = (7, 2)
+    u = np.array([(1, 0), (0, 1), (-0.6, 0.8), (0.70710677, -0.70710677)], dtype=np.float32)
+    direct[-1] = u                                   # per keypoint: which ulp neighbours lie inside the cone differs
+    ang = rng.uniform(0, 2 * np.pi, tile)
+    direct[tile:2 * tile] = np.stack([np.cos(ang), np.sin(ang)], -1).astype(np.float32)[:, None, :]
+    direct[tile:tile + 4] = u[None]                  # some of the shared-position pixels point at the ring exactly
+    near = np.concatenate([_ulp_ring(3, 5), _ulp_ring(7, 2), _ulp_ring(0, 0), _ulp_ring(1, 15)])
+    hyp[:len(near)] = near[:, None, :]
+    want = oracle.vote_count(direct, coords, hyp, 0.99)
+    vote_variant(variant)
+    got = pvb.ransac_voting.vote_count(*cuda(direct, coords, hyp), 0.99).cpu().numpy()
+    assert np.array_equal(got, want)
+    assert (want[:len(near)] > 0).any() and want.max() > 10
 
 
 def test_vote_count_empty_and_ragged(pvb, oracle):

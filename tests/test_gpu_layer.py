@@ -2,14 +2,15 @@
 through the C ABI against the CPU oracle on the same seeded inputs.
 
 Bars: selected pixel lists, sample indices, hypotheses (bit pattern), inlier counts and winners are
-exact; refit keypoints within 1e-4 px of the oracle (both accumulate in double; the reference's own
+exact; the refit's normal equations equal the sums over the reference predicate's inliers of the winner within rtol 1e-12
+(summation order; one pixel more or less is far outside it); refit keypoints within 1e-4 px of the oracle (both accumulate in double; the reference's own
 fp32 accumulation noise is ~1e-4 px, the north-star tolerance vs the reference is 1e-3 px);
 covariances within rtol 1e-5."""
 import numpy as np
 import pytest
 import torch
 
-from util import bits_equal
+from util import bits_equal, check_normal_eq, oracle_inliers, twin_inliers
 
 pytestmark = pytest.mark.gpu
 
@@ -39,6 +40,7 @@ def _check_v3(pvb, oracle, mask, vertex, hn, thresh=0.99, seed=99, img_base=0, *
     assert bits_equal(dbg["hyp"].cpu().numpy(), odbg["hyp"])
     assert np.array_equal(dbg["counts"].cpu().numpy(), odbg["counts"])
     assert bits_equal(dbg["win"].cpu().numpy(), odbg["win"])
+    check_normal_eq(dbg, thresh, oracle_inliers(oracle))
     got = out.cpu().numpy()
     assert np.isfinite(got).all()
     assert np.abs(got - want).max() < KPT_TOL
@@ -326,6 +328,18 @@ def test_full_size_counts_against_reference_formulation(pvb):
                                                 hyp[:, k0:k0 + 3].contiguous(), inl, 0.99)
         want = inl.sum(dim=2, dtype=torch.int32)                          # [hn,3]
         assert torch.equal(dbg["counts"][0, k0:k0 + 3].t().contiguous(), want)
+
+
+def test_full_size_refit_normal_equations(pvb):
+    """cfg-2 shape, B = 2 (~30 000 selected pixels = 15 refit CTAs per keypoint): the refit sums exactly the winner's
+    inliers under the reference predicate, evaluated by the byte-tensor twin kernel."""
+    mask, vertex, _ = _inputs(pvb, "cfg2", seed=1243, B=2)
+    _, dbg = pvb.ransac_voting_layer_v3(mask, vertex, 512, inlier_thresh=0.99, seed=9, debug=True)
+    tn = dbg["tn"].cpu().numpy()
+    assert (np.abs(tn - 30000) < 1200).all()
+    assert ((tn + 2047) // 2048 >= 14).all()
+    cnt = check_normal_eq(dbg, 0.99, twin_inliers(pvb))
+    assert (cnt > 1000).all()
 
 
 @pytest.mark.parametrize("H,W,K,max_num,layout", [

@@ -30,6 +30,80 @@ def bits_equal(a, b):
     return np.array_equal(a, b)
 
 
+def normal_eq_of_inliers(dirs, xy, inl):
+    """The refit's normal equations over the pixels flagged in `inl` (ransac_voting_gpu.py:177-191), in float64:
+    normal n = (v_y, -v_x), b = n.c; returns ((a00, a01, a11, b0, b1), sum over the same terms of |term|, inlier count).
+    dirs [tn,2] float32, xy [tn,2] float32, inl [tn] bool."""
+    v = np.asarray(dirs, dtype=np.float64)[inl]
+    c = np.asarray(xy, dtype=np.float64)[inl]
+    nx, ny = v[:, 1], -v[:, 0]
+    bb = nx * c[:, 0] + ny * c[:, 1]
+    terms = np.stack([nx * nx, nx * ny, ny * ny, nx * bb, ny * bb])
+    return terms.sum(axis=1), np.abs(terms).sum(axis=1), int(inl.sum())
+
+
+def reference_normal_eq(dbg, thresh, inliers_of):
+    """What the refit must sum, per (image, keypoint): the reference predicate applied to the winner
+    (voting_for_hypothesis with hn = 1, hyp = win) over the image's selected pixels.  `inliers_of(direct [tn,K,2],
+    coords [tn,2], hyp [1,K,2], thresh)` returns the uint8 inlier bytes [1,K,tn].  Returns float64 [B,K,5] sums, the
+    matching |term| sums and int [B,K] inlier counts; skipped images give zeros."""
+    tn = dbg["tn"].cpu().numpy()
+    state = dbg["state"].cpu().numpy()
+    B, K = dbg["win"].shape[:2]
+    eq, scale, cnt = np.zeros((B, K, 5)), np.zeros((B, K, 5)), np.zeros((B, K), dtype=np.int64)
+    for b in range(B):
+        n = int(tn[b])
+        if state[b] != 0 or n <= 0:
+            continue
+        xy = dbg["xy"][b, :n].cpu().numpy()
+        direct = dbg["dirs"][b, :, :n].permute(1, 0, 2).contiguous().cpu().numpy()      # [tn,K,2]
+        hyp = dbg["win"][b][None].cpu().numpy()                                         # [1,K,2]
+        inl = inliers_of(direct, xy, hyp, thresh)
+        for k in range(K):
+            eq[b, k], scale[b, k], cnt[b, k] = normal_eq_of_inliers(direct[:, k], xy, inl[0, k] != 0)
+    return eq, scale, cnt
+
+
+def oracle_inliers(oracle):
+    def inliers_of(direct, coords, hyp, thresh):
+        out = np.zeros((1, direct.shape[1], direct.shape[0]), dtype=np.uint8)
+        with np.errstate(all="ignore"):
+            oracle.voting_for_hypothesis(direct, coords, hyp, out, thresh)
+        return out
+    return inliers_of
+
+
+def twin_inliers(pvb):
+    """The same bytes from the repo's CUDA twin of the reference's voting_for_hypothesis (pinned to the reference's
+    stored output in test_gpu_reference_parity.py): for images too large for the CPU oracle."""
+    def inliers_of(direct, coords, hyp, thresh):
+        d, c, h = cuda(direct, coords, hyp)
+        out = torch.zeros((1, direct.shape[1], direct.shape[0]), dtype=torch.uint8, device="cuda")
+        pvb.ransac_voting.voting_for_hypothesis(d, c, h, out, thresh)
+        return out.cpu().numpy()
+    return inliers_of
+
+
+NEQ_RTOL = 1e-12     # the only difference left is the order of the float64 sums
+
+
+def check_normal_eq(dbg, thresh, inliers_of):
+    """The refit's normal equations (debug `normal_eq`) equal the sums over the reference predicate's inliers of the
+    winner up to float64 summation order, and the inlier count equals the winner's vote count.  One pixel too many or too
+    few changes a00 + a11 by |v|^2, far outside the bar.  Returns the reference inlier counts [B,K]."""
+    got = dbg["normal_eq"].cpu().numpy()
+    want, scale, cnt = reference_normal_eq(dbg, thresh, inliers_of)
+    assert got.shape == want.shape and got.dtype == np.float64
+    err = np.abs(got - want)
+    bad = ~(err <= NEQ_RTOL * scale)
+    assert not bad.any(), f"normal_eq mismatch at {np.argwhere(bad)[:5].tolist()}: got {got[bad][:5]}, want {want[bad][:5]}"
+    counts = dbg["counts"].cpu().numpy()
+    best = counts.max(axis=2) if counts.shape[2] else np.zeros(cnt.shape, dtype=counts.dtype)
+    voted = best > 0
+    assert np.array_equal(cnt[voted], best[voted])
+    return cnt
+
+
 def pnp_case(seed, pn=9, noise=1.0, pert=(0.05, 0.02)):
     """One synthetic uncertainty-PnP problem in the LINEMOD geometry (model points within +-10 cm, object 0.6-1.2 m away,
     LINEMOD intrinsics): (pts2d [pn,2], pts3d [pn,3], wgt2d [pn,3], K [3,3], init_rt [6], true_rt [6]), float64.
