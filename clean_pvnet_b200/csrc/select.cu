@@ -246,7 +246,8 @@ thin_gather_kernel(uint32_t *__restrict__ bits, unsigned *__restrict__ blocktot,
     __syncthreads();
     const int blk = s_blk;
     const bool thin = fg > (unsigned long long)(max_num < 0 ? 0 : max_num);   // :135
-    const float ratio = thin ? __fdiv_rn((float)max_num, (float)fg) : 0.f;     // max_num / fg.float()
+    // max_num / fg.float() is Tensor.__rtruediv__ = fg.float().reciprocal() * max_num: two roundings, as the reference
+    const float ratio = thin ? __fmul_rn(__fdiv_rn(1.f, (float)fg), (float)max_num) : 0.f;
     const int w = blk * TS_THREADS + tid;
     uint32_t word = (w < nwords) ? bits[(size_t)b * nwords + w] : 0u;
     if (thin && word) {

@@ -25,6 +25,7 @@
  *     :170-229  generate_hypothesis_vanishing_point -> orc_generate_hypothesis_vp
  *     :268-310  voting_for_hypothesis_vanishing_pt  -> orc_voting_for_hypothesis_vp
  *   lib/csrc/ransac_voting/ransac_voting_gpu.py
+ *     :125-143  pixel selection (v3), :207-227 (dist) -> orc_select_pixels
  *     :112-199  ransac_voting_layer_v3              -> orc_ransac_voting_v3
  *     :202-274  estimate_voting_distribution_with_mean -> orc_estimate_voting_distribution
  */
@@ -233,23 +234,28 @@ ORC_API void orc_voting_for_hypothesis_vp(const float *direct, const float *coor
 /* (the reference's `selection`, :136); when NULL and thinning is needed the */
 /* philox stream (seed, tag, img) is used.  Outputs pix (row-major order =   */
 /* torch.nonzero order, :140) and returns tn, or -1 when fg < min_num.       */
-/* fg_out receives the value later used as the ratio denominator:            */
-/* v3: tn (:161);  dist: foreground recomputed after thinning (:223) == tn.  */
+/* Optional (may be NULL): fg_out = fg, nz_out = pixels selected before      */
+/* thinning (cur_mask's nonzero count).                                      */
 /* ------------------------------------------------------------------------ */
 static int select_pixels(const int64_t *mask, int H, int W, int mode, int min_num, int max_num,
                          const float *selection, uint64_t seed, uint32_t tag, uint32_t img,
-                         int32_t *pix)
+                         int32_t *pix, int64_t *fg_out, int32_t *nz_out)
 {
     const int n = H * W;
     int64_t fg = 0;
+    int32_t nz = 0;
     for (int i = 0; i < n; ++i) {
-        if (mode == 0) fg += (uint8_t)mask[i];
-        else fg += (mask[i] == 1);
+        if (mode == 0) { fg += (uint8_t)mask[i]; nz += ((uint8_t)mask[i] != 0); }
+        else { fg += (mask[i] == 1); nz += (mask[i] == 1); }
     }
+    if (fg_out) *fg_out = fg;
+    if (nz_out) *nz_out = nz;
     if (fg < min_num) return -1;
     int thin = fg > max_num;
     float ratio = 0.f;
-    if (thin) ratio = (float)max_num / (float)fg;    /* max_num / foreground_num.float() */
+    /* max_num / foreground_num.float(): a Python number divided by a tensor is Tensor.__rtruediv__,
+     * i.e. reciprocal() * max_num -- two fp32 roundings, not one correctly rounded quotient */
+    if (thin) ratio = (1.f / (float)fg) * (float)max_num;
     int tn = 0;
     for (int i = 0; i < n; ++i) {
         int sel = (mode == 0) ? ((uint8_t)mask[i] != 0) : (mask[i] == 1);
@@ -261,6 +267,20 @@ static int select_pixels(const int64_t *mask, int H, int W, int mode, int min_nu
         pix[tn++] = i;
     }
     return tn;
+}
+
+/* Pixel selection alone, batched -- the front of ransac_voting_gpu.py:125-143 (mode 0, tag 2) and :207-227
+ * (mode 1, tag 4).  mask int64 [B,H*W]; selection optional float [B,H*W] (NULL: philox stream (seed, tag,
+ * img_base+b)).  Per image: fg_out[b], nz_out[b], tn_out[b] (-1 when skipped) and the first tn entries of
+ * pix[b*H*W ...] (row-major pixel indices). */
+ORC_API void orc_select_pixels(const int64_t *mask, int B, int H, int W, int mode, int min_num, int max_num,
+                               const float *selection, uint64_t seed, int img_base, uint32_t tag,
+                               int64_t *fg_out, int32_t *nz_out, int32_t *tn_out, int32_t *pix)
+{
+    const size_t HW = (size_t)H * W;
+    for (int b = 0; b < B; ++b)
+        tn_out[b] = select_pixels(mask + b * HW, H, W, mode, min_num, max_num, selection ? selection + b * HW : NULL,
+                                  seed, tag, (uint32_t)(img_base + b), pix + b * HW, fg_out + b, nz_out + b);
 }
 
 /* Least-squares ray intersection of the winner's inliers -- ransac_voting_gpu.py:177-196.
@@ -316,7 +336,7 @@ ORC_API int orc_ransac_voting_v3(const int64_t *mask, const float *vertex, int B
         if (win_out) memset(win_out + (size_t)b * K * 2, 0, sizeof(float) * K * 2);
         int tn = select_pixels(mask + b * HW, H, W, 0, min_num, max_num,
                                selection ? selection + b * HW : NULL, seed, ORC_TAG_V3_SEL,
-                               (uint32_t)(img_base + b), pix);
+                               (uint32_t)(img_base + b), pix, NULL, NULL);
         if (tn_out) tn_out[b] = tn < 0 ? 0 : tn;
         if (tn < 0) continue;                                   /* :129-132 zeros */
         if (tn == 0) continue;   /* unreachable in the reference unless thinning drops everything */
@@ -380,7 +400,7 @@ ORC_API int orc_estimate_voting_distribution(const int64_t *mask, const float *v
     for (int b = 0; b < B; ++b) {
         int tn = select_pixels(mask + b * HW, H, W, 1, min_num, max_num,
                                selection ? selection + b * HW : NULL, seed, ORC_TAG_DIST_SEL,
-                               (uint32_t)(img_base + b), pix);
+                               (uint32_t)(img_base + b), pix, NULL, NULL);
         const float *vb = vertex + (size_t)b * HW * K * 2;
         if (tn > 0)
             for (int t = 0; t < tn; ++t)

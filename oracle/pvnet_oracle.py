@@ -84,6 +84,28 @@ def vote_count(direct, coords, hyp, thresh):
     return counts
 
 
+def select_pixels(mask, mode=0, min_num=5, max_num=30000, selection=None, seed=0, img_base=0, tag=None):
+    """Pixel selection of ransac_voting_gpu.py:125-143 (mode 0: v3, `mask.byte()`, fg = sum of byte values) or
+    :207-227 (mode 1: distribution, `mask == 1`).  mask int64 [B,H,W]; selection optional float [B,H,W]; without it
+    thinning draws from the philox stream (seed, tag, img_base + b), tag defaulting to 2 (v3) / 4 (distribution).
+    Returns dict(fg int64 [B], nz int32 [B] (selected before thinning), tn int32 [B] (-1: skipped),
+    pix: list of B int32 arrays of row-major pixel indices)."""
+    mask = _c(mask, np.int64); selection = _c(selection, np.float32)
+    B, H, W = mask.shape
+    if selection is not None:
+        assert selection.shape == (B, H, W)
+    if tag is None:
+        tag = 2 if mode == 0 else 4
+    fg = np.zeros(B, dtype=np.int64)
+    nz = np.zeros(B, dtype=np.int32)
+    tn = np.zeros(B, dtype=np.int32)
+    pix = np.zeros((B, H * W), dtype=np.int32)
+    lib().orc_select_pixels(_p(mask, _i64p), B, H, W, int(mode), int(min_num), int(max_num), _p(selection, _f32p),
+                            ctypes.c_uint64(seed), int(img_base), ctypes.c_uint32(tag),
+                            _p(fg, _i64p), _p(nz, _i32p), _p(tn, _i32p), _p(pix, _i32p))
+    return dict(fg=fg, nz=nz, tn=tn, pix=[pix[b, :max(int(tn[b]), 0)].copy() for b in range(B)])
+
+
 def ransac_voting_layer_v3(mask, vertex, round_hyp_num, inlier_thresh=0.999, confidence=0.99, max_iter=20,
                            min_num=5, max_num=30000, idxs=None, selection=None, seed=0, img_base=0,
                            debug=False):

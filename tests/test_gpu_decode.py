@@ -80,3 +80,48 @@ def test_uncertainty_pnp_weights_match_reference_formula(pvb):
         want = np.asarray(cov_invs).reshape([-1, 4])[:, (0, 1, 3)]
         assert np.allclose(got[b], np.real(want), rtol=2e-4, atol=1e-6), (got[b], want)
     assert (got[0, 0] == 0).all() and (got[1, 1] == 0).all()
+
+
+def _weights_f64(c):
+    """inv(sqrtm(C)) of the symmetric part of fp32 covariances c [n,2,2] by a float64 eigendecomposition
+    V diag(lambda^-1/2) V^T, packed (wxx, wxy, wyy)."""
+    import numpy as np
+    a = c.astype(np.float64)
+    a = 0.5 * (a + a.transpose(0, 2, 1))
+    lam, V = np.linalg.eigh(a)
+    Wm = np.einsum("nij,nj,nkj->nik", V, lam ** -0.5, V)
+    return np.stack([Wm[:, 0, 0], Wm[:, 0, 1], Wm[:, 1, 1]], 1)
+
+
+def test_uncertainty_pnp_weights_sweep(pvb):
+    """Closed-form inv(sqrtm(cov)) (cov_to_weights, csrc/common.cuh) against a float64 eigendecomposition over condition
+    numbers 1..1e7, scales 1e-5..1e5 and both signs of the off-diagonal: every weight within 2 fp32 ulp (plus 1e-12 of
+    the largest weight, for an off-diagonal that vanishes).  Guards: cov[0,0] < fp32(1e-6) -> zeros (fp32(1e-6) itself
+    and the float above it are computed), NaN -> zeros, det <= 0 (rank 1, indefinite) -> zeros."""
+    import numpy as np
+    rows = []
+    for kappa in (1.0, 3.0, 1e2, 1e4, 1e5, 1e6, 1e7):
+        for scale in (1e-5, 1e-3, 1.0, 1e2, 1e5):
+            for th in (0.0, 0.3, -0.3, 1.1, -1.1, np.pi / 2):
+                R = np.array([[np.cos(th), -np.sin(th)], [np.sin(th), np.cos(th)]])
+                rows.append(R @ np.diag([scale, scale / kappa]) @ R.T)
+    c = np.asarray(rows).astype(np.float32)
+    c[:, 1, 0] = c[:, 0, 1]
+    got = pvb.uncertainty_pnp_weights(torch.from_numpy(c).cuda()).cpu().numpy()
+    live = (c[:, 0, 0] >= np.float32(1e-6)) & (np.linalg.det(c.astype(np.float64)) > 0)
+    assert live.sum() > 150 and (got[~live] == 0).all()
+    want = _weights_f64(c[live])
+    bar = 2 * np.spacing(np.abs(want).astype(np.float32)).astype(np.float64) + 1e-12 * np.abs(want).max(1, keepdims=True)
+    err = np.abs(got[live].astype(np.float64) - want)
+    assert (err <= bar).all(), (np.max(err / bar), c[live][np.argmax((err / bar).max(1))])
+    assert np.signbit(got[live][:, 1][np.abs(want[:, 1]) > 1e-3 * np.abs(want).max(1)]).tolist() == \
+        np.signbit(want[:, 1][np.abs(want[:, 1]) > 1e-3 * np.abs(want).max(1)]).tolist()
+    # the cov[0,0] guard at fp32(1e-6) and its neighbours; NaN; rank 1; indefinite; zero
+    e = np.float32(1e-6)
+    g = np.array([[[np.nextafter(e, np.float32(0)), 0], [0, 1]], [[e, 0], [0, 1]], [[np.nextafter(e, np.float32(1)), 0], [0, 1]],
+                  [[np.nan, 0], [0, 1]], [[1, 0], [0, np.nan]], [[1, 2], [2, 4]], [[4, 2], [2, 1]], [[1, 3], [3, 1]],
+                  [[1e-3, 0], [0, -1e-3]], [[0, 0], [0, 0]], [[2, 1e3], [1e3, 2]]], dtype=np.float32)
+    w = pvb.uncertainty_pnp_weights(torch.from_numpy(g).cuda()).cpu().numpy()
+    assert (w[0] == 0).all() and (w[3:] == 0).all()
+    want = _weights_f64(g[1:3])
+    assert (np.abs(w[1:3] - want) <= 2 * np.spacing(np.abs(want).astype(np.float32)) + 1e-12 * np.abs(want).max()).all()

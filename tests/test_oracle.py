@@ -223,3 +223,77 @@ def test_cfg1_cpu_plumbing_case(oracle):
     _, cov = oracle.estimate_voting_distribution_with_mean(m, v, out, seed=12)
     assert cov.shape == (1, 1, 2, 2) and np.isfinite(cov).all()
     assert dt < 5.0                                                    # 64 x 5 000 tests: milliseconds on one core
+
+
+def _torch_select(mask, mode, min_num, max_num, selection):
+    """The reference's selection ops, one image at a time on CPU tensors (ransac_voting_gpu.py:125-143 for mode 0,
+    :205-227 for mode 1): fg, nz, tn (-1 = skipped) and the row-major indices torch.nonzero returns."""
+    import torch
+    res = []
+    for bi in range(mask.shape[0]):
+        cur_mask = mask[bi].byte() if mode == 0 else (mask[bi] == 1)
+        foreground_num = torch.sum(cur_mask)
+        nz = int(torch.count_nonzero(cur_mask))
+        if foreground_num < min_num:
+            res.append((int(foreground_num), nz, -1, np.zeros(0, np.int64)))
+            continue
+        if foreground_num > max_num:
+            selected_mask = selection[bi] < (max_num / foreground_num.float())   # fp32, strict
+            cur_mask = cur_mask * selected_mask.to(cur_mask.dtype)
+        pix = torch.nonzero(cur_mask.reshape(-1))[:, 0].numpy()
+        res.append((int(foreground_num), nz, len(pix), pix))
+    return res
+
+
+def test_select_pixels_matches_torch_ops(oracle):
+    """orc_select_pixels with explicit draws against the reference's own torch ops: byte values (wrap-around, sums of
+    values above 1), `== 1` for the distribution op, the fp32 ratio `max_num / fg.float()` (torch evaluates it as
+    reciprocal() * max_num) compared strictly, draws placed exactly on that ratio, one ulp below it and at 0."""
+    import torch
+    rng = np.random.default_rng(21)
+    B, H, W = 12, 37, 53
+    vals = np.array([0, 0, 0, 0, 1, 1, 1, 2, 3, 255, 256, 257, -1, -255, 2 ** 32 + 1], np.int64)
+    mask = np.zeros((B, H, W), np.int64)
+    for b in range(B):
+        fill = [0.02, 0.1, 0.3, 0.6, 0.9][b % 5]
+        on = rng.uniform(size=(H, W)) < fill
+        mask[b] = np.where(on, rng.choice(vals, size=(H, W)), 0)
+    mask[11] = 0
+    mask[11, 3, 2:6] = 1                                   # 4 pixels: skipped at min_num 5 (both modes)
+    sel = rng.uniform(size=(B, H, W)).astype(np.float32)
+    mt, st = torch.from_numpy(mask), torch.from_numpy(sel)
+    for mode in (0, 1):
+        for max_num in (40, 200, 30000):
+            # plant draws on the ratio boundary of every thinned image
+            fgs = [r[0] for r in _torch_select(mt, mode, 5, max_num, st)]
+            s2 = sel.copy()
+            for b, fg in enumerate(fgs):
+                if fg > max_num:
+                    ratio = (torch.tensor(fg).float().reciprocal() * max_num).item()
+                    r32 = np.float32(ratio)
+                    assert r32 == (max_num / torch.tensor(fg).float()).item()
+                    on = np.flatnonzero(mask[b].reshape(-1) != 0)
+                    s2[b].reshape(-1)[on[0::3]] = r32                                        # dropped
+                    s2[b].reshape(-1)[on[1::3]] = np.nextafter(r32, np.float32(0))           # kept
+                    s2[b].reshape(-1)[on[2::7]] = 0.0                                        # kept
+            want = _torch_select(mt, mode, 5, max_num, torch.from_numpy(s2))
+            got = oracle.select_pixels(mask, mode, 5, max_num, selection=s2)
+            for b in range(B):
+                fg, nz, tn, pix = want[b]
+                assert (int(got["fg"][b]), int(got["nz"][b]), int(got["tn"][b])) == (fg, nz, tn), (mode, max_num, b)
+                assert np.array_equal(got["pix"][b], pix), (mode, max_num, b)
+    # the value semantics the expectations above rest on
+    assert mt.byte()[mt == 256].eq(0).all() and mt.byte()[mt == -1].eq(255).all() and mt.byte()[mt == 2 ** 32 + 1].eq(1).all()
+    # the ratio is NOT the correctly rounded quotient for every fg: the oracle must follow torch where they differ
+    fg = 30001
+    assert np.float32(30000) / np.float32(fg) != (30000 / torch.tensor(fg).float()).item()
+    m1 = np.ones((1, 1, fg), np.int64)
+    r = np.float32((30000 / torch.tensor(fg).float()).item())
+    s1 = np.full((1, 1, fg), 0.99999, np.float32)
+    s1[0, 0, :5] = [r, np.nextafter(r, np.float32(2)), np.nextafter(r, np.float32(0)), 0.0, np.float32(30000) / np.float32(fg)]
+    got = oracle.select_pixels(m1, 0, 5, 30000, selection=s1)
+    assert got["tn"][0] == 2 + (s1[0, 0, 4] < r) and list(got["pix"][0][:2]) == [2, 3]
+    # philox draws (selection=None) follow the tag: v3 and the distribution op thin with different streams
+    a = oracle.select_pixels(mask, 0, 5, 40, seed=5)
+    b = oracle.select_pixels(mask, 0, 5, 40, seed=5, tag=4)
+    assert np.array_equal(a["fg"], b["fg"]) and any(not np.array_equal(x, y) for x, y in zip(a["pix"], b["pix"]))

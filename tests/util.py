@@ -131,3 +131,42 @@ def pnp_case(seed, pn=9, noise=1.0, pert=(0.05, 0.02)):
     true_rt = np.concatenate([aa, t])
     init = true_rt + np.concatenate([rng.normal(size=3) * pert[0], rng.normal(size=3) * pert[1]])
     return uv, pts3d, wgt, K, init, true_rt
+
+
+def restated_covariance(dbg, mean):
+    """float64 restatement of covariance_kernel (ransac_voting_gpu.py:243-244, 254-269) from the distribution op's
+    debug `hyp` [B,K,hn,2] and `counts` [B,K,hn]: ratio = fp32(count) / fp32(tn) (skipped images: hyp 0, ratio 1),
+    th = fp32(max - 0.1f), w = 0 where w < th, d = fp32(hyp - mean), S = sum w*d*d^T in float64,
+    den = fp32(fp32(sum w) + 1e-3f).  Returns (S / den as float64 [B,K,2,2], the matching sums of |term| / den)."""
+    hyp = dbg["hyp"].cpu().numpy()
+    counts = dbg["counts"].cpu().numpy()
+    tn = dbg["tn"].cpu().numpy()
+    skipped = (dbg["state"].cpu().numpy() != 0)[:, None, None]
+    mean = np.asarray(mean.cpu() if isinstance(mean, torch.Tensor) else mean, dtype=np.float32)
+    with np.errstate(all="ignore"):
+        ratio = np.where(skipped, np.float32(1), counts.astype(np.float32) / tn.astype(np.float32)[:, None, None])
+        hyp = np.where(skipped[..., None], np.float32(0), hyp)
+        th = (ratio.max(axis=2) - np.float32(0.1)).astype(np.float32)
+        w = np.where(ratio < th[..., None], np.float32(0), ratio).astype(np.float64)
+        d = (hyp - mean[:, :, None, :]).astype(np.float64)               # fp32 difference, then widened
+        t00, t01, t11 = d[..., 0] * (d[..., 0] * w), d[..., 0] * (d[..., 1] * w), d[..., 1] * (d[..., 1] * w)
+        den = (np.float32(w.sum(axis=2)) + np.float32(1e-3)).astype(np.float64)
+        S = np.stack([t00.sum(2), t01.sum(2), t01.sum(2), t11.sum(2)], -1).reshape(hyp.shape[:2] + (2, 2))
+        A = np.stack([np.abs(t00).sum(2), np.abs(t01).sum(2), np.abs(t01).sum(2), np.abs(t11).sum(2)], -1)
+        return S / den[..., None, None], A.reshape(S.shape) / den[..., None, None]
+
+
+def check_covariance(cov, dbg, mean):
+    """The op's covariance against restated_covariance: every entry within 1 fp32 ulp of the float64 value, plus
+    1e-12 * sum|terms| / den (float64 summation order, matters only for off-diagonals that cancel to ~0); NaN exactly
+    where the restatement is NaN; the two off-diagonals bit-equal.  Returns the restated float64 covariance."""
+    got = cov.cpu().numpy().astype(np.float64)
+    want, scale = restated_covariance(dbg, mean)
+    nan = np.isnan(want)
+    assert np.array_equal(np.isnan(got), nan), np.argwhere(np.isnan(got) != nan)[:5]
+    bar = np.spacing(np.abs(want[~nan]).astype(np.float32)).astype(np.float64) + 1e-12 * scale[~nan]
+    err = np.abs(got[~nan] - want[~nan])
+    assert (err <= bar).all(), f"cov off by {np.max(err / bar):.2f}x the bar; got {got[~nan][err > bar][:4]}, want {want[~nan][err > bar][:4]}"
+    c = cov.cpu().numpy()
+    assert bits_equal(c[..., 0, 1], c[..., 1, 0])
+    return want
