@@ -154,6 +154,10 @@ PVB_HD void p3p_select4(const double *w /*[pn][3]*/, int pn, int *idx)
 // Writes rt[6] = (angle-axis, translation).  Returns the number of admissible solutions found (0: rt untouched).
 PVB_HD int p3p_solve4(const double X[4][3], const double x2[4][2], const double *cam, double *rt)
 {
+    // Three coincident image points (an image the voting layer skipped: every keypoint at 0) put the three bearings on one
+    // ray, which cannot carry three non-collinear model points: no solution.  Tested up front because with cos = 1 the
+    // quartic degenerates and its rounding noise can pass for a root (the device build, with FMA contraction, found one).
+    if (x2[0][0] == x2[1][0] && x2[0][1] == x2[1][1] && x2[0][0] == x2[2][0] && x2[0][1] == x2[2][1]) return 0;
     double f[4][3];
     for (int i = 0; i < 4; ++i) {
         f[i][0] = (x2[i][0] - cam[2]) / cam[0]; f[i][1] = (x2[i][1] - cam[3]) / cam[1]; f[i][2] = 1.0;

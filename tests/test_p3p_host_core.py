@@ -121,6 +121,9 @@ def test_degenerate_triples_report_no_solution(p3p):
     X[2] = X[0] + 2.0 * (X[1] - X[0])                                  # collinear model points
     n, rt = p3p(X, x2, K)
     assert n == 0 and np.isnan(rt).all()
+    for pt in ([0.0, 0.0], uv[0]):                                     # coincident image points (a skipped image: all 0)
+        n, rt = p3p(p3[:4], np.tile(pt, (4, 1)), K)
+        assert n == 0 and np.isnan(rt).all()
 
 
 def test_selection_of_the_four_best_weighted_points(p3p):
@@ -135,3 +138,57 @@ def test_selection_of_the_four_best_weighted_points(p3p):
             w[rng.integers(0, pn), 0] = np.nan
         want = list(np.argsort(w[:, 0] + w[:, 1], kind="stable")[-4:])
         assert p3p.select4(w) == want, (trial, w)
+
+
+def test_tied_keys_take_the_stable_tail(p3p):
+    """The tie rule, pinned: among equal keys the larger index ranks higher (the tail of a stable ascending argsort).  The
+    reference calls np.argsort with numpy's default kind, whose order among ties depends on the sort implementation numpy
+    was built with and dispatches to (with numpy 2.3 on an AVX-512 host it picks [13 15 16 3] here); this project keeps
+    the stable tail, so the choice does not depend on the machine (DESIGN.md section 8 row 3)."""
+    w = np.zeros((17, 3))
+    w[3, 0] = 1.0
+    assert p3p.select4(w) == [14, 15, 16, 3] == list(np.argsort(w[:, 0] + w[:, 1], kind="stable")[-4:])
+    w = np.zeros((9, 3))
+    w[2, 1] = 2.0
+    w[[0, 4], 0] = -0.5                                               # negative keys rank below the zero-weight keypoints
+    assert p3p.select4(w) == [6, 7, 8, 2]
+    assert p3p.select4(np.zeros((9, 3))) == [5, 6, 7, 8]              # a skipped image: the last four keypoints
+
+
+def _fp32_fixture():
+    return np.load(os.path.join(ROOT, "tests", "golden", "ceres_pnp_fp32.npz"))
+
+
+def test_fp32_fixture_p3p_matches_stored_opencv(p3p):
+    """tests/golden/ceres_pnp_fp32.npz stores OpenCV's P3P pose on the stable top four (`p3ps_rt`) of every problem with
+    pn >= 4: p3p_select4 picks those four, and p3p_solve4 gives OpenCV's pose to 1e-6 unless the fourth point cannot tell
+    the candidates apart (the allowance of test_selected_pose_matches_opencv_p3p); where OpenCV has no finite pose (the
+    skipped images: four coincident image points) it reports no solution."""
+    F = _fp32_fixture()
+    ties = checked = 0
+    for i in range(len(F["pn"])):
+        pn = int(F["pn"][i])
+        if pn < 4:
+            continue
+        w = F["wgt2d"][i, :pn].astype(np.float64)
+        idx = p3p.select4(w)
+        assert idx == F["idx_stable"][i].tolist(), i
+        uv, X, K = F["kpt2d"][i, :pn].astype(np.float64)[idx], F["pts3d"][i, :pn][idx], F["K"][i]
+        n, rt = p3p(X, uv, K)
+        want = F["p3ps_rt"][i]
+        if not np.isfinite(want).all():
+            assert n == 0 and np.isnan(rt).all(), i
+            continue
+        checked += 1
+        assert n >= 1, i
+        d = max(np.abs(_rodrigues(rt[:3]) - _rodrigues(want[:3])).max(), np.abs(rt[3:] - want[3:]).max())
+        if d > 1e-6:
+            e_ours = np.linalg.norm(_reproject(rt, X[3:], K) - uv[3:])
+            e_cv = np.linalg.norm(_reproject(want, X[3:], K) - uv[3:])
+            assert abs(e_ours - e_cv) <= 1e-3 * e_cv and e_ours <= e_cv * (1 + 1e-9), i
+            ties += 1
+    assert checked >= 200 and ties <= 2
+    # where the two sort kinds picked the same four, the reference's own start is the stored stable one
+    same = (F["idx_default"] == F["idx_stable"]).all(1)
+    assert np.array_equal(F["p3p_rt"][same], F["p3ps_rt"][same], equal_nan=True)
+    assert (~same).sum() >= 4 and (F["kind"][~same] == "zeros").all()              # ties only where keys are zero

@@ -133,6 +133,23 @@ def pnp_case(seed, pn=9, noise=1.0, pert=(0.05, 0.02)):
     return uv, pts3d, wgt, K, init, true_rt
 
 
+def cov_to_weights_f32(cov):
+    """float64 restatement of cov_to_weights (csrc/common.cuh): fp32 covariances [..., 2, 2] -> fp32 (wxx, wxy, wyy) [..., 3].
+    Closed-form inv(sqrtm) of the symmetric part; cov[0,0] < fp32(1e-6), any NaN or det <= 0 -> zeros."""
+    c = np.asarray(cov, np.float32).reshape(-1, 4)
+    with np.errstate(all="ignore"):
+        a, b, d = c[:, 0].astype(np.float64), 0.5 * (c[:, 1].astype(np.float64) + c[:, 2].astype(np.float64)), c[:, 3].astype(np.float64)
+        det = a * d - b * b
+        s = np.sqrt(det)
+        t = np.sqrt(a + d + 2.0 * s)
+        a2, d2 = a + s, d + s
+        den = a2 * d2 - b * b
+        w = np.stack([t * d2 / den, -t * b / den, t * a2 / den], 1).astype(np.float32)
+    live = ~((c[:, 0] < np.float32(1e-6)) | np.isnan(c).any(1)) & (det > 0.0)
+    w[~live] = 0.0
+    return w.reshape(np.shape(cov)[:-2] + (3,))
+
+
 def restated_covariance(dbg, mean):
     """float64 restatement of covariance_kernel (ransac_voting_gpu.py:243-244, 254-269) from the distribution op's
     debug `hyp` [B,K,hn,2] and `counts` [B,K,hn]: ratio = fp32(count) / fp32(tn) (skipped images: hyp 0, ratio 1),
