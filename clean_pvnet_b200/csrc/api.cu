@@ -377,26 +377,44 @@ PVB_API int pvb_uncertainty_weights(const float *cov, float *weights, int32_t n,
     return e == cudaSuccess ? PVB_OK : cuda_fail(e, "pnp weights kernel");
 }
 
+namespace {
+
+// The checks every PnP entry point makes after its own ones on n and pn: NULL tensors (`given`: every required pointer is
+// set), then the strides.
+int pnp_check_inputs(int32_t n, bool given, int64_t pts3d_stride, int64_t k_stride)
+{
+    if (n && !given) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (pts3d_stride < 0 || k_stride < 0) return fail(PVB_ERR_INVALID, "negative stride");
+    return PVB_OK;
+}
+
+// options == NULL: Ceres' defaults
+int pnp_read_options(const pvb_pnp_options *options, PnpOptions &opt)
+{
+    opt = pnp_default_options();
+    if (!options) return PVB_OK;
+    if (options->max_num_iterations < 0 || !(options->function_tolerance >= 0.0) || !(options->gradient_tolerance >= 0.0) ||
+        !(options->parameter_tolerance >= 0.0))
+        return fail(PVB_ERR_INVALID, "pvb_pnp_options: negative or NaN entry");
+    opt.max_num_iterations = options->max_num_iterations; opt.function_tolerance = options->function_tolerance;
+    opt.gradient_tolerance = options->gradient_tolerance; opt.parameter_tolerance = options->parameter_tolerance;
+    return PVB_OK;
+}
+
+} // namespace
+
 PVB_API int pvb_uncertainty_pnp(const double *pts2d, const double *pts3d, const double *wgt2d, const double *K,
                                 const double *init_rt, double *result_rt, int32_t *info, int32_t n, int32_t pn,
                                 int64_t pts3d_stride, int64_t k_stride, const pvb_pnp_options *options, pvb_stream_t stream)
 {
     if (n < 0) return fail(PVB_ERR_INVALID, "n < 0");
     if (pn < 1) return fail(PVB_ERR_INVALID, "pn must be >= 1 (got %d)", pn);
-    if (n && (!pts2d || !pts3d || !wgt2d || !K || !init_rt || !result_rt)) return fail(PVB_ERR_INVALID, "NULL tensor");
-    if (pts3d_stride < 0 || k_stride < 0) return fail(PVB_ERR_INVALID, "negative stride");
-    PnpArgs a;
-    a.pts2d = pts2d; a.pts3d = pts3d; a.wgt2d = wgt2d; a.K = K; a.init_rt = init_rt; a.result_rt = result_rt; a.info = info;
+    PnpArgs a = {};
+    if (int rc = pnp_check_inputs(n, pts2d && pts3d && wgt2d && K && init_rt && result_rt, pts3d_stride, k_stride)) return rc;
+    if (int rc = pnp_read_options(options, a.opt)) return rc;
+    a.pts2d = pts2d; a.wgt2d = wgt2d; a.pts3d = pts3d; a.K = K; a.init_rt = init_rt; a.result_rt = result_rt; a.info = info;
     a.n = n; a.pn = pn; a.pts3d_stride = pts3d_stride; a.k_stride = k_stride;
-    a.max_num_iterations = 50; a.function_tolerance = 1e-6; a.gradient_tolerance = 1e-10; a.parameter_tolerance = 1e-8;
-    if (options) {
-        if (options->max_num_iterations < 0 || !(options->function_tolerance >= 0.0) || !(options->gradient_tolerance >= 0.0) ||
-            !(options->parameter_tolerance >= 0.0))
-            return fail(PVB_ERR_INVALID, "pvb_pnp_options: negative or NaN entry");
-        a.max_num_iterations = options->max_num_iterations; a.function_tolerance = options->function_tolerance;
-        a.gradient_tolerance = options->gradient_tolerance; a.parameter_tolerance = options->parameter_tolerance;
-    }
-    cudaError_t e = launch_pnp(a, static_cast<cudaStream_t>(stream));
+    cudaError_t e = launch_pnp_batch(a, static_cast<cudaStream_t>(stream));
     return e == cudaSuccess ? PVB_OK : cuda_fail(e, "uncertainty pnp kernel");
 }
 
@@ -408,24 +426,20 @@ PVB_API int pvb_uncertainty_pnp_from_votes(const float *kpt_2d, const float *cov
     if (n < 0) return fail(PVB_ERR_INVALID, "n < 0");
     if (pn < 1 || pn > PNP_FUSED_MAX_PN) return fail(PVB_ERR_INVALID, "pn must be in [1,%d] (got %d)", PNP_FUSED_MAX_PN, pn);
     if (!init_rt && pn < 4) return fail(PVB_ERR_INVALID, "the P3P initialisation needs pn >= 4 (got %d)", pn);
-    if (n && (!kpt_2d || !pts3d || !K || !result_rt)) return fail(PVB_ERR_INVALID, "NULL tensor");
-    if (n && ((cov == nullptr) == (weights == nullptr))) return fail(PVB_ERR_INVALID, "pass exactly one of cov / weights");
-    if (pts3d_stride < 0 || k_stride < 0) return fail(PVB_ERR_INVALID, "negative stride");
+    const bool given = kpt_2d && pts3d && K && result_rt;
+    // before pnp_check_inputs, but only once every required tensor is set: a caller keeps getting "NULL tensor" first,
+    // then this, then "negative stride"
+    if (n && given && ((cov == nullptr) == (weights == nullptr)))
+        return fail(PVB_ERR_INVALID, "pass exactly one of cov / weights");
+    PnpArgs a = {};
+    if (int rc = pnp_check_inputs(n, given, pts3d_stride, k_stride)) return rc;
     if ((reinterpret_cast<uintptr_t>(kpt_2d) & 7u) || (reinterpret_cast<uintptr_t>(cov) & 15u))
         return fail(PVB_ERR_INVALID, "kpt_2d must be 8-byte and cov 16-byte aligned");
-    PnpFusedArgs a;
-    a.kpt2d = kpt_2d; a.cov = cov; a.weights = weights; a.pts3d = pts3d; a.K = K; a.init_rt = init_rt; a.result_rt = result_rt;
-    a.init_out = init_out; a.weights_out = weights_out; a.info = info; a.n = n; a.pn = pn;
-    a.pts3d_stride = pts3d_stride; a.k_stride = k_stride;
-    a.max_num_iterations = 50; a.function_tolerance = 1e-6; a.gradient_tolerance = 1e-10; a.parameter_tolerance = 1e-8;
-    if (options) {
-        if (options->max_num_iterations < 0 || !(options->function_tolerance >= 0.0) || !(options->gradient_tolerance >= 0.0) ||
-            !(options->parameter_tolerance >= 0.0))
-            return fail(PVB_ERR_INVALID, "pvb_pnp_options: negative or NaN entry");
-        a.max_num_iterations = options->max_num_iterations; a.function_tolerance = options->function_tolerance;
-        a.gradient_tolerance = options->gradient_tolerance; a.parameter_tolerance = options->parameter_tolerance;
-    }
-    cudaError_t e = launch_pnp_fused(a, static_cast<cudaStream_t>(stream));
+    if (int rc = pnp_read_options(options, a.opt)) return rc;
+    a.kpt2d = kpt_2d; a.cov = cov; a.weights = weights; a.weights_out = weights_out; a.pts3d = pts3d; a.K = K;
+    a.init_rt = init_rt; a.init_out = init_out; a.result_rt = result_rt; a.info = info;
+    a.n = n; a.pn = pn; a.pts3d_stride = pts3d_stride; a.k_stride = k_stride;
+    cudaError_t e = launch_pnp_batch(a, static_cast<cudaStream_t>(stream));
     return e == cudaSuccess ? PVB_OK : cuda_fail(e, "fused uncertainty pnp kernel");
 }
 
@@ -435,13 +449,11 @@ PVB_API int pvb_uncertainty_pnp_init(const double *pts2d, const double *pts3d, c
 {
     if (n < 0) return fail(PVB_ERR_INVALID, "n < 0");
     if (pn < 4) return fail(PVB_ERR_INVALID, "P3P needs pn >= 4 (got %d)", pn);
-    if (n && (!pts2d || !pts3d || !wgt2d || !K || !init_rt)) return fail(PVB_ERR_INVALID, "NULL tensor");
-    if (pts3d_stride < 0 || k_stride < 0) return fail(PVB_ERR_INVALID, "negative stride");
-    PnpArgs a;
-    a.pts2d = pts2d; a.pts3d = pts3d; a.wgt2d = wgt2d; a.K = K; a.init_rt = nullptr; a.result_rt = init_rt; a.info = nullptr;
+    if (int rc = pnp_check_inputs(n, pts2d && pts3d && wgt2d && K && init_rt, pts3d_stride, k_stride)) return rc;
+    PnpArgs a = {};                    // no result_rt: the P3P start alone, written to init_out
+    a.pts2d = pts2d; a.wgt2d = wgt2d; a.pts3d = pts3d; a.K = K; a.init_out = init_rt;
     a.n = n; a.pn = pn; a.pts3d_stride = pts3d_stride; a.k_stride = k_stride;
-    a.max_num_iterations = 0; a.function_tolerance = a.gradient_tolerance = a.parameter_tolerance = 0.0;
-    cudaError_t e = launch_p3p_init(a, static_cast<cudaStream_t>(stream));
+    cudaError_t e = launch_pnp_batch(a, static_cast<cudaStream_t>(stream));
     return e == cudaSuccess ? PVB_OK : cuda_fail(e, "p3p init kernel");
 }
 

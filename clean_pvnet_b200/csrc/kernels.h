@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "../../include/pvnet_vote_b200.h"
+#include "pnp_core.cuh"
 
 namespace pvb {
 
@@ -79,43 +80,28 @@ cudaError_t launch_covariance(const VoteArgs &a, const float *mean, float *out_c
 // inv(sqrtm(cov)) packed (wxx,wxy,wyy): cov [n][2][2] -> w [n][3]
 cudaError_t launch_pnp_weights(const float *cov, float *w, int n, cudaStream_t st);
 
-// batched uncertainty-PnP refinement (pnp.cu): n problems of pn points, fp64 like the reference
+// batched uncertainty PnP (pnp.cu): n problems of pn points, one warp per problem, fp64 like the reference.  The 2D
+// inputs are either fp64 pts2d + wgt2d, read in place, or (kpt2d != NULL) the voting layer's fp32 keypoints with their
+// covariances or weights, converted into shared memory (pn <= PNP_FUSED_MAX_PN).
+constexpr int PNP_FUSED_MAX_PN = 64;
 struct PnpArgs {
     const double *pts2d;      // [n][pn][2]
-    const double *pts3d;      // [pn][3], problem p at pts3d + p*pts3d_stride (0: shared)
     const double *wgt2d;      // [n][pn][3]  (wxx, wxy, wyy)
-    const double *K;          // [3][3] row-major, problem p at K + p*k_stride (0: shared)
-    const double *init_rt;    // [n][6]
-    double *result_rt;        // [n][6]
-    int *info;                // optional [n][2]: iterations, termination code
-    int n, pn;
-    long long pts3d_stride, k_stride;
-    int max_num_iterations;
-    double function_tolerance, gradient_tolerance, parameter_tolerance;
-};
-cudaError_t launch_pnp(const PnpArgs &a, cudaStream_t st);
-// initial poses by P3P on the 4 best-weighted points (uses pts2d/pts3d/wgt2d/K, writes result_rt)
-cudaError_t launch_p3p_init(const PnpArgs &a, cudaStream_t st);
-
-// the un_pnp tail in one launch (pnp.cu): fp32 keypoints + covariances (or weights) in, refined poses out
-constexpr int PNP_FUSED_MAX_PN = 64;
-struct PnpFusedArgs {
     const float *kpt2d;       // [n][pn][2]  (the voting layer's kpt_2d)
     const float *cov;         // [n][pn][2][2] (the voting layer's var), or NULL ...
     const float *weights;     // ... then [n][pn][3] precomputed (wxx, wxy, wyy)
+    float *weights_out;       // optional [n][pn][3]: the fp32 weights used (kpt2d only)
     const double *pts3d;      // [pn][3], problem p at pts3d + p*pts3d_stride (0: shared)
     const double *K;          // [3][3] row-major, problem p at K + p*k_stride (0: shared)
     const double *init_rt;    // optional [n][6]; NULL: P3P on the four best-weighted points
-    double *result_rt;        // [n][6]
     double *init_out;         // optional [n][6]: the initial pose that was used
-    float *weights_out;       // optional [n][pn][3]
-    int *info;                // optional [n][2]
+    double *result_rt;        // [n][6]: the refined pose; NULL: the P3P start alone (fp64 inputs, into init_out)
+    int *info;                // optional [n][2]: iterations, termination code
     int n, pn;
     long long pts3d_stride, k_stride;
-    int max_num_iterations;
-    double function_tolerance, gradient_tolerance, parameter_tolerance;
+    PnpOptions opt;
 };
-cudaError_t launch_pnp_fused(const PnpFusedArgs &a, cudaStream_t st);
+cudaError_t launch_pnp_batch(const PnpArgs &a, cudaStream_t st);
 
 // twins of the reference extension on its own layouts
 cudaError_t launch_compat_generate(const float *direct, const float *coords, const int32_t *idxs, float *hyp,

@@ -249,4 +249,22 @@ PVB_HD int p3p_solve4(const double X[4][3], const double x2[4][2], const double 
     return found;
 }
 
+// The initial pose of one problem as un_pnp_utils.py:25-31 computes it: p3p_select4 on the weights, p3p_solve4 on those
+// four correspondences.  p2 [pn][2], X [pn][3], w [pn][3]; rt[6] is all NaN when pn < 4 or no pose is admissible (what
+// OpenCV hands the reference then; the refinement stops at once on it).
+PVB_HD void p3p_start(const double *p2, const double *X, const double *w, int pn, const double *cam, double *rt)
+{
+    const double nan = -(double)NAN;                   // bits 0xfff8000000000000, CUDART_NAN
+    for (int i = 0; i < 6; ++i) rt[i] = nan;
+    if (pn < 4) return;
+    int idx[4];
+    p3p_select4(w, pn, idx);
+    double X4[4][3], x4[4][2];
+    for (int r = 0; r < 4; ++r) {
+        for (int c = 0; c < 3; ++c) X4[r][c] = X[3 * idx[r] + c];
+        x4[r][0] = p2[2 * idx[r]]; x4[r][1] = p2[2 * idx[r] + 1];
+    }
+    p3p_solve4(X4, x4, cam, rt);
+}
+
 } // namespace pvb

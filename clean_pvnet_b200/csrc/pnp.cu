@@ -1,4 +1,5 @@
-// pnp.cu -- batched uncertainty-PnP refinement: one warp per pose problem (SURVEY.md 8f row 3).
+// pnp.cu -- the uncertainty-PnP tail on the device (SURVEY.md 8f rows 2+3): per-keypoint weights, P3P initial pose and the
+// batched Levenberg-Marquardt refinement.
 //
 // Replaces the per-image CPU call lib/csrc/uncertainty_pnp/src/uncertainty_pnp.cpp:61-92 (ceres::Solve on 6 parameters and
 // 2*pn residuals, pn = 9..17 keypoints).  A problem is far too small for more than a warp: lane i owns points i, i+32, ...,
@@ -12,6 +13,27 @@
 #include "p3p_core.cuh"
 
 namespace pvb {
+
+// ---------------------------------------------------------------------------------
+// SURVEY 8f row 2: weights of the uncertainty PnP, inv(sqrtm(cov)) per keypoint packed as (wxx, wxy, wyy)
+// (cov_to_weights in common.cuh; pnp_batch_kernel's fp32 inputs use the same function).
+// ---------------------------------------------------------------------------------
+__global__ void __launch_bounds__(128)
+pnp_weights_kernel(const float *__restrict__ cov, float *__restrict__ w, int n)
+{
+    const int i = blockIdx.x * 128 + threadIdx.x;
+    if (i >= n) return;
+    float o0, o1, o2;
+    cov_to_weights(__ldg(reinterpret_cast<const float4 *>(cov) + i), o0, o1, o2);
+    w[(size_t)i * 3] = o0; w[(size_t)i * 3 + 1] = o1; w[(size_t)i * 3 + 2] = o2;
+}
+
+cudaError_t launch_pnp_weights(const float *cov, float *w, int n, cudaStream_t st)
+{
+    if (n <= 0) return cudaSuccess;
+    pnp_weights_kernel<<<(n + 127) / 128, 128, 0, st>>>(cov, w, n);
+    return cudaGetLastError();
+}
 
 // normal equations of one problem at `pose`: lane i owns points i, i+32, ...; butterfly sum -> every lane holds the same bits
 __device__ __forceinline__ void pnp_warp_normal_at(const double *pose, const double *p2, const double *p3, const double *w,
@@ -29,160 +51,99 @@ __device__ __forceinline__ void pnp_warp_normal_at(const double *pose, const dou
     }
 }
 
-__device__ __forceinline__ void pnp_warp_normal(const double *pose, const PnpArgs &a, int prob, int lane, PnpNormal &n)
+// Problem `prob`'s camera (fx, fy, px, py) and model points: one for the batch (stride 0) or one per problem
+__device__ __forceinline__ const double *pnp_model_camera(const PnpArgs &a, int prob, double *cam)
 {
-    const double *K = a.K + (size_t)prob * a.k_stride;
-    const double cam[4] = { K[0], K[4], K[2], K[5] };     // fx, fy, px, py (uncertainty_pnp.cpp:77)
-    pnp_warp_normal_at(pose, a.pts2d + (size_t)prob * a.pn * 2, a.pts3d + (size_t)prob * a.pts3d_stride,
-                       a.wgt2d + (size_t)prob * a.pn * 3, cam, a.pn, lane, n);
-}
-
-__global__ void __launch_bounds__(128)
-pnp_kernel(PnpArgs a)
-{
-    const int lane = threadIdx.x & 31;
-    const int prob = blockIdx.x * 4 + (threadIdx.x >> 5);
-    if (prob >= a.n) return;
-    PnpOptions opt;
-    opt.max_num_iterations = a.max_num_iterations; opt.function_tolerance = a.function_tolerance;
-    opt.gradient_tolerance = a.gradient_tolerance; opt.parameter_tolerance = a.parameter_tolerance;
-    double init[6];
-#pragma unroll
-    for (int i = 0; i < 6; ++i) init[i] = a.init_rt[(size_t)prob * 6 + i];
-    PnpState st;
-    PnpNormal n;
-    pnp_warp_normal(init, a, prob, lane, n);
-    pnp_init(st, init, n);
-    double cand[6];
-    while (pnp_propose(st, opt, cand)) {
-        pnp_warp_normal(cand, a, prob, lane, n);
-        if (!pnp_update(st, opt, cand, n)) break;
-    }
-    if (lane < 6) a.result_rt[(size_t)prob * 6 + lane] = st.x[lane];
-    if (a.info && lane == 0) { a.info[2 * prob] = st.iterations; a.info[2 * prob + 1] = st.code; }
-}
-
-// Initial poses: the reference's recipe (un_pnp_utils.py:25-31) -- the four keypoints with the largest wxx + wxy, ascending;
-// P3P on the first three, the best-weighted one picks the root (p3p_core.cuh).  One thread per problem: the work is a
-// short scalar chain (quartic, <= 4 alignments).  No admissible solution -> NaN pose, which is what OpenCV hands the
-// reference in that case; the refinement then stops at once with that pose.
-__global__ void __launch_bounds__(64)
-p3p_init_kernel(PnpArgs a)
-{
-    const int prob = blockIdx.x * 64 + threadIdx.x;
-    if (prob >= a.n) return;
-    const double *p2 = a.pts2d + (size_t)prob * a.pn * 2;
-    const double *p3 = a.pts3d + (size_t)prob * a.pts3d_stride;
-    const double *w = a.wgt2d + (size_t)prob * a.pn * 3;
-    const double *K = a.K + (size_t)prob * a.k_stride;
-    const double cam[4] = { K[0], K[4], K[2], K[5] };
-    int idx[4];
-    p3p_select4(w, a.pn, idx);
-    double X[4][3], x2[4][2], rt[6];
-    const double nan = CUDART_NAN;
-#pragma unroll
-    for (int i = 0; i < 6; ++i) rt[i] = nan;
-    bool ok = a.pn >= 4;
-    if (ok) {
-        for (int r = 0; r < 4; ++r) {
-            for (int c = 0; c < 3; ++c) X[r][c] = p3[3 * idx[r] + c];
-            x2[r][0] = p2[2 * idx[r]]; x2[r][1] = p2[2 * idx[r] + 1];
-        }
-        p3p_solve4(X, x2, cam, rt);
-    }
-#pragma unroll
-    for (int i = 0; i < 6; ++i) a.result_rt[(size_t)prob * 6 + i] = rt[i];
+    pnp_camera(a.K + (size_t)prob * a.k_stride, cam);
+    return a.pts3d + (size_t)prob * a.pts3d_stride;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// The un_pnp tail in ONE launch (SURVEY 8f rows 2+3 fused): what lib/evaluators/linemod/pvnet.py:118-130 +
-// un_pnp_utils.uncertainty_pnp (:6-57) do per image on the CPU -- weights = inv(sqrtm(cov)) per keypoint, P3P initial pose
-// on the four best-weighted keypoints, Ceres refinement -- straight from the fp32 tensors the voting layer produced
-// (kpt_2d [n,pn,2], var [n,pn,2,2]).  One warp per problem; the problem's data is converted once into shared memory
-// (fp64, weights rounded to fp32 first so the result is bit-identical to pvb_uncertainty_weights -> pvb_uncertainty_pnp_init
-// -> pvb_uncertainty_pnp run one after the other); lane 0 runs the scalar P3P chain, then all lanes run the LM loop.
+// Refinement: one warp per problem, PNP_WARPS problems per CTA.  What lib/evaluators/linemod/pvnet.py:118-130 + un_pnp_utils.
+// uncertainty_pnp (:6-57) do per image on the CPU, in the order they do it:
+//   - the 2D inputs: fp64 points and weights read in place (Fp64), or the voting layer's fp32 kpt_2d with var (or
+//     precomputed weights) converted once into shared memory (Fp32Staged; the weights are rounded to fp32 first, so the
+//     result is bit-identical to pvb_uncertainty_weights followed by the Fp64 path);
+//   - the start: init_rt, or P3P on the four best-weighted points (un_pnp_utils.py:25-31), a short scalar chain run by
+//     lane 0 (p3p_core.cuh); no admissible pose -> NaN, on which the refinement stops at once;
+//   - the refinement.
 // ---------------------------------------------------------------------------------------------------------------------
-constexpr int PNPF_WARPS = 4;
+constexpr int PNP_WARPS = 4;
+enum class PnpInput { Fp64, Fp32Staged };
 
-__global__ void __launch_bounds__(PNPF_WARPS * 32)
-pnp_fused_kernel(PnpFusedArgs a)
+template <PnpInput IN>
+__global__ void __launch_bounds__(PNP_WARPS * 32)
+pnp_batch_kernel(PnpArgs a)
 {
-    __shared__ double s_p2[PNPF_WARPS][PNP_FUSED_MAX_PN * 2], s_p3[PNPF_WARPS][PNP_FUSED_MAX_PN * 3],
-        s_w[PNPF_WARPS][PNP_FUSED_MAX_PN * 3];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const int prob = blockIdx.x * PNPF_WARPS + wid;
+    const int prob = blockIdx.x * PNP_WARPS + wid;
     if (prob >= a.n) return;
-    double *p2 = s_p2[wid], *p3 = s_p3[wid], *w = s_w[wid];
-    const double *K = a.K + (size_t)prob * a.k_stride;
-    const double cam[4] = { K[0], K[4], K[2], K[5] };
-    const double *X = a.pts3d + (size_t)prob * a.pts3d_stride;
-    for (int i = lane; i < a.pn; i += 32) {
-        const float2 q = __ldg(reinterpret_cast<const float2 *>(a.kpt2d) + (size_t)prob * a.pn + i);
-        p2[2 * i] = (double)q.x; p2[2 * i + 1] = (double)q.y;
-        float w0, w1, w2;
-        if (a.cov) cov_to_weights(__ldg(reinterpret_cast<const float4 *>(a.cov) + (size_t)prob * a.pn + i), w0, w1, w2);
-        else { const float *ww = a.weights + ((size_t)prob * a.pn + i) * 3; w0 = ww[0]; w1 = ww[1]; w2 = ww[2]; }
-        w[3 * i] = (double)w0; w[3 * i + 1] = (double)w1; w[3 * i + 2] = (double)w2;
-        if (a.weights_out) { float *wo = a.weights_out + ((size_t)prob * a.pn + i) * 3; wo[0] = w0; wo[1] = w1; wo[2] = w2; }
-        p3[3 * i] = X[3 * i]; p3[3 * i + 1] = X[3 * i + 1]; p3[3 * i + 2] = X[3 * i + 2];
+    double cam[4];
+    const double *p3 = pnp_model_camera(a, prob, cam), *p2, *w;
+    if constexpr (IN == PnpInput::Fp32Staged) {
+        __shared__ double s_p2[PNP_WARPS][PNP_FUSED_MAX_PN * 2], s_p3[PNP_WARPS][PNP_FUSED_MAX_PN * 3],
+            s_w[PNP_WARPS][PNP_FUSED_MAX_PN * 3];
+        double *d2 = s_p2[wid], *d3 = s_p3[wid], *dw = s_w[wid];
+        for (int i = lane; i < a.pn; i += 32) {
+            const float2 q = __ldg(reinterpret_cast<const float2 *>(a.kpt2d) + (size_t)prob * a.pn + i);
+            d2[2 * i] = (double)q.x; d2[2 * i + 1] = (double)q.y;
+            float w0, w1, w2;
+            if (a.cov) cov_to_weights(__ldg(reinterpret_cast<const float4 *>(a.cov) + (size_t)prob * a.pn + i), w0, w1, w2);
+            else { const float *ww = a.weights + ((size_t)prob * a.pn + i) * 3; w0 = ww[0]; w1 = ww[1]; w2 = ww[2]; }
+            dw[3 * i] = (double)w0; dw[3 * i + 1] = (double)w1; dw[3 * i + 2] = (double)w2;
+            if (a.weights_out) { float *wo = a.weights_out + ((size_t)prob * a.pn + i) * 3; wo[0] = w0; wo[1] = w1; wo[2] = w2; }
+            d3[3 * i] = p3[3 * i]; d3[3 * i + 1] = p3[3 * i + 1]; d3[3 * i + 2] = p3[3 * i + 2];
+        }
+        __syncwarp();
+        p2 = d2; p3 = d3; w = dw;
+    } else {
+        p2 = a.pts2d + (size_t)prob * a.pn * 2;
+        w = a.wgt2d + (size_t)prob * a.pn * 3;
     }
-    __syncwarp();
     double init[6];
     if (a.init_rt) {
 #pragma unroll
         for (int i = 0; i < 6; ++i) init[i] = a.init_rt[(size_t)prob * 6 + i];
     } else {
-        const double nan = CUDART_NAN;
 #pragma unroll
-        for (int i = 0; i < 6; ++i) init[i] = nan;
-        if (lane == 0 && a.pn >= 4) {
-            int idx[4];
-            p3p_select4(w, a.pn, idx);
-            double X4[4][3], x4[4][2];
-            for (int r = 0; r < 4; ++r) {
-                for (int c = 0; c < 3; ++c) X4[r][c] = p3[3 * idx[r] + c];
-                x4[r][0] = p2[2 * idx[r]]; x4[r][1] = p2[2 * idx[r] + 1];
-            }
-            p3p_solve4(X4, x4, cam, init);
-        }
+        for (int i = 0; i < 6; ++i) init[i] = CUDART_NAN;
+        if (lane == 0) p3p_start(p2, p3, w, a.pn, cam, init);
 #pragma unroll
         for (int i = 0; i < 6; ++i) init[i] = __shfl_sync(0xffffffffu, init[i], 0);
     }
     if (a.init_out && lane < 6) a.init_out[(size_t)prob * 6 + lane] = init[lane];
-    PnpOptions opt;
-    opt.max_num_iterations = a.max_num_iterations; opt.function_tolerance = a.function_tolerance;
-    opt.gradient_tolerance = a.gradient_tolerance; opt.parameter_tolerance = a.parameter_tolerance;
     PnpState st;
-    PnpNormal n;
-    pnp_warp_normal_at(init, p2, p3, w, cam, a.pn, lane, n);
-    pnp_init(st, init, n);
-    double cand[6];
-    while (pnp_propose(st, opt, cand)) {
-        pnp_warp_normal_at(cand, p2, p3, w, cam, a.pn, lane, n);
-        if (!pnp_update(st, opt, cand, n)) break;
-    }
+    pnp_solve(a.opt, init, [&](const double *pose, PnpNormal &n) { pnp_warp_normal_at(pose, p2, p3, w, cam, a.pn, lane, n); },
+              st);
     if (lane < 6) a.result_rt[(size_t)prob * 6 + lane] = st.x[lane];
     if (a.info && lane == 0) { a.info[2 * prob] = st.iterations; a.info[2 * prob + 1] = st.code; }
 }
 
-cudaError_t launch_pnp_fused(const PnpFusedArgs &a, cudaStream_t st)
+// The P3P start alone (pvb_uncertainty_pnp_init), one thread per problem.  The chain is scalar, so a warp per problem would
+// leave 31 lanes idle, and without the LM code the kernel needs about 156 registers instead of 254: a batch of 4096
+// problems runs in one wave here, in about four as the start of pnp_batch_kernel<Fp64>.
+__global__ void __launch_bounds__(64)
+p3p_start_kernel(PnpArgs a)
 {
-    if (a.n <= 0) return cudaSuccess;
-    pnp_fused_kernel<<<(a.n + PNPF_WARPS - 1) / PNPF_WARPS, PNPF_WARPS * 32, 0, st>>>(a);
-    return cudaGetLastError();
+    const int prob = blockIdx.x * 64 + threadIdx.x;
+    if (prob >= a.n) return;
+    double cam[4], rt[6];
+    const double *p3 = pnp_model_camera(a, prob, cam);
+    p3p_start(a.pts2d + (size_t)prob * a.pn * 2, p3, a.wgt2d + (size_t)prob * a.pn * 3, a.pn, cam, rt);
+#pragma unroll
+    for (int i = 0; i < 6; ++i) a.init_out[(size_t)prob * 6 + i] = rt[i];
 }
 
-cudaError_t launch_p3p_init(const PnpArgs &a, cudaStream_t st)
+cudaError_t launch_pnp_batch(const PnpArgs &a, cudaStream_t st)
 {
     if (a.n <= 0) return cudaSuccess;
-    p3p_init_kernel<<<(a.n + 63) / 64, 64, 0, st>>>(a);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_pnp(const PnpArgs &a, cudaStream_t st)
-{
-    if (a.n <= 0) return cudaSuccess;
-    pnp_kernel<<<(a.n + 3) / 4, 128, 0, st>>>(a);
+    if (!a.result_rt) {
+        p3p_start_kernel<<<(a.n + 63) / 64, 64, 0, st>>>(a);
+        return cudaGetLastError();
+    }
+    const int blocks = (a.n + PNP_WARPS - 1) / PNP_WARPS;
+    if (a.kpt2d) pnp_batch_kernel<PnpInput::Fp32Staged><<<blocks, PNP_WARPS * 32, 0, st>>>(a);
+    else pnp_batch_kernel<PnpInput::Fp64><<<blocks, PNP_WARPS * 32, 0, st>>>(a);
     return cudaGetLastError();
 }
 

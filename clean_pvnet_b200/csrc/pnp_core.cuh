@@ -33,6 +33,12 @@ PVB_HD PnpOptions pnp_default_options()
     return o;
 }
 
+// cam = (fx, fy, px, py) of a row-major 3x3 intrinsic matrix (uncertainty_pnp.cpp:77)
+PVB_HD void pnp_camera(const double *K, double *cam)
+{
+    cam[0] = K[0]; cam[1] = K[4]; cam[2] = K[2]; cam[3] = K[5];
+}
+
 // termination codes written to `info` (documented in include/pvnet_vote_b200.h)
 enum { PNP_CONV_GRADIENT = 1, PNP_CONV_PARAMETER = 2, PNP_CONV_FUNCTION = 3, PNP_CONV_RADIUS = 4, PNP_NO_CONVERGENCE = 5,
        PNP_FAILURE = 6 };
@@ -111,10 +117,7 @@ PVB_HD void pnp_accumulate_point(const double *pose, const double *X, const doub
     n.cost += 0.5 * (r0 * r0 + r1 * r1);
 }
 
-// Trust-region state of one problem.  The caller drives it:
-//     pnp_init(st, init_rt, normal(init_rt));
-//     while (pnp_propose(st, opt, cand))  pnp_update(st, opt, cand, normal(cand));
-//     result = st.x, st.code, st.iterations
+// Trust-region state of one problem, driven by pnp_solve; result = st.x, st.code, st.iterations
 struct PnpState {
     double x[6], x_norm, grad_max;
     PnpNormal n;                 // normal equations at x
@@ -254,6 +257,24 @@ PVB_HD bool pnp_update(PnpState &st, const PnpOptions &opt, const double *cand, 
         st.reuse_diagonal = 1;
     }
     return true;
+}
+
+// The whole solve from init_rt.  eval(pose, n) fills n with the normal equations at pose: a warp reduction in the kernel
+// (pnp.cu), a serial sum in the host build (tests/pnp_host_harness.cpp).
+#if defined(__CUDACC__)
+#pragma nv_exec_check_disable
+#endif
+template <class Eval>
+PVB_HD void pnp_solve(const PnpOptions &opt, const double *init_rt, Eval &&eval, PnpState &st)
+{
+    PnpNormal n;
+    eval(init_rt, n);
+    pnp_init(st, init_rt, n);
+    double cand[6];
+    while (pnp_propose(st, opt, cand)) {
+        eval(cand, n);
+        if (!pnp_update(st, opt, cand, n)) break;
+    }
 }
 
 } // namespace pvb

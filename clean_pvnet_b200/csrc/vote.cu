@@ -544,25 +544,4 @@ cudaError_t launch_covariance(const VoteArgs &a, const float *mean, float *out_c
     return cudaGetLastError();
 }
 
-// ---------------------------------------------------------------------------------
-// SURVEY 8f row 2: weights of the uncertainty PnP, inv(sqrtm(cov)) per keypoint packed as (wxx, wxy, wyy)
-// (cov_to_weights in common.cuh; the fused un_pnp tail in pnp.cu uses the same function).
-// ---------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128)
-pnp_weights_kernel(const float *__restrict__ cov, float *__restrict__ w, int n)
-{
-    const int i = blockIdx.x * 128 + threadIdx.x;
-    if (i >= n) return;
-    float o0, o1, o2;
-    cov_to_weights(__ldg(reinterpret_cast<const float4 *>(cov) + i), o0, o1, o2);
-    w[(size_t)i * 3] = o0; w[(size_t)i * 3 + 1] = o1; w[(size_t)i * 3 + 2] = o2;
-}
-
-cudaError_t launch_pnp_weights(const float *cov, float *w, int n, cudaStream_t st)
-{
-    if (n <= 0) return cudaSuccess;
-    pnp_weights_kernel<<<(n + 127) / 128, 128, 0, st>>>(cov, w, n);
-    return cudaGetLastError();
-}
-
 } // namespace pvb

@@ -27,7 +27,32 @@ def _options(max_num_iterations, function_tolerance, gradient_tolerance, paramet
     o.max_num_iterations, o.reserved = int(max_num_iterations), 0
     o.function_tolerance, o.gradient_tolerance = float(function_tolerance), float(gradient_tolerance)
     o.parameter_tolerance = float(parameter_tolerance)
-    return o
+    return ctypes.cast(ctypes.pointer(o), ctypes.c_void_p)
+
+
+def _batch(points_2d, name):
+    """The first check of the three batched entries: `points_2d` must be a CUDA tensor [n,pn,2].  Returns (device, n, pn)."""
+    if not (isinstance(points_2d, torch.Tensor) and points_2d.is_cuda):
+        raise RuntimeError(f"{name} must be a CUDA tensor")
+    if points_2d.dim() != 3 or points_2d.shape[-1] != 2:
+        raise RuntimeError(f"{name} must be [n,pn,2]")
+    return points_2d.device, int(points_2d.shape[0]), int(points_2d.shape[1])
+
+
+def _model_camera(points_3d, camera_matrix, dev, pn):
+    """The model points ([pn,3] for the whole batch, or [n,pn,3]) and the camera ([3,3] or [n,3,3]), already checked by
+    the entry, as float64 on `dev`, with the strides the C entries take (0: shared)."""
+    p3 = points_3d.to(device=dev, dtype=torch.float64).contiguous()
+    km = camera_matrix.to(device=dev, dtype=torch.float64).contiguous()
+    return p3, km, 0 if p3.dim() == 2 else pn * 3, 0 if km.dim() == 2 else 9
+
+
+def _call(entry, dev, *args):
+    """lib.<entry>(*args, stream) on the current stream of `dev`; tensors go in as their device pointers, None as NULL."""
+    lib = _lib.load()
+    args = [ctypes.c_void_p(a.data_ptr()) if isinstance(a, torch.Tensor) else a for a in args]
+    with torch.cuda.device(dev):
+        _lib.check(getattr(lib, entry)(*args, ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
 
 
 def uncertainty_pnp_batch(points_2d, weights_2d, points_3d, camera_matrix, init_rt=None, *, max_num_iterations=50,
@@ -36,41 +61,32 @@ def uncertainty_pnp_batch(points_2d, weights_2d, points_3d, camera_matrix, init_
     init_rt [n,6] (angle-axis, translation): CUDA tensors of any float dtype.  Returns result_rt [n,6] float64 on the same
     device (and info [n,2] int32 = iterations, termination code when return_info).  Stream-ordered, no host sync.
     init_rt=None: the initial poses come from `p3p_init_batch` (the reference's P3P recipe, on the device)."""
-    if not (isinstance(points_2d, torch.Tensor) and points_2d.is_cuda):
-        raise RuntimeError("points_2d must be a CUDA tensor")
-    dev = points_2d.device
-    if points_2d.dim() != 3 or points_2d.shape[-1] != 2:
-        raise RuntimeError("points_2d must be [n,pn,2]")
-    n, pn = int(points_2d.shape[0]), int(points_2d.shape[1])
+    dev, n, pn = _batch(points_2d, "points_2d")
     if pn < 1:
         raise RuntimeError("need at least one point per problem")
 
-    def prep(t, shape, name):
+    def check(t, shape, name):
         if not (isinstance(t, torch.Tensor) and t.device == dev):
             raise RuntimeError(f"{name} must be a CUDA tensor on {dev}")
         if tuple(t.shape) != shape:
             raise RuntimeError(f"{name} must have shape {list(shape)}, got {list(t.shape)}")
-        return t.to(torch.float64).contiguous()
 
-    p2 = prep(points_2d, (n, pn, 2), "points_2d")
-    w2 = prep(weights_2d, (n, pn, 3), "weights_2d")
-    shared3 = points_3d.dim() == 2
-    p3 = prep(points_3d, (pn, 3) if shared3 else (n, pn, 3), "points_3d")
-    sharedk = camera_matrix.dim() == 2
-    km = prep(camera_matrix, (3, 3) if sharedk else (n, 3, 3), "camera_matrix")
-    rt0 = prep(init_rt, (n, 6), "init_rt") if init_rt is not None else _p3p_init_prepared(p2, p3, w2, km, shared3, sharedk)
+    f64 = lambda t: t.to(torch.float64).contiguous()   # noqa: E731
+    check(points_2d, (n, pn, 2), "points_2d")
+    check(weights_2d, (n, pn, 3), "weights_2d")
+    shared = lambda t: isinstance(t, torch.Tensor) and t.dim() == 2   # noqa: E731
+    check(points_3d, (pn, 3) if shared(points_3d) else (n, pn, 3), "points_3d")
+    check(camera_matrix, (3, 3) if shared(camera_matrix) else (n, 3, 3), "camera_matrix")
+    if init_rt is not None:
+        check(init_rt, (n, 6), "init_rt")
+    p2, w2 = f64(points_2d), f64(weights_2d)
+    p3, km, s3, sk = _model_camera(points_3d, camera_matrix, dev, pn)
+    rt0 = f64(init_rt) if init_rt is not None else p3p_init_batch(p2, w2, p3, km)
     out = torch.empty((n, 6), dtype=torch.float64, device=dev)
     info = torch.zeros((n, 2), dtype=torch.int32, device=dev) if return_info else None
     if n:
-        lib = _lib.load()
-        opt = _options(max_num_iterations, function_tolerance, gradient_tolerance, parameter_tolerance)
-        vp = ctypes.c_void_p
-        with torch.cuda.device(dev):
-            _lib.check(lib.pvb_uncertainty_pnp(
-                vp(p2.data_ptr()), vp(p3.data_ptr()), vp(w2.data_ptr()), vp(km.data_ptr()), vp(rt0.data_ptr()),
-                vp(out.data_ptr()), vp(info.data_ptr()) if info is not None else None, n, pn,
-                0 if shared3 else pn * 3, 0 if sharedk else 9, ctypes.cast(ctypes.pointer(opt), vp),
-                vp(torch.cuda.current_stream(dev).cuda_stream)))
+        _call("pvb_uncertainty_pnp", dev, p2, p3, w2, km, rt0, out, info, n, pn, s3, sk,
+              _options(max_num_iterations, function_tolerance, gradient_tolerance, parameter_tolerance))
     return (out, info) if return_info else out
 
 
@@ -89,12 +105,7 @@ def uncertainty_pnp_from_votes(kpt_2d, var, points_3d, camera_matrix, init_rt=No
     `weights` [n,pn,3] float32 instead of `var` (var=None) if they already exist.  Bit-identical to
     uncertainty_pnp_weights -> p3p_init_batch -> uncertainty_pnp_batch.  No host sync.
     return_info: also info [n,2] int32 (iterations, termination code); return_aux: also (init_rt used, weights)."""
-    if not (isinstance(kpt_2d, torch.Tensor) and kpt_2d.is_cuda):
-        raise RuntimeError("kpt_2d must be a CUDA tensor")
-    dev = kpt_2d.device
-    if kpt_2d.dim() != 3 or kpt_2d.shape[-1] != 2:
-        raise RuntimeError("kpt_2d must be [n,pn,2]")
-    n, pn = int(kpt_2d.shape[0]), int(kpt_2d.shape[1])
+    dev, n, pn = _batch(kpt_2d, "kpt_2d")
     if (var is None) == (weights is None):
         raise RuntimeError("pass exactly one of var / weights")
     k2 = kpt_2d.float().contiguous()
@@ -107,11 +118,9 @@ def uncertainty_pnp_from_votes(kpt_2d, var, points_3d, camera_matrix, init_rt=No
         if tuple(weights.shape) != (n, pn, 3) or weights.device != dev:
             raise RuntimeError(f"weights must be a CUDA tensor [{n},{pn},3] on {dev}")
         wt = weights.float().contiguous()
-    shared3, sharedk = points_3d.dim() == 2, camera_matrix.dim() == 2
     if tuple(points_3d.shape[-2:]) != (pn, 3) or tuple(camera_matrix.shape[-2:]) != (3, 3):
         raise RuntimeError("points_3d must be [pn,3] | [n,pn,3] and camera_matrix [3,3] | [n,3,3]")
-    p3 = points_3d.to(device=dev, dtype=torch.float64).contiguous()
-    km = camera_matrix.to(device=dev, dtype=torch.float64).contiguous()
+    p3, km, s3, sk = _model_camera(points_3d, camera_matrix, dev, pn)
     rt0 = None
     if init_rt is not None:
         if tuple(init_rt.shape) != (n, 6):
@@ -122,15 +131,8 @@ def uncertainty_pnp_from_votes(kpt_2d, var, points_3d, camera_matrix, init_rt=No
     init_out = torch.empty((n, 6), dtype=torch.float64, device=dev) if return_aux else None
     w_out = torch.empty((n, pn, 3), dtype=torch.float32, device=dev) if return_aux else None
     if n:
-        lib = _lib.load()
-        opt = _options(max_num_iterations, function_tolerance, gradient_tolerance, parameter_tolerance)
-        vp = ctypes.c_void_p
-        ptr = lambda t: vp(t.data_ptr()) if t is not None else None   # noqa: E731
-        with torch.cuda.device(dev):
-            _lib.check(lib.pvb_uncertainty_pnp_from_votes(
-                ptr(k2), ptr(cv), ptr(wt), ptr(p3), ptr(km), ptr(rt0), ptr(out), ptr(init_out), ptr(w_out), ptr(info), n, pn,
-                0 if shared3 else pn * 3, 0 if sharedk else 9, ctypes.cast(ctypes.pointer(opt), vp),
-                vp(torch.cuda.current_stream(dev).cuda_stream)))
+        _call("pvb_uncertainty_pnp_from_votes", dev, k2, cv, wt, p3, km, rt0, out, init_out, w_out, info, n, pn, s3, sk,
+              _options(max_num_iterations, function_tolerance, gradient_tolerance, parameter_tolerance))
     res = (out,)
     if return_info:
         res += (info,)
@@ -139,34 +141,22 @@ def uncertainty_pnp_from_votes(kpt_2d, var, points_3d, camera_matrix, init_rt=No
     return res if len(res) > 1 else out
 
 
-def _p3p_init_prepared(p2, p3, w2, km, shared3, sharedk):
-    n, pn = int(p2.shape[0]), int(p2.shape[1])
-    if pn < 4:
-        raise RuntimeError("the P3P initialisation needs at least 4 points per problem")
-    out = torch.empty((n, 6), dtype=torch.float64, device=p2.device)
-    if n:
-        lib = _lib.load()
-        vp = ctypes.c_void_p
-        with torch.cuda.device(p2.device):
-            _lib.check(lib.pvb_uncertainty_pnp_init(
-                vp(p2.data_ptr()), vp(p3.data_ptr()), vp(w2.data_ptr()), vp(km.data_ptr()), vp(out.data_ptr()), n, pn,
-                0 if shared3 else pn * 3, 0 if sharedk else 9, vp(torch.cuda.current_stream(p2.device).cuda_stream)))
-    return out
-
-
 def p3p_init_batch(points_2d, weights_2d, points_3d, camera_matrix):
     """Initial poses [n,6] as un_pnp_utils.py:25-31 computes them with OpenCV (P3P on the 2nd..4th best-weighted keypoints by
     wxx+wxy, the best one picks the root), on the device and for the whole batch; NaN rows where no pose is admissible.
     Pinned against cv2.solvePnP on the CPU (tests/test_p3p_host_core.py) and on the GPU (tests/test_gpu_zz_p3p.py)."""
-    if not (isinstance(points_2d, torch.Tensor) and points_2d.is_cuda):
-        raise RuntimeError("points_2d must be a CUDA tensor")
-    dev = points_2d.device
-    n, pn = int(points_2d.shape[0]), int(points_2d.shape[1])
-    f = lambda t: t.to(device=dev, dtype=torch.float64).contiguous()   # noqa: E731
-    shared3, sharedk = points_3d.dim() == 2, camera_matrix.dim() == 2
+    dev, n, pn = _batch(points_2d, "points_2d")
     if tuple(weights_2d.shape) != (n, pn, 3) or tuple(points_3d.shape[-2:]) != (pn, 3) or tuple(camera_matrix.shape[-2:]) != (3, 3):
         raise RuntimeError("shapes: points_2d [n,pn,2], weights_2d [n,pn,3], points_3d [pn,3]|[n,pn,3], camera_matrix [3,3]|[n,3,3]")
-    return _p3p_init_prepared(f(points_2d), f(points_3d), f(weights_2d), f(camera_matrix), shared3, sharedk)
+    if pn < 4:
+        raise RuntimeError("the P3P initialisation needs at least 4 points per problem")
+    p3, km, s3, sk = _model_camera(points_3d, camera_matrix, dev, pn)
+    p2 = points_2d.to(torch.float64).contiguous()
+    w2 = weights_2d.to(device=dev, dtype=torch.float64).contiguous()
+    out = torch.empty((n, 6), dtype=torch.float64, device=dev)
+    if n:
+        _call("pvb_uncertainty_pnp_init", dev, p2, p3, w2, km, out, n, pn, s3, sk)
+    return out
 
 
 def rodrigues(rt):

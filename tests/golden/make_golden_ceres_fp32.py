@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Generates tests/golden/ceres_pnp_fp32.npz: uncertainty-PnP problems whose inputs are exactly what the fused un_pnp tail
-(`uncertainty_pnp_from_votes`, csrc/pnp.cu pnp_fused_kernel) sees -- fp32 keypoints, fp32 covariances and the fp32 weights
+(`uncertainty_pnp_from_votes`, csrc/pnp.cu pnp_batch_kernel<Fp32Staged>) sees -- fp32 keypoints, fp32 covariances and the fp32 weights
 cov_to_weights derives from them, float64 model points and intrinsics -- solved by REAL Ceres 2.0 (the reference's prebuilt
 libceres + its unmodified uncertainty_pnp.cpp, built by oracle/build_ceres_ref.py) and started from OpenCV's P3P pose as
 un_pnp_utils.py:25-31 computes it.  CPU only; needs /root/reference:

@@ -1,6 +1,6 @@
 // Host build of clean_pvnet_b200/csrc/pnp_core.cuh for the CPU test-suite (tests/test_pnp_host_core.py): the same
-// arithmetic and trust-region state machine the CUDA kernel runs, driven by a serial loop over the points instead of the
-// warp reduction.  Test infrastructure only -- nothing in the product links or loads this.
+// arithmetic and the same pnp_solve loop the CUDA kernel runs, with a serial sum over the points as its evaluation instead
+// of the warp reduction.  Test infrastructure only -- nothing in the product links or loads this.
 #include "../clean_pvnet_b200/csrc/pnp_core.cuh"
 
 static void normal_at(const double *pose, const double *pts2d, const double *pts3d, const double *wgt2d, const double *cam,
@@ -14,19 +14,14 @@ extern "C" int pnp_host_solve(const double *pts2d, const double *pts3d, const do
                               const double *init_rt, double *result_rt, int *info, int pn, int max_num_iterations,
                               double function_tolerance, double gradient_tolerance, double parameter_tolerance)
 {
-    const double cam[4] = { K[0], K[4], K[2], K[5] };     // uncertainty_pnp.cpp:77
+    double cam[4];
+    pvb::pnp_camera(K, cam);
     pvb::PnpOptions opt;
     opt.max_num_iterations = max_num_iterations; opt.function_tolerance = function_tolerance;
     opt.gradient_tolerance = gradient_tolerance; opt.parameter_tolerance = parameter_tolerance;
     pvb::PnpState st;
-    pvb::PnpNormal n;
-    normal_at(init_rt, pts2d, pts3d, wgt2d, cam, pn, n);
-    pvb::pnp_init(st, init_rt, n);
-    double cand[6];
-    while (pvb::pnp_propose(st, opt, cand)) {
-        normal_at(cand, pts2d, pts3d, wgt2d, cam, pn, n);
-        if (!pvb::pnp_update(st, opt, cand, n)) break;
-    }
+    pvb::pnp_solve(opt, init_rt, [&](const double *pose, pvb::PnpNormal &n) { normal_at(pose, pts2d, pts3d, wgt2d, cam, pn, n); },
+                   st);
     for (int i = 0; i < 6; ++i) result_rt[i] = st.x[i];
     if (info) { info[0] = st.iterations; info[1] = st.code; }
     return 0;
@@ -35,7 +30,8 @@ extern "C" int pnp_host_solve(const double *pts2d, const double *pts3d, const do
 extern "C" void pnp_host_normal(const double *pose, const double *pts2d, const double *pts3d, const double *wgt2d,
                                 const double *K, int pn, double *H21, double *g6, double *cost)
 {
-    const double cam[4] = { K[0], K[4], K[2], K[5] };
+    double cam[4];
+    pvb::pnp_camera(K, cam);
     pvb::PnpNormal n;
     normal_at(pose, pts2d, pts3d, wgt2d, cam, pn, n);
     for (int i = 0; i < 21; ++i) H21[i] = n.H[i];

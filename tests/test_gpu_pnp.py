@@ -143,6 +143,11 @@ def test_input_checks(pvb):
     with pytest.raises(RuntimeError):
         pvb.uncertainty_pnp_batch(uv, torch.zeros((2, 9, 2), device="cuda"), torch.zeros((9, 3), device="cuda"),
                                   torch.zeros((3, 3), device="cuda"), torch.zeros((2, 6), device="cuda"))
+    w = torch.zeros((2, 9, 3), device="cuda")
+    for model, cam, name in ((np.zeros((9, 3)), torch.eye(3, device="cuda"), "points_3d"),
+                             (torch.zeros((9, 3), device="cuda"), np.eye(3), "camera_matrix")):
+        with pytest.raises(RuntimeError, match=f"{name} must be a CUDA tensor"):
+            pvb.uncertainty_pnp_batch(uv, w, model, cam, torch.zeros((2, 6), device="cuda"))
 
 
 def test_kernel_follows_real_ceres(pvb):

@@ -1,6 +1,6 @@
-"""GPU: the fused un_pnp tail (`uncertainty_pnp_from_votes`, csrc/pnp.cu pnp_fused_kernel) and the batched refinement
-(`uncertainty_pnp_batch`, pnp_kernel) against real Ceres and OpenCV, through tests/golden/ceres_pnp_fp32.npz
-(tests/golden/make_golden_ceres_fp32.py; the CPU side, tests/test_ceres_golden.py and tests/test_p3p_host_core.py, checks
+"""GPU: the fused un_pnp tail (`uncertainty_pnp_from_votes`, the fp32 instantiation of csrc/pnp.cu pnp_batch_kernel) and
+the batched refinement (`uncertainty_pnp_batch`, its fp64 instantiation) against real Ceres and OpenCV, through
+tests/golden/ceres_pnp_fp32.npz (tests/golden/make_golden_ceres_fp32.py; the CPU side, tests/test_ceres_golden.py and tests/test_p3p_host_core.py, checks
 that the oracle and the host builds of pnp_core.cuh / p3p_core.cuh follow the same fixture).
 
 The fixture's inputs are fp32 keypoints, fp32 covariances and the fp32 weights cov_to_weights makes of them -- exactly what
@@ -78,7 +78,7 @@ def bits(x):
 @pytest.mark.parametrize("start", ["", "p3ps_"])
 def test_fused_kernel_follows_ceres(pvb, start):
     """The fused entry with `weights` and an explicit start (the perturbed truth, or OpenCV's P3P pose on the stable top
-    four) against Ceres from the same start, every set; pnp_kernel on the same data gives identical bits; the problem's
+    four) against Ceres from the same start, every set; the fp64 instantiation on the same data gives identical bits; the problem's
     place in the batch (n = 1, 3, 5, 130, partly filled CTAs) changes nothing."""
     tally = Tally()
     init_all = F["init_rt"] if start == "" else F["p3ps_rt"]
@@ -91,7 +91,7 @@ def test_fused_kernel_follows_ceres(pvb, start):
         rt_np, info_np = rt.cpu().numpy(), info.cpu().numpy()
         for j, i in enumerate(idx):
             tally.check(i, start, rt_np[j], info_np[j], (kind, pn))
-        # pnp_kernel (double inputs, the same values) must give the same bits, incl. pn > 32
+        # the fp64 instantiation (double inputs, the same values) must give the same bits, incl. pn > 32
         rt2, info2 = pvb.uncertainty_pnp_batch(kpt.double(), w.double(), model, cam, init, return_info=True)
         assert torch.equal(bits(rt2), bits(rt)) and torch.equal(info2, info), (kind, pn)
         # partly filled CTAs and many problems per launch: each row is the same as in the whole-set batch

@@ -1,4 +1,5 @@
-"""GPU: the device launch of the P3P initialisation (pvb_uncertainty_pnp_init, csrc/pnp.cu p3p_init_kernel).
+"""GPU: the device launch of the P3P initialisation (pvb_uncertainty_pnp_init, csrc/pnp.cu p3p_start_kernel:
+p3p_start, one thread per problem).
 
 Its arithmetic (csrc/p3p_core.cuh) is pinned against cv2.solvePnP on the CPU by tests/test_p3p_host_core.py; what is checked
 here is the launch, the point selection on the device and the memory layout (first GPU run: the round-1 driver, passed)."""

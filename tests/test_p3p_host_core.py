@@ -41,8 +41,16 @@ def p3p():
         lib.p3p_host_select4(w.ctypes.data_as(DP), ctypes.c_int(len(w)), idx)
         return list(idx)
 
+    def start(x2, X, w, K):
+        x2, X, w, K = [np.ascontiguousarray(a, np.float64) for a in (x2, X, w, K)]
+        rt = np.zeros(6)
+        lib.p3p_host_start(x2.ctypes.data_as(DP), X.ctypes.data_as(DP), w.ctypes.data_as(DP), ctypes.c_int(len(w)),
+                           K.ctypes.data_as(DP), rt.ctypes.data_as(DP))
+        return rt
+
     solve.quartic = quartic
     solve.select4 = select4
+    solve.start = start
     return solve
 
 
@@ -163,18 +171,22 @@ def test_fp32_fixture_p3p_matches_stored_opencv(p3p):
     """tests/golden/ceres_pnp_fp32.npz stores OpenCV's P3P pose on the stable top four (`p3ps_rt`) of every problem with
     pn >= 4: p3p_select4 picks those four, and p3p_solve4 gives OpenCV's pose to 1e-6 unless the fourth point cannot tell
     the candidates apart (the allowance of test_selected_pose_matches_opencv_p3p); where OpenCV has no finite pose (the
-    skipped images: four coincident image points) it reports no solution."""
+    skipped images: four coincident image points) it reports no solution.  p3p_start, the composition the kernel runs
+    (select, gather, solve, NaN without a pose), gives the same bits from the whole problem, and all NaN at pn < 4."""
     F = _fp32_fixture()
     ties = checked = 0
     for i in range(len(F["pn"])):
         pn = int(F["pn"][i])
-        if pn < 4:
-            continue
         w = F["wgt2d"][i, :pn].astype(np.float64)
+        start = p3p.start(F["kpt2d"][i, :pn], F["pts3d"][i, :pn], w, F["K"][i])
+        if pn < 4:
+            assert np.isnan(start).all(), i
+            continue
         idx = p3p.select4(w)
         assert idx == F["idx_stable"][i].tolist(), i
         uv, X, K = F["kpt2d"][i, :pn].astype(np.float64)[idx], F["pts3d"][i, :pn][idx], F["K"][i]
         n, rt = p3p(X, uv, K)
+        assert np.array_equal(start, rt, equal_nan=True), i
         want = F["p3ps_rt"][i]
         if not np.isfinite(want).all():
             assert n == 0 and np.isnan(rt).all(), i

@@ -1,6 +1,8 @@
 #!/usr/bin/env python
-"""Times pvb_uncertainty_pnp (batched LM refinement, one warp per problem) for a few batch sizes, next to the same
-arithmetic core compiled for the host (tests/pnp_host_harness.cpp, one core) on the same problems."""
+"""Times the three batched uncertainty-PnP entries for a few batch sizes (one warp per problem): uncertainty_pnp_batch
+(fp64 inputs, LM refinement from a given start), p3p_init_batch (the P3P start alone) and uncertainty_pnp_from_votes (fp32
+keypoints and weights, LM refinement from the same start), next to the same arithmetic core compiled for the host
+(tests/pnp_host_harness.cpp, one core) on the same problems."""
 import ctypes
 import os
 import subprocess
@@ -30,20 +32,29 @@ for c in cases:
                        ctypes.c_double(1e-6), ctypes.c_double(1e-10), ctypes.c_double(1e-8))
 cpu_us = (time.perf_counter() - t0) / len(cases) * 1e6
 print(f"host build of the same core, 1 core: {cpu_us:.1f} us per problem (incl. ctypes call)")
-for n in (1, 16, 256, 4096):
-    reps = [cases[i % 256] for i in range(n)]
-    f = lambda i: torch.from_numpy(np.stack([c[i] for c in reps])).cuda()  # noqa: E731
-    uv, p3, W, K, init = f(0), torch.from_numpy(cases[0][1]).cuda(), f(2), torch.from_numpy(cases[0][3]).cuda(), f(4)
-    p3 = f(1)
-    K = f(3)
+
+
+def per_call_us(fn, reps=20):
     for _ in range(3):
-        rt, inf = pvb.uncertainty_pnp_batch(uv, W, p3, K, init, return_info=True)
+        fn()
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
-    for _ in range(20):
-        rt = pvb.uncertainty_pnp_batch(uv, W, p3, K, init)
+    for _ in range(reps):
+        fn()
     e1.record()
     torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / 20
-    print(f"n={n:5d}: {ms*1e3:8.1f} us per call  {ms*1e3/n:8.2f} us per problem  mean iterations {inf[:,0].float().mean().item():.2f}")
+    return e0.elapsed_time(e1) / reps * 1e3
+
+
+for n in (1, 16, 256, 4096):
+    reps = [cases[i % 256] for i in range(n)]
+    f = lambda i: torch.from_numpy(np.stack([c[i] for c in reps])).cuda()  # noqa: E731
+    uv, p3, W, K, init = f(0), f(1), f(2), f(3), f(4)
+    uv32, W32 = uv.float(), W.float()
+    _, inf = pvb.uncertainty_pnp_batch(uv, W, p3, K, init, return_info=True)
+    t_batch = per_call_us(lambda: pvb.uncertainty_pnp_batch(uv, W, p3, K, init))
+    t_p3p = per_call_us(lambda: pvb.p3p_init_batch(uv, W, p3, K))
+    t_votes = per_call_us(lambda: pvb.uncertainty_pnp_from_votes(uv32, None, p3, K, init, weights=W32))
+    print(f"n={n:5d}: uncertainty_pnp_batch {t_batch:8.1f} us ({t_batch / n:7.2f} us/problem, mean iterations "
+          f"{inf[:, 0].float().mean().item():.2f})  p3p_init_batch {t_p3p:8.1f} us  uncertainty_pnp_from_votes {t_votes:8.1f} us")
