@@ -34,9 +34,9 @@ class PvbDesc(ctypes.Structure):
 class PvbLayout(ctypes.Structure):
     _fields_ = [(n, ctypes.c_size_t) for n in
                 ("total", "status", "fgsum", "nz", "tn", "state", "bits", "ticket", "blocktot", "xy", "dirs", "hyp",
-                 "counts", "win", "refit_partial", "refit_ticket")] + [
+                 "counts", "win", "refit_partial", "refit_ticket", "prune_tiles", "prune_key", "prune_list", "prune_len")] + [
                     ("nwords", ctypes.c_int32), ("nblocks", ctypes.c_int32), ("capacity", ctypes.c_int32),
-                    ("refit_splits", ctypes.c_int32)]
+                    ("refit_splits", ctypes.c_int32), ("prune_ntiles", ctypes.c_int32)]
 
 
 class PvbPnpOptions(ctypes.Structure):
@@ -73,6 +73,7 @@ SIGNATURES = {
     "pvb_exchange_connect": (ctypes.c_int, [_vp, _vp]),
     "pvb_exchange_connect_ptrs": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_void_p)]),
     "pvb_ransac_voting_v3_push": (ctypes.c_int, [_dp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, ctypes.c_uint64, _vp]),
+    "pvb_ransac_voting_v3_all_counts": (ctypes.c_int, [_dp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, ctypes.c_uint64, _vp]),
     "pvb_estimate_voting_distribution_push": (ctypes.c_int, [_dp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, ctypes.c_uint64, _vp]),
     "pvb_exchange_wait": (ctypes.c_int, [_vp, ctypes.c_uint64, _vp, _vp, ctypes.c_double, _vp]),
     "pvb_exchange_status": (ctypes.c_int, [_vp, _vp]),

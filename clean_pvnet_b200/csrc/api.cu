@@ -117,11 +117,17 @@ int make_layout(const pvb_desc *d, pvb_layout *L)
     L->counts = take(B * K * hn * sizeof(int));
     L->win = take(B * K * sizeof(float2));
     L->refit_partial = take(B * K * splits * 5 * sizeof(double));
+    const int ntiles = (cap + PRUNE_TILE - 1) / PRUNE_TILE;
+    L->prune_tiles = take(B * K * ntiles * PRUNE_REC * sizeof(int));
+    L->prune_key = take(B * K * hn * sizeof(int));
+    L->prune_list = take(2 * B * K * hn * sizeof(int));
+    L->prune_len = take(2 * B * K * sizeof(int));
     L->total = off;
     L->nwords = nwords;
     L->nblocks = nblocks;
     L->capacity = cap;
     L->refit_splits = splits;
+    L->prune_ntiles = ntiles;
     return PVB_OK;
 }
 
@@ -131,6 +137,7 @@ struct Plan {
     VoteArgs v;
     float2 *win;
     RefitScratch refit;
+    PruneArgs prune;
 };
 
 int make_plan(const pvb_desc *d, const void *mask, const float *vertex, const int32_t *idxs,
@@ -177,7 +184,21 @@ int make_plan(const pvb_desc *d, const void *mask, const float *vertex, const in
     P->refit.partial = reinterpret_cast<double *>(w + L.refit_partial);
     P->refit.ticket = reinterpret_cast<int *>(w + L.refit_ticket);
     P->refit.splits = L.refit_splits;
+    P->prune.tiles = reinterpret_cast<int *>(w + L.prune_tiles);
+    P->prune.key = reinterpret_cast<int *>(w + L.prune_key);
+    P->prune.list = reinterpret_cast<int *>(w + L.prune_list);
+    P->prune.len = reinterpret_cast<int *>(w + L.prune_len);
+    P->prune.ntiles = L.prune_ntiles;
+    P->prune.cos_w = P->prune.sin_w = 0.f;
     return PVB_OK;
+}
+
+// the vote stage after launch_generate: v3 callers that read no counts (`prune`) score only the hypotheses that can win
+cudaError_t run_vote(const Plan &P, bool prune, cudaStream_t st)
+{
+    PruneArgs q = P.prune;
+    if (prune && prune_setup(P.v, q)) return launch_vote_pruned(P.v, q, st);
+    return launch_vote(P.v, false, st);
 }
 
 int run_select(const Plan &P, cudaStream_t st)
@@ -190,7 +211,7 @@ int run_select(const Plan &P, cudaStream_t st)
     return PVB_OK;
 }
 
-int run_front(const Plan &P, cudaStream_t st, ProfCall *pc)
+int run_front(const Plan &P, bool prune, cudaStream_t st, ProfCall *pc)
 {
     prof_start(pc, PVB_STAGE_SELECT, st);
     int rc = run_select(P, st);
@@ -201,7 +222,7 @@ int run_front(const Plan &P, cudaStream_t st, ProfCall *pc)
     if (e != cudaSuccess) return cuda_fail(e, "generate kernel");
     prof_end(pc, PVB_STAGE_GENERATE, st);
     prof_start(pc, PVB_STAGE_VOTE, st);
-    e = launch_vote(P.v, false, st);
+    e = run_vote(P, prune, st);
     if (e != cudaSuccess) return cuda_fail(e, "vote kernel");
     prof_end(pc, PVB_STAGE_VOTE, st);
     return PVB_OK;
@@ -270,7 +291,7 @@ PVB_API int pvb_workspace_layout(const pvb_desc *d, pvb_layout *out)
 
 static int run_v3(const pvb_desc *d, const void *mask, const float *vertex, const int32_t *idxs, const float *selection,
                   float *out_kpt, void *workspace, size_t workspace_bytes, const float *seg, int32_t classes,
-                  int64_t class_stride, int64_t *mask_out, pvb_exchange *ex, uint64_t seq, cudaStream_t st)
+                  int64_t class_stride, int64_t *mask_out, pvb_exchange *ex, uint64_t seq, bool prune, cudaStream_t st)
 {
     Plan P;
     int rc = make_plan(d, seg ? static_cast<const void *>(seg) : mask, vertex, idxs, selection, workspace, workspace_bytes, 1u, 2u, &P);
@@ -289,7 +310,7 @@ static int run_v3(const pvb_desc *d, const void *mask, const float *vertex, cons
         P.s.mask_out = reinterpret_cast<long long *>(mask_out);
     }
     ProfCall *pc = prof_begin(true);
-    rc = run_front(P, st, pc);
+    rc = run_front(P, prune, st, pc);
     if (rc) return rc;
     prof_start(pc, PVB_STAGE_FINISH, st);
     cudaError_t e = launch_refit(P.v, P.win, P.refit, out_kpt, pp, st);
@@ -303,7 +324,15 @@ PVB_API int pvb_ransac_voting_v3(const pvb_desc *d, const void *mask, const floa
                          pvb_stream_t stream)
 {
     return run_v3(d, mask, vertex, idxs, selection, out_kpt, workspace, workspace_bytes, nullptr, 0, 0, nullptr, nullptr, 0,
-                  static_cast<cudaStream_t>(stream));
+                  true, static_cast<cudaStream_t>(stream));
+}
+
+PVB_API int pvb_ransac_voting_v3_all_counts(const pvb_desc *d, const void *mask, const float *vertex, const int32_t *idxs,
+                                            const float *selection, float *out_kpt, void *workspace, size_t workspace_bytes,
+                                            pvb_exchange *exchange, uint64_t seq, pvb_stream_t stream)
+{
+    return run_v3(d, mask, vertex, idxs, selection, out_kpt, workspace, workspace_bytes, nullptr, 0, 0, nullptr, exchange, seq,
+                  false, static_cast<cudaStream_t>(stream));
 }
 
 PVB_API int pvb_ransac_voting_v3_push(const pvb_desc *d, const void *mask, const float *vertex, const int32_t *idxs,
@@ -312,7 +341,7 @@ PVB_API int pvb_ransac_voting_v3_push(const pvb_desc *d, const void *mask, const
 {
     if (!exchange) return fail(PVB_ERR_INVALID, "exchange is NULL");
     return run_v3(d, mask, vertex, idxs, selection, out_kpt, workspace, workspace_bytes, nullptr, 0, 0, nullptr, exchange, seq,
-                  static_cast<cudaStream_t>(stream));
+                  true, static_cast<cudaStream_t>(stream));
 }
 
 PVB_API int pvb_decode_v3(const pvb_desc *d, const float *seg, int32_t classes, int64_t class_stride, int64_t *mask_out,
@@ -322,7 +351,7 @@ PVB_API int pvb_decode_v3(const pvb_desc *d, const float *seg, int32_t classes, 
     if (classes < 1 || classes > 4096) return fail(PVB_ERR_INVALID, "classes must be in [1,4096]");
     if (!seg) return fail(PVB_ERR_INVALID, "seg is NULL");
     return run_v3(d, nullptr, vertex, idxs, selection, out_kpt, workspace, workspace_bytes, seg, classes, class_stride, mask_out,
-                  nullptr, 0, static_cast<cudaStream_t>(stream));
+                  nullptr, 0, true, static_cast<cudaStream_t>(stream));
 }
 
 static int run_distribution(const pvb_desc *d, const void *mask, const float *vertex, const float *mean, const int32_t *idxs,
@@ -341,7 +370,7 @@ static int run_distribution(const pvb_desc *d, const void *mask, const float *ve
         return PVB_OK;
     }
     ProfCall *pc = prof_begin(true);
-    rc = run_front(P, st, pc);
+    rc = run_front(P, false, st, pc);
     if (rc) return rc;
     prof_start(pc, PVB_STAGE_FINISH, st);
     cudaError_t e = launch_covariance(P.v, mean, out_cov, pp, st);
@@ -641,7 +670,7 @@ PVB_API int pvb_ransac_voting_v3_host(const pvb_desc *d, const void *mask_host, 
         PeerPush none;
         memset(&none, 0, sizeof(none));
         e = launch_generate(P.v, hp->cmp);
-        if (e == cudaSuccess) e = launch_vote(P.v, false, hp->cmp);
+        if (e == cudaSuccess) e = run_vote(P, true, hp->cmp);
         if (e == cudaSuccess) e = launch_refit(P.v, P.win, P.refit, reinterpret_cast<float *>(sb + S.out), none, hp->cmp);
         if (e != cudaSuccess) return cuda_fail(e, "compute kernels");
         e = cudaMemcpyAsync(reinterpret_cast<char *>(out_kpt_host) + (size_t)b0 * obytes, sb + S.out, (size_t)c * obytes, cudaMemcpyDeviceToHost, hp->cmp);

@@ -77,6 +77,8 @@ cudaError_t launch_generate(const VoteArgs &a, cudaStream_t st)
 struct VoteK {
     VoteArgs a;
     ConeParams cone;
+    const int *list;   // optional [B][K][hn]: slot s of (b,k) scores hypothesis list[s] (NULL: slot s is hypothesis s)
+    const int *len;    // [B][K] slots in use (with list)
 };
 
 constexpr int VOTE_BLOCK = 16;    // pixels per unrolled block (one guard-band check per block)
@@ -117,12 +119,15 @@ vote_kernel(const VoteK p)
     const int k = blockIdx.y % a.K, slice = blockIdx.y / a.K;
     const int tn = min(a.tn[b], a.cap);
     const int t0 = blockIdx.x * VOTE_TILE;
-    if (t0 >= tn) return;
+    const size_t bk = (size_t)b * a.K + k;
+    const int nh = p.list ? __ldg(p.len + bk) : a.hn;      // hypothesis slots of this (image, keypoint)
+    if (t0 >= tn || slice * (TEAM * HPT) >= nh) return;
+    const int *lst = p.list ? p.list + bk * a.hn : nullptr;
     const int n = min(VOTE_TILE, tn - t0);
     const int npad = (n + VOTE_BLOCK - 1) / VOTE_BLOCK * VOTE_BLOCK;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const float kappa = p.cone.kappa, thresh = p.cone.thresh;
-    const float2 *hyp = a.hyp + ((size_t)b * a.K + k) * a.hn;
+    const float2 *hyp = a.hyp + bk * a.hn;
     const float2 *xy = a.xy + (size_t)b * a.cap + t0;
     const float2 *dk = a.dirs + ((size_t)b * a.K + k) * a.cap + t0;
     const int team = tid / TEAM;
@@ -189,8 +194,8 @@ vote_kernel(const VoteK p)
     int neg[HPT];   // tests whose margin is negative (sign bit) = non-inliers, padding included
 #pragma unroll
     for (int j = 0; j < HPT; ++j) {
-        const int h = hbase + j * TEAM;
-        const float2 q = (h < a.hn) ? hyp[h] : make_float2(0.f, 0.f);
+        const int s = hbase + j * TEAM;
+        const float2 q = (s < nh) ? hyp[lst ? __ldg(lst + s) : s] : make_float2(0.f, 0.f);
         float xc = q.x - ox, yc = q.y - oy;
         const float S = fabsf(xc) + fabsf(yc) + cmax;
         float d = fmaxf(p.cone.band * S, p.cone.floor);    // the floor binds only for tiles narrower than ~0.4 px
@@ -244,8 +249,8 @@ vote_kernel(const VoteK p)
                     bm &= bm - 1;
                     const float hx_ = __shfl_sync(0xffffffffu, hxc[j], L), hy_ = __shfl_sync(0xffffffffu, hyc[j], L);
                     const float dl_ = __shfl_sync(0xffffffffu, dl[j], L);
-                    const int h = hbase - lane + L + j * TEAM;
-                    const float2 q = (h < a.hn) ? __ldg(hyp + h) : make_float2(0.f, 0.f);
+                    const int s = hbase - lane + L + j * TEAM;
+                    const float2 q = (s < nh) ? __ldg(hyp + (lst ? __ldg(lst + s) : s)) : make_float2(0.f, 0.f);
                     int delta = 0;
                     if (lane < nb) {
                         const float m = cone_margin(ra, rb, hx_, hy_);
@@ -260,12 +265,12 @@ vote_kernel(const VoteK p)
             }
         }
     }
-    int *counts = a.counts + ((size_t)b * a.K + k) * a.hn;
+    int *counts = a.counts + bk * a.hn;
 #pragma unroll
     for (int j = 0; j < HPT; ++j) {
-        const int h = hbase + j * TEAM;
+        const int s = hbase + j * TEAM;
         const int cnt = mine - neg[j];
-        if (h < a.hn && cnt) atomicAdd(counts + h, cnt);
+        if (s < nh && cnt) atomicAdd(counts + (lst ? __ldg(lst + s) : s), cnt);
     }
 }
 
@@ -314,6 +319,8 @@ cudaError_t launch_vote(const VoteArgs &a, bool zero_counts, cudaStream_t st)
     VoteK p;
     p.a = a;
     p.cone = make_cone(a.thresh);
+    p.list = nullptr;
+    p.len = nullptr;
     const int variant = g_vote_variant.load(std::memory_order_relaxed);
 #define PVB_VOTE(HPT, NT, MINB, TILE, WS)                                               \
     do {                                                                                \
@@ -329,6 +336,24 @@ cudaError_t launch_vote(const VoteArgs &a, bool zero_counts, cudaStream_t st)
     else if (variant == 3) PVB_VOTE(4, 128, 8, 512, 4);
     else PVB_VOTE(4, 128, 8, 1024, 4);    // H100 (400 W), cfg-2: 0.72 ms per launch vs 0.75 ms with 512-pixel tiles
 #undef PVB_VOTE
+    return cudaGetLastError();
+}
+
+// Both passes of the pruned v3 vote use one shape: 128-hypothesis slices (4 per thread, WS = 1) whose four warps split the
+// 1024-pixel tile, so a pass scores its list in whole slices of 128 and CTAs past a list's end return at once.
+cudaError_t launch_vote_list(const VoteArgs &a, const int *list, const int *len, int max_len, cudaStream_t st)
+{
+    constexpr int HPT = 4, NT = 128, TILE = 1024;
+    static_assert(HPT * 32 == PRUNE_M, "pass 1 is one slice");
+    if (max_len <= 0) return cudaSuccess;
+    VoteK p;
+    p.a = a;
+    p.cone = make_cone(a.thresh);
+    p.list = list;
+    p.len = len;
+    const int slices = (max_len + HPT * 32 - 1) / (HPT * 32);
+    dim3 g((a.cap + TILE - 1) / TILE, a.K * slices, a.B);
+    vote_kernel<HPT, NT, 8, TILE, 1><<<g, NT, 0, st>>>(p);
     return cudaGetLastError();
 }
 

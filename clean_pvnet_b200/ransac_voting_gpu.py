@@ -235,7 +235,12 @@ def _run(op, mask, vertex, hn, inlier_thresh, min_num, max_num, mean=None, idxs=
         sp = selection.data_ptr() if selection is not None else None
         if op == "v3":
             out = torch.empty((B, K, 2), dtype=torch.float32, device=dev)
-            if exchange is not None:          # (handle, seq): the refit kernel also pushes `out` to every peer
+            if debug and (B or exchange is not None):
+                # the counts are returned: score every hypothesis (the plain entries skip those that cannot win)
+                ex, seq = exchange if exchange is not None else (None, 0)
+                _lib.check(lib.pvb_ransac_voting_v3_all_counts(d, mask.data_ptr(), vertex.data_ptr(), ip, sp, out.data_ptr(),
+                                                               ws.data_ptr(), ws.numel(), ex, seq, stream))
+            elif exchange is not None:        # (handle, seq): the refit kernel also pushes `out` to every peer
                 _lib.check(lib.pvb_ransac_voting_v3_push(d, mask.data_ptr(), vertex.data_ptr(), ip, sp, out.data_ptr(),
                                                          ws.data_ptr(), ws.numel(), exchange[0], exchange[1], stream))
             elif B:

@@ -119,10 +119,16 @@ typedef struct pvb_layout {
     size_t win;      /* float2[B][K] winning hypothesis before the refit */
     size_t refit_partial; /* double[B][K][refit_splits][5] partial normal equations */
     size_t refit_ticket;  /* int32[B][K] arrival counters of the refit CTAs */
+    size_t prune_tiles;   /* int32[B][K][prune_ntiles][68] per 1024-pixel tile: bounding box (4 floats), then the
+                             inclusive prefix sums of a 64-bin histogram of the pixels' direction pseudo-angles */
+    size_t prune_key;     /* int32[B][K][hn] angular upper bound of each hypothesis's count, -1 if scored in pass 1 */
+    size_t prune_list;    /* int32[2][B][K][hn] hypotheses scored by pass 1 / pass 2 of the pruned v3 vote */
+    size_t prune_len;     /* int32[2][B][K] lengths of those lists */
     int32_t nwords;  /* ceil(H*W/32) */
     int32_t nblocks; /* ceil(nwords/128) */
     int32_t capacity;
     int32_t refit_splits;
+    int32_t prune_ntiles; /* ceil(capacity/1024) */
 } pvb_layout;
 
 PVB_API int pvb_version(void);
@@ -141,7 +147,10 @@ PVB_API int pvb_workspace_layout(const pvb_desc *d, pvb_layout *out);
  *           (:136), consulted only for images with fg > max_num.  NULL -> philox.
  *   out_kpt device fp32 [B,K,2] contiguous.
  * `confidence` / `max_iter` of the reference do not influence its result (idxs is drawn once,
- * outside the loop, :145 vs :150) and therefore have no counterpart here. */
+ * outside the loop, :145 vs :150) and therefore have no counterpart here.
+ * Only the winners and their inliers are observable, so this entry (like pvb_decode_v3, the _push and the host-buffer
+ * entries) does not score hypotheses that an angular bound proves cannot win (DESIGN.md 4.2): their `counts` in the
+ * workspace stay 0.  pvb_ransac_voting_v3_all_counts (below) computes the same keypoints and scores every hypothesis. */
 PVB_API int pvb_ransac_voting_v3(const pvb_desc *d, const void *mask, const float *vertex,
                          const int32_t *idxs, const float *selection, float *out_kpt,
                          void *workspace, size_t workspace_bytes, pvb_stream_t stream);
@@ -264,6 +273,11 @@ PVB_API int pvb_exchange_connect_ptrs(pvb_exchange *ex, void *const *bases /* wo
 PVB_API int pvb_ransac_voting_v3_push(const pvb_desc *d, const void *mask, const float *vertex, const int32_t *idxs,
                                       const float *selection, float *out_kpt, void *workspace, size_t workspace_bytes,
                                       pvb_exchange *exchange, uint64_t seq, pvb_stream_t stream);
+/* pvb_ransac_voting_v3 (exchange == NULL) or pvb_ransac_voting_v3_push with every hypothesis scored: afterwards the
+ * workspace's `counts` hold the reference's inlier count of every hypothesis (the Python operator's debug=True). */
+PVB_API int pvb_ransac_voting_v3_all_counts(const pvb_desc *d, const void *mask, const float *vertex, const int32_t *idxs,
+                                            const float *selection, float *out_kpt, void *workspace, size_t workspace_bytes,
+                                            pvb_exchange *exchange, uint64_t seq, pvb_stream_t stream);
 /* the same for the second half of the un_pnp pair (resnet18.py:71-72): every [2,2] covariance goes to every peer as the
  * covariance kernel produces it (4 floats per (image, keypoint); use an exchange of its own: bytes_per_rank >= B*K*16) */
 PVB_API int pvb_estimate_voting_distribution_push(const pvb_desc *d, const void *mask, const float *vertex, const float *mean,
