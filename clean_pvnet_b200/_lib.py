@@ -34,9 +34,9 @@ class PvbDesc(ctypes.Structure):
 class PvbLayout(ctypes.Structure):
     _fields_ = [(n, ctypes.c_size_t) for n in
                 ("total", "status", "fgsum", "nz", "tn", "state", "bits", "ticket", "blocktot", "xy", "dirs", "hyp",
-                 "counts", "win", "refit_partial", "refit_ticket", "prune_tiles", "prune_key", "prune_list", "prune_len")] + [
+                 "counts", "win", "refit_partial", "refit_ticket", "prune_cells", "prune_key", "prune_list", "prune_len")] + [
                     ("nwords", ctypes.c_int32), ("nblocks", ctypes.c_int32), ("capacity", ctypes.c_int32),
-                    ("refit_splits", ctypes.c_int32), ("prune_ntiles", ctypes.c_int32)]
+                    ("refit_splits", ctypes.c_int32), ("prune_ncells", ctypes.c_int32)]
 
 
 class PvbPnpOptions(ctypes.Structure):

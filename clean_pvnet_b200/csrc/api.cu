@@ -117,8 +117,8 @@ int make_layout(const pvb_desc *d, pvb_layout *L)
     L->counts = take(B * K * hn * sizeof(int));
     L->win = take(B * K * sizeof(float2));
     L->refit_partial = take(B * K * splits * 5 * sizeof(double));
-    const int ntiles = (cap + PRUNE_TILE - 1) / PRUNE_TILE;
-    L->prune_tiles = take(B * K * ntiles * PRUNE_REC * sizeof(int));
+    const size_t ncells = (size_t)((d->H + PRUNE_CELL - 1) / PRUNE_CELL) * ((d->W + PRUNE_CELL - 1) / PRUNE_CELL);
+    L->prune_cells = take(B * K * ncells * PRUNE_REC * sizeof(int));
     L->prune_key = take(B * K * hn * sizeof(int));
     L->prune_list = take(2 * B * K * hn * sizeof(int));
     L->prune_len = take(2 * B * K * sizeof(int));
@@ -127,7 +127,7 @@ int make_layout(const pvb_desc *d, pvb_layout *L)
     L->nblocks = nblocks;
     L->capacity = cap;
     L->refit_splits = splits;
-    L->prune_ntiles = ntiles;
+    L->prune_ncells = (int)ncells;
     return PVB_OK;
 }
 
@@ -184,11 +184,12 @@ int make_plan(const pvb_desc *d, const void *mask, const float *vertex, const in
     P->refit.partial = reinterpret_cast<double *>(w + L.refit_partial);
     P->refit.ticket = reinterpret_cast<int *>(w + L.refit_ticket);
     P->refit.splits = L.refit_splits;
-    P->prune.tiles = reinterpret_cast<int *>(w + L.prune_tiles);
+    P->prune.cells = reinterpret_cast<int *>(w + L.prune_cells);
     P->prune.key = reinterpret_cast<int *>(w + L.prune_key);
     P->prune.list = reinterpret_cast<int *>(w + L.prune_list);
     P->prune.len = reinterpret_cast<int *>(w + L.prune_len);
-    P->prune.ntiles = L.prune_ntiles;
+    P->prune.ncx = (d->W + PRUNE_CELL - 1) / PRUNE_CELL;
+    P->prune.ncells = L.prune_ncells;
     P->prune.cos_w = P->prune.sin_w = 0.f;
     return PVB_OK;
 }

@@ -50,29 +50,31 @@ cudaError_t launch_generate(const VoteArgs &a, cudaStream_t st);
 cudaError_t launch_vote(const VoteArgs &a, bool zero_counts, cudaStream_t st);
 
 // Pruned v3 vote (prune.cu, DESIGN.md 4.2): only hypotheses that can still be the first maximum are scored.  A bound
-// B(h) >= count(h) comes from per-tile direction histograms; pass 1 scores the PRUNE_M largest bounds, pass 2 every other
+// B(h) >= count(h) comes from per-cell direction histograms; pass 1 scores the PRUNE_M largest bounds, pass 2 every other
 // hypothesis whose bound reaches pass 1's best count.  The others keep count 0, below the winner's.
-constexpr int PRUNE_TILE = 1024;            // pixels per histogram tile
-constexpr int PRUNE_NBIN = 64;              // pseudo-angle bins per tile
-constexpr int PRUNE_REC = 4 + PRUNE_NBIN;   // words per (image, keypoint, tile): box, inclusive prefix counts
+constexpr int PRUNE_CELL = 32;              // histogram cells are PRUNE_CELL x PRUNE_CELL pixels of the image
+constexpr int PRUNE_NBIN = 128;             // pseudo-angle bins per cell
+constexpr int PRUNE_REC = 4 + PRUNE_NBIN / 2;   // words per (image, keypoint, cell): box, 16-bit inclusive prefix counts
 constexpr int PRUNE_M = 128;                // pass-1 hypotheses = one slice of the pruned vote shape
 constexpr int PRUNE_MAX_HN = 2048;          // the plan kernel holds two hypotheses per thread
 constexpr int PRUNE_MIN_UNITS = 32;         // fewer (image, keypoint) pairs: the full vote is faster
+static_assert(PRUNE_CELL * PRUNE_CELL < 65536, "a cell's prefix counts fit 16 bits");
 struct PruneArgs {
-    int *tiles;          // [B][K][ntiles][PRUNE_REC]
+    int *cells;          // [B][K][ncells][PRUNE_REC], cell (row band y, column x) at y * ncx + x
     int *key;            // [B][K][hn]  bound, or -1 for pass-1 hypotheses
     int *list;           // [2][B][K][hn]
     int *len;            // [2][B][K]
-    int ntiles;
+    int ncx, ncells;     // ceil(W / PRUNE_CELL), ceil(H / PRUNE_CELL) * ncx
     float cos_w, sin_w;  // rotation by the widened cone half-angle theta'
 };
 // false when pruning cannot pay (thresholds outside (0,1) or nearly 0, hn <= PRUNE_M, hn > PRUNE_MAX_HN, B*K < PRUNE_MIN_UNITS);
 // otherwise fills cos_w / sin_w
 bool prune_setup(const VoteArgs &a, PruneArgs &q);
-// histograms + bounds + pass 1 + pass 2; counts must be zeroed (launch_generate)
+// cell histograms + bounds + pass 1 + pass 2; counts must be zeroed (launch_generate)
 cudaError_t launch_vote_pruned(const VoteArgs &a, const PruneArgs &q, cudaStream_t st);
-// the vote kernel over hypothesis lists: slot s of (b,k) scores hypothesis list[(b*K+k)*hn + s], s < len[b*K+k]
-cudaError_t launch_vote_list(const VoteArgs &a, const int *list, const int *len, int max_len, cudaStream_t st);
+// the vote kernel over hypothesis lists: slot s of (b,k) scores hypothesis list[(b*K+k)*hn + s], s < len[b*K+k], in slices
+// of 128 hypotheses (`narrow`: 64)
+cudaError_t launch_vote_list(const VoteArgs &a, const int *list, const int *len, int max_len, bool narrow, cudaStream_t st);
 void set_vote_tuning(int variant);   // tooling: pixel-tile size per CTA
 void set_gather_tuning(int mode);    // tooling: gather access pattern (select.cu)
 // argmax + winner refit -> out_kpt [B][K][2], win [B][K].  The pixels of one (image,keypoint) are split

@@ -1,16 +1,17 @@
 // prune.cu -- the pruned v3 vote: hypotheses that an angular bound proves cannot be the first maximum are never scored.
 //
 // For v3 only the first-max winner of each (image, keypoint) and its inliers are observable.  A pixel c with direction u
-// votes for h only if angle(u, h-c) < theta = acos(t).  For a tile of pixels with bounding box Q and h outside Q, every
+// votes for h only if angle(u, h-c) < theta = acos(t).  For a set of pixels with bounding box Q and h outside Q, every
 // h-c (c in Q) lies in the angular interval [psi_lo, psi_hi] that Q subtends from h (convexity: the extremes are corners),
-// so at most #{c in tile : angle(u_c) in [psi_lo - theta', psi_hi + theta']} of its pixels vote for h.  Summed over the
-// tiles this is B(h) >= count(h).  A hypothesis with B(h) < L, L the exact count of any hypothesis, cannot be the first
-// maximum.  DESIGN.md 4.2 has the argument, including the slack theta' - theta.
+// so at most #{c in set : angle(u_c) in [psi_lo - theta', psi_hi + theta']} of its pixels vote for h.  The sets are the
+// 32x32-pixel cells of the image; summed over the cells this is B(h) >= count(h).  A hypothesis with B(h) < L, L the exact
+// count of any hypothesis, cannot be the first maximum.  DESIGN.md 4.2 has the argument, including the slack theta' - theta.
 //
-//   prune_hist_kernel   (tile, k, b): bounding box + prefix histogram of direction pseudo-angles of one tile
-//   prune_plan_kernel   (k, b):       B(h) for every hypothesis, the PRUNE_M largest -> list 0 (pass 1)
+//   prune_hist_kernel   (band, k, b):   per cell of a 32-row band: bounding box + prefix histogram of direction pseudo-angles
+//   prune_bound_kernel  (h group, k, b): B(h), one thread per hypothesis -> key
+//   prune_plan_kernel   (k, b):         the PRUNE_M largest bounds -> list 0 (pass 1)
 //   vote_kernel         list 0
-//   prune_next_kernel   (k, b):       L = best pass-1 count; {h not in pass 1 : B(h) >= L} -> list 1 (pass 2)
+//   prune_next_kernel   (k, b):         L = best pass-1 count; {h not in pass 1 : B(h) >= L} -> list 1 (pass 2)
 //   vote_kernel         list 1
 #include <cmath>
 #include <math_constants.h>
@@ -19,83 +20,134 @@
 
 namespace pvb {
 
-// Monotone pseudo-angle of a non-zero direction, in [0, 4] counter-clockwise from +x (one unit per quadrant).
+// Monotone pseudo-angle of a non-zero direction, in [0, 4] counter-clockwise from +x (one unit per quadrant).  The bound
+// divides approximately; the histogram divides with IEEE rounding (EXACT), so its bins are reproducible bit for bit.
+template <bool EXACT = false>
 __device__ __forceinline__ float pseudo_angle(float x, float y)
 {
-    if (y >= 0.f) return x >= 0.f ? __fdividef(y, x + y) : 1.f + __fdividef(-x, y - x);
-    return x < 0.f ? 2.f + __fdividef(-y, -x - y) : 3.f + __fdividef(x, x - y);
+    auto div = [](float a, float b) { return EXACT ? __fdiv_rn(a, b) : __fdividef(a, b); };
+    if (y >= 0.f) return x >= 0.f ? div(y, x + y) : 1.f + div(-x, y - x);
+    return x < 0.f ? 2.f + div(-y, -x - y) : 3.f + div(x, x - y);
+}
+
+// First index i in [0, n) with xy[i].y >= y (n if none); xy is sorted by y.  Warp-cooperative 32-ary search: three rounds
+// of 32 probes for 30 000 pixels instead of fifteen dependent loads.
+__device__ int first_row_at(const float2 *xy, int n, float y)
+{
+    const int lane = threadIdx.x & 31;
+    int lo = 0, hi = n;                                  // the answer lies in [lo, hi]
+    while (hi > lo) {
+        const int step = (hi - lo + 31) / 32;
+        const int p = lo + lane * step;
+        const unsigned below = __ballot_sync(0xffffffffu, p < hi && __ldg(&xy[p].y) < y);   // a prefix of the lanes
+        const int nb = __popc(below);
+        const int nlo = nb ? lo + (nb - 1) * step + 1 : lo;
+        hi = min(hi, lo + nb * step);
+        lo = nlo;
+    }
+    return lo;
 }
 
 constexpr int HIST_THREADS = 256;
+constexpr int HIST_CELLS = 32;                 // cells of a band histogrammed at a time (16 KB of shared memory)
 
+// One CTA per (band of PRUNE_CELL pixel rows, k, b).  The selected-pixel list is in raster (torch.nonzero) order, so the
+// band's pixels are one contiguous segment of it.  Every cell of the band gets a record, empty ones with total 0.
 __global__ void __launch_bounds__(HIST_THREADS)
 prune_hist_kernel(VoteArgs a, PruneArgs q)
 {
-    const int tile = blockIdx.x, k = blockIdx.y, b = blockIdx.z;
-    const int tn = min(a.tn[b], a.cap);
-    const int t0 = tile * PRUNE_TILE;
-    if (t0 >= tn) return;
-    const int n = min(PRUNE_TILE, tn - t0);
+    const int band = blockIdx.x, k = blockIdx.y, b = blockIdx.z;
+    const int tn = max(0, min(a.tn[b], a.cap));
     const size_t bk = (size_t)b * a.K + k;
-    const float2 *xy = a.xy + (size_t)b * a.cap + t0;
-    const float2 *dk = a.dirs + bk * a.cap + t0;
-    __shared__ int s_hist[PRUNE_NBIN];
-    __shared__ float s_box[4][HIST_THREADS / 32];
+    const float2 *xy = a.xy + (size_t)b * a.cap;
+    const float2 *dk = a.dirs + bk * a.cap;
+    __shared__ __align__(16) int s_hist[HIST_CELLS][PRUNE_NBIN];
+    __shared__ int s_box[HIST_CELLS][4];                 // float bits of x0, x1, y0, y1: coordinates are >= 0
+    __shared__ int s_seg[2];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid < PRUNE_NBIN) s_hist[tid] = 0;
-    __syncthreads();
-    float x0 = CUDART_INF_F, x1 = -CUDART_INF_F, y0 = CUDART_INF_F, y1 = -CUDART_INF_F;
-    for (int i = tid; i < n; i += HIST_THREADS) {
-        const float2 c = __ldg(xy + i), v = __ldg(dk + i);
-        x0 = fminf(x0, c.x); x1 = fmaxf(x1, c.x); y0 = fminf(y0, c.y); y1 = fmaxf(y1, c.y);
-        // the reference never lets a pixel vote whose norm1 is below 1e-6 or NaN (.cu:121), nor one whose norm1
-        // overflows (its cosine is then 0 or NaN): such pixels are left out of the histogram
-        const float n1 = __fsqrt_rn(__fmaf_rn(v.x, v.x, __fmul_rn(v.y, v.y)));
-        if (n1 > below_1e6() && n1 < CUDART_INF_F) {
-            const int bin = min(PRUNE_NBIN - 1, (int)(pseudo_angle(v.x, v.y) * (PRUNE_NBIN / 4)));
-            atomicAdd(&s_hist[bin], 1);
-        }
+    if (warp < 2) {
+        const int i = first_row_at(xy, tn, (float)((band + warp) * PRUNE_CELL));
+        if (lane == 0) s_seg[warp] = i;
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        x0 = fminf(x0, __shfl_xor_sync(0xffffffffu, x0, o)); x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, o));
-        y0 = fminf(y0, __shfl_xor_sync(0xffffffffu, y0, o)); y1 = fmaxf(y1, __shfl_xor_sync(0xffffffffu, y1, o));
-    }
-    if (lane == 0) { s_box[0][warp] = x0; s_box[1][warp] = x1; s_box[2][warp] = y0; s_box[3][warp] = y1; }
-    __syncthreads();
-    int *rec = q.tiles + (bk * q.ntiles + tile) * PRUNE_REC;
-    if (warp == 0) {
-        // inclusive prefix of the 64 bins, two per lane
-        const int h0 = s_hist[2 * lane], h1 = s_hist[2 * lane + 1];
-        int s = h0 + h1;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int t = __shfl_up_sync(0xffffffffu, s, o);
-            if (lane >= o) s += t;
+    for (int cx0 = 0; cx0 < q.ncx; cx0 += HIST_CELLS) {
+        const int nc = min(HIST_CELLS, q.ncx - cx0);
+        for (int i = tid; i < HIST_CELLS * PRUNE_NBIN; i += HIST_THREADS) (&s_hist[0][0])[i] = 0;
+        if (tid < HIST_CELLS * 4) (&s_box[0][0])[tid] = __float_as_int((tid & 1) ? -CUDART_INF_F : CUDART_INF_F);
+        __syncthreads();
+        const int s0 = s_seg[0], s1 = s_seg[1];
+        float2 cn = make_float2(0.f, 0.f), vn = make_float2(0.f, 0.f);
+        if (s0 + tid < s1) { cn = __ldg(xy + s0 + tid); vn = __ldg(dk + s0 + tid); }
+        for (int i0 = s0 + warp * 32; i0 < s1; i0 += HIST_THREADS) {
+            const int i = i0 + lane;
+            const float2 c = cn, v = vn;
+            if (i + HIST_THREADS < s1) { cn = __ldg(xy + i + HIST_THREADS); vn = __ldg(dk + i + HIST_THREADS); }
+            int key = -1, hkey = -1, cx = 0;
+            if (i < s1) {
+                cx = (int)c.x / PRUNE_CELL - cx0;
+                // the reference never lets a pixel vote whose norm1 is below 1e-6 or NaN (.cu:121), nor one whose norm1
+                // overflows (its cosine is then 0 or NaN): such pixels are left out of the box and the histogram
+                const float n1 = __fsqrt_rn(__fmaf_rn(v.x, v.x, __fmul_rn(v.y, v.y)));
+                if (cx >= 0 && cx < nc && n1 > below_1e6() && n1 < CUDART_INF_F) {
+                    const int bin = min(PRUNE_NBIN - 1, (int)(pseudo_angle<true>(v.x, v.y) * (PRUNE_NBIN / 4)));
+                    key = ((int)c.y - band * PRUNE_CELL) * HIST_CELLS + cx;
+                    hkey = cx * PRUNE_NBIN + bin;
+                }
+            }
+            // neighbouring pixels mostly share a cell and a bin, and shared atomics on one address serialise: each run
+            // of lanes with equal (cell, bin) adds its length once
+            const int hprev = __shfl_up_sync(0xffffffffu, hkey, 1);
+            const unsigned heads = __ballot_sync(0xffffffffu, lane == 0 || hprev != hkey);
+            if (hkey >= 0 && (lane == 0 || hprev != hkey)) {
+                const unsigned later = heads & ~((2u << lane) - 1u);
+                atomicAdd(&(&s_hist[0][0])[hkey], (later ? __ffs(later) - 1 : 32) - lane);
+            }
+            // in raster order the lanes of one (row, cell) form runs sorted by x: only a run's first and last lane update
+            // the box
+            const int prev = __shfl_up_sync(0xffffffffu, key, 1), next = __shfl_down_sync(0xffffffffu, key, 1);
+            if (key >= 0 && (lane == 0 || prev != key)) {
+                atomicMin(&s_box[cx][0], __float_as_int(c.x));
+                atomicMin(&s_box[cx][2], __float_as_int(c.y));
+            }
+            if (key >= 0 && (lane == 31 || next != key)) {
+                atomicMax(&s_box[cx][1], __float_as_int(c.x));
+                atomicMax(&s_box[cx][3], __float_as_int(c.y));
+            }
         }
-        rec[4 + 2 * lane] = s - h1;
-        rec[4 + 2 * lane + 1] = s;
-        if (lane < 4) {
-            float e = s_box[lane][0];
-            for (int w = 1; w < HIST_THREADS / 32; ++w) e = (lane & 1) ? fmaxf(e, s_box[lane][w]) : fminf(e, s_box[lane][w]);
-            rec[lane] = __float_as_int(e);
+        __syncthreads();
+        // one warp per cell: inclusive prefix of the 128 bins, four per lane, stored as 16-bit counts two per word
+        for (int cc = warp; cc < nc; cc += HIST_THREADS / 32) {
+            const int4 h = reinterpret_cast<const int4 *>(s_hist[cc])[lane];
+            int s = h.x + h.y + h.z + h.w;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int t = __shfl_up_sync(0xffffffffu, s, o);
+                if (lane >= o) s += t;
+            }
+            const int p1 = s - h.w - h.z, p0 = p1 - h.y;
+            int *rec = q.cells + (bk * q.ncells + (size_t)band * q.ncx + cx0 + cc) * PRUNE_REC;
+            rec[4 + 2 * lane] = p0 | (p1 << 16);
+            rec[4 + 2 * lane + 1] = (s - h.w) | (s << 16);
+            if (lane < 4) rec[lane] = s_box[cc][lane];
         }
+        __syncthreads();                                  // s_hist / s_box are reset for the next cells
     }
 }
 
-// Pixels of a tile whose direction bin lies in [blo, bhi] (bins taken modulo PRUNE_NBIN; bhi - blo + 1 < PRUNE_NBIN)
-__device__ __forceinline__ int bins_between(const int *P, int blo, int bhi, int tot)
+__device__ __forceinline__ int cell_total(const int *rec) { return (int)((unsigned)rec[PRUNE_REC - 1] >> 16); }
+
+// Pixels of a cell whose direction bin lies in [blo, bhi] (bins taken modulo PRUNE_NBIN; bhi - blo + 1 < PRUNE_NBIN)
+__device__ __forceinline__ int bins_between(const unsigned short *P, int blo, int bhi, int tot)
 {
     // C(j) = pixels with (unwrapped) bin < j = P[j mod NB - 1] + tot * floor(j / NB)
     auto C = [&](int j) {
         const int w = (j >= 0) ? j / PRUNE_NBIN : -((PRUNE_NBIN - 1 - j) / PRUNE_NBIN);
         const int r = j - w * PRUNE_NBIN;
-        return (r ? P[r - 1] : 0) + tot * w;
+        return (r ? (int)P[r - 1] : 0) + tot * w;
     };
     return C(bhi + 1) - C(blo);
 }
 
-// Adds to `bound` the bound of h over nt tile records `rec` (shared memory)
+// Adds to `bound` the bound of h over nt cell records `rec` (shared memory)
 __device__ void count_bound(const PruneArgs &q, const int *rec, int nt, float hx, float hy, int &bound)
 {
     const float c = q.cos_w, s = q.sin_w;
@@ -103,7 +155,7 @@ __device__ void count_bound(const PruneArgs &q, const int *rec, int nt, float hx
     for (int t = 0; t < nt; ++t, rec += PRUNE_REC) {
         const float x0 = __int_as_float(rec[0]), x1 = __int_as_float(rec[1]);
         const float y0 = __int_as_float(rec[2]), y1 = __int_as_float(rec[3]);
-        const int tot = rec[4 + PRUNE_NBIN - 1];
+        const int tot = cell_total(rec);
         if (hx >= x0 - 0.5f && hx <= x1 + 0.5f && hy >= y0 - 0.5f && hy <= y1 + 0.5f) { bound += tot; continue; }
         // h is at least half a pixel outside the box: the directions h - corner lie in an open half-plane, where
         // "counter-clockwise of" (cross product > 0) orders them; lo / hi are the extreme ones
@@ -121,13 +173,62 @@ __device__ void count_bound(const PruneArgs &q, const int *rec, int nt, float hx
         if (phi < plo) phi += 4.f;
         const int blo = (int)floorf((plo - EPS) * (PRUNE_NBIN / 4));
         const int bhi = (int)floorf((phi + EPS) * (PRUNE_NBIN / 4));
-        bound += (bhi - blo + 1 >= PRUNE_NBIN) ? tot : bins_between(rec + 4, blo, bhi, tot);
+        bound += (bhi - blo + 1 >= PRUNE_NBIN)
+                     ? tot : bins_between(reinterpret_cast<const unsigned short *>(rec + 4), blo, bhi, tot);
     }
+}
+
+constexpr int BOUND_HYPS = 128;                // hypotheses per CTA
+constexpr int BOUND_SPLIT = 3;                 // threads per hypothesis, each over a third of the records: one thread per
+                                               // hypothesis leaves ~4 warps per scheduler, too few to hide the latency
+constexpr int BOUND_THREADS = BOUND_HYPS * BOUND_SPLIT;
+constexpr int BOUND_CELLS = 64;                // non-empty cell records staged in shared memory at a time (17 KB)
+
+__global__ void __launch_bounds__(BOUND_THREADS)
+prune_bound_kernel(VoteArgs a, PruneArgs q)
+{
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int part = tid / BOUND_HYPS;
+    const int h = blockIdx.x * BOUND_HYPS + tid % BOUND_HYPS, k = blockIdx.y, b = blockIdx.z;
+    const size_t bk = (size_t)b * a.K + k;
+    const int tn = max(0, min(a.tn[b], a.cap));
+    __shared__ int s_rec[BOUND_CELLS * PRUNE_REC];
+    __shared__ int s_idx[BOUND_CELLS];
+    __shared__ int s_bound[BOUND_HYPS];
+    __shared__ int s_n, s_next;
+    if (tid < BOUND_HYPS) s_bound[tid] = 0;
+    const float2 hp = (h < a.hn) ? a.hyp[bk * a.hn + h] : make_float2(0.f, 0.f);
+    const int *rec = q.cells + bk * q.ncells * PRUNE_REC;
+    int bound = 0;
+    for (int c0 = 0; c0 < q.ncells;) {
+        if (warp == 0) {                                  // the next non-empty cells: an empty one adds nothing
+            int m = 0, c = c0;
+            for (; c < q.ncells && m <= BOUND_CELLS - 32; c += 32) {
+                const bool f = c + lane < q.ncells && cell_total(rec + (size_t)(c + lane) * PRUNE_REC) > 0;
+                const unsigned bal = __ballot_sync(0xffffffffu, f);
+                if (f) s_idx[m + __popc(bal & ((1u << lane) - 1u))] = c + lane;
+                m += __popc(bal);
+            }
+            if (lane == 0) { s_n = m; s_next = c; }
+        }
+        __syncthreads();
+        const int m = s_n;
+        c0 = s_next;
+        for (int r = warp; r < m; r += BOUND_THREADS / 32)
+            for (int w = lane; w < PRUNE_REC; w += 32) s_rec[r * PRUNE_REC + w] = __ldg(rec + (size_t)s_idx[r] * PRUNE_REC + w);
+        __syncthreads();
+        const int r0 = part * m / BOUND_SPLIT, r1 = (part + 1) * m / BOUND_SPLIT;
+        count_bound(q, s_rec + r0 * PRUNE_REC, r1 - r0, hp.x, hp.y, bound);
+        __syncthreads();                                  // s_idx, s_rec, s_n, s_next are rewritten
+    }
+    if (part > 0) atomicAdd(&s_bound[tid % BOUND_HYPS], bound);
+    __syncthreads();
+    // non-finite or huge: not bounded
+    if (part == 0 && h < a.hn) q.key[bk * a.hn + h] = (fabsf(hp.x) + fabsf(hp.y) <= 1e15f) ? bound + s_bound[tid] : tn;
 }
 
 constexpr int PLAN_THREADS = 1024;
 constexpr int PLAN_HPT = PRUNE_MAX_HN / PLAN_THREADS;
-constexpr int PLAN_TILES = 32;                 // tile records staged in shared memory at a time (8.7 KB)
 
 // exclusive prefix of `flag` over the CTA in thread order; returns it, *total gets the sum.  Every thread calls it.
 __device__ __forceinline__ int cta_scan(bool flag, int *s_warp, int *total)
@@ -154,29 +255,12 @@ prune_plan_kernel(VoteArgs a, PruneArgs q)
     const size_t bk = (size_t)b * a.K + k;
     const int tn = max(0, min(a.tn[b], a.cap));
     __shared__ int s_warp[PLAN_THREADS / 32];
-    __shared__ int s_rec[PLAN_TILES * PRUNE_REC];
     int bnd[PLAN_HPT];
-    float2 hp[PLAN_HPT];
 #pragma unroll
     for (int j = 0; j < PLAN_HPT; ++j) {
         const int h = j * PLAN_THREADS + tid;
-        bnd[j] = (h < a.hn) ? 0 : -1;                     // no hypothesis: -1, never selected
-        hp[j] = (h < a.hn) ? a.hyp[bk * a.hn + h] : make_float2(0.f, 0.f);
+        bnd[j] = (h < a.hn) ? q.key[bk * a.hn + h] : -1;  // no hypothesis: -1, never selected
     }
-    const int nt = (tn + PRUNE_TILE - 1) / PRUNE_TILE;
-    const int *rec = q.tiles + bk * q.ntiles * PRUNE_REC;
-    for (int t0 = 0; t0 < nt; t0 += PLAN_TILES) {
-        const int m = min(PLAN_TILES, nt - t0);
-        __syncthreads();
-        for (int i = tid; i < m * PRUNE_REC; i += PLAN_THREADS) s_rec[i] = __ldg(rec + t0 * PRUNE_REC + i);
-        __syncthreads();
-#pragma unroll
-        for (int j = 0; j < PLAN_HPT; ++j)
-            if (bnd[j] >= 0) count_bound(q, s_rec, m, hp[j].x, hp[j].y, bnd[j]);
-    }
-#pragma unroll
-    for (int j = 0; j < PLAN_HPT; ++j)                   // non-finite or huge: not bounded
-        if (bnd[j] >= 0 && !(fabsf(hp[j].x) + fabsf(hp[j].y) <= 1e15f)) bnd[j] = tn;
     // pass 1: the M largest bounds (ties in index order).  thr = largest v with #{B >= v} >= M, by bisection over [0, tn]
     const int M = min(PRUNE_M, a.hn);
     int lo = 0, hi = tn + 1;
@@ -200,7 +284,7 @@ prune_plan_kernel(VoteArgs a, PruneArgs q)
         const bool sel = bnd[j] > lo || (bnd[j] == lo && r < M - gt);
         const int pos = base_sel + cta_scan(sel, s_warp, &n_sel);
         if (sel) list[pos] = h;
-        if (h < a.hn) q.key[bk * a.hn + h] = sel ? -1 : bnd[j];
+        if (h < a.hn && sel) q.key[bk * a.hn + h] = -1;
         base_eq += n_eq;
         base_sel += n_sel;
     }
@@ -242,10 +326,10 @@ bool prune_setup(const VoteArgs &a, PruneArgs &q)
 {
     const double t = (double)a.thresh;
     if (!(t > 0.0 && t < 1.0) || a.hn <= PRUNE_M || a.hn > PRUNE_MAX_HN) return false;
-    // below PRUNE_MIN_UNITS (image, keypoint) pairs the full vote is short of a wave and latency bound: the four extra
+    // below PRUNE_MIN_UNITS (image, keypoint) pairs the full vote is short of a wave and latency bound: the extra
     // launches cost more than the skipped tests save (H100, B=1, K=9: 0.104 ms per call in full, 0.151 ms pruned)
     if ((long long)a.B * a.K < PRUNE_MIN_UNITS) return false;
-    if ((long long)a.K * ((a.hn + PRUNE_M - 1) / PRUNE_M) > 65535) return false;
+    if ((long long)a.K * ((a.hn + 63) / 64) > 65535) return false;     // grid.y of pass 2's 64-hypothesis slices
     // theta' >= every angle at which the reference can still count a vote: its fp32 cosine is within 9u of the exact one
     // (DESIGN.md 4.1), so a vote needs cos > t - 9u; 64u and 1e-5 rad on top cover the rounding of the bound itself
     const double u = ldexp(1.0, -24);
@@ -260,12 +344,14 @@ bool prune_setup(const VoteArgs &a, PruneArgs &q)
 cudaError_t launch_vote_pruned(const VoteArgs &a, const PruneArgs &q, cudaStream_t st)
 {
     const size_t BK = (size_t)a.B * a.K;
-    prune_hist_kernel<<<dim3(q.ntiles, a.K, a.B), HIST_THREADS, 0, st>>>(a, q);
+    const int nbands = (a.H + PRUNE_CELL - 1) / PRUNE_CELL;
+    prune_hist_kernel<<<dim3(nbands, a.K, a.B), HIST_THREADS, 0, st>>>(a, q);
+    prune_bound_kernel<<<dim3((a.hn + BOUND_HYPS - 1) / BOUND_HYPS, a.K, a.B), BOUND_THREADS, 0, st>>>(a, q);
     prune_plan_kernel<<<dim3(a.K, a.B), PLAN_THREADS, 0, st>>>(a, q);
-    cudaError_t e = launch_vote_list(a, q.list, q.len, PRUNE_M, st);
+    cudaError_t e = launch_vote_list(a, q.list, q.len, PRUNE_M, false, st);
     if (e != cudaSuccess) return e;
     prune_next_kernel<<<dim3(a.K, a.B), PLAN_THREADS, 0, st>>>(a, q);
-    return launch_vote_list(a, q.list + BK * a.hn, q.len + BK, a.hn - PRUNE_M, st);
+    return launch_vote_list(a, q.list + BK * a.hn, q.len + BK, a.hn - PRUNE_M, true, st);
 }
 
 } // namespace pvb

@@ -339,12 +339,12 @@ cudaError_t launch_vote(const VoteArgs &a, bool zero_counts, cudaStream_t st)
     return cudaGetLastError();
 }
 
-// Both passes of the pruned v3 vote use one shape: 128-hypothesis slices (4 per thread, WS = 1) whose four warps split the
-// 1024-pixel tile, so a pass scores its list in whole slices of 128 and CTAs past a list's end return at once.
-cudaError_t launch_vote_list(const VoteArgs &a, const int *list, const int *len, int max_len, cudaStream_t st)
+// The passes of the pruned v3 vote score (HPT*32)-hypothesis slices (WS = 1) whose four warps split the 1024-pixel tile,
+// so a pass scores its list in whole slices and CTAs past a list's end return at once.
+template <int HPT>
+static cudaError_t vote_list(const VoteArgs &a, const int *list, const int *len, int max_len, cudaStream_t st)
 {
-    constexpr int HPT = 4, NT = 128, TILE = 1024;
-    static_assert(HPT * 32 == PRUNE_M, "pass 1 is one slice");
+    constexpr int NT = 128, TILE = 1024;
     if (max_len <= 0) return cudaSuccess;
     VoteK p;
     p.a = a;
@@ -355,6 +355,13 @@ cudaError_t launch_vote_list(const VoteArgs &a, const int *list, const int *len,
     dim3 g((a.cap + TILE - 1) / TILE, a.K * slices, a.B);
     vote_kernel<HPT, NT, 8, TILE, 1><<<g, NT, 0, st>>>(p);
     return cudaGetLastError();
+}
+
+// Pass 1 is one 128-slice; pass 2 lists are mostly shorter than 128 (cfg-2: 0.13 hn on average), so it scores 64-slices
+cudaError_t launch_vote_list(const VoteArgs &a, const int *list, const int *len, int max_len, bool narrow, cudaStream_t st)
+{
+    static_assert(4 * 32 == PRUNE_M, "pass 1 is one slice");
+    return narrow ? vote_list<2>(a, list, len, max_len, st) : vote_list<4>(a, list, len, max_len, st);
 }
 
 // Multi-GPU exchange tail shared by the refit and the covariance kernel: one thread stores NV floats of unit `bk` into every

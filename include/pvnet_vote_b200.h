@@ -119,8 +119,9 @@ typedef struct pvb_layout {
     size_t win;      /* float2[B][K] winning hypothesis before the refit */
     size_t refit_partial; /* double[B][K][refit_splits][5] partial normal equations */
     size_t refit_ticket;  /* int32[B][K] arrival counters of the refit CTAs */
-    size_t prune_tiles;   /* int32[B][K][prune_ntiles][68] per 1024-pixel tile: bounding box (4 floats), then the
-                             inclusive prefix sums of a 64-bin histogram of the pixels' direction pseudo-angles */
+    size_t prune_cells;   /* int32[B][K][prune_ncells][68] per 32x32-pixel cell of the image (row-major): bounding box
+                             (4 floats) of the cell's pixels that can vote, then the inclusive prefix sums of a 128-bin
+                             histogram of their direction pseudo-angles as uint16 */
     size_t prune_key;     /* int32[B][K][hn] angular upper bound of each hypothesis's count, -1 if scored in pass 1 */
     size_t prune_list;    /* int32[2][B][K][hn] hypotheses scored by pass 1 / pass 2 of the pruned v3 vote */
     size_t prune_len;     /* int32[2][B][K] lengths of those lists */
@@ -128,7 +129,7 @@ typedef struct pvb_layout {
     int32_t nblocks; /* ceil(nwords/128) */
     int32_t capacity;
     int32_t refit_splits;
-    int32_t prune_ntiles; /* ceil(capacity/1024) */
+    int32_t prune_ncells; /* ceil(H/32) * ceil(W/32) */
 } pvb_layout;
 
 PVB_API int pvb_version(void);
