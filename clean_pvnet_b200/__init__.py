@@ -6,8 +6,12 @@ Public surface (same names/signatures as the reference):
     un_pnp.uncertainty_pnp / uncertainty_pnp_v2 (twins of lib/csrc/uncertainty_pnp/un_pnp_utils.py), uncertainty_pnp_batch,
     uncertainty_pnp_from_votes (the evaluator's whole un_pnp tail in one launch)
     parallel.ShardedVotingLayer (images sharded over the GPUs of one box, results exchanged over NVLink peer memory)
+    nn.find_nearest_point_idx (twin of lib/csrc/nn/nn_utils.py), nearest_point_idx, add_metric_batch (the evaluators'
+    ADD / ADD-S distance for n pose pairs), install_nn_as_reference_module
 """
 from . import _lib  # noqa: F401
+from . import nn  # noqa: F401
+from .nn import find_nearest_point_idx, nearest_point_idx, add_metric_batch, install_nn_as_reference_module  # noqa: F401
 from . import ransac_voting  # noqa: F401
 from . import ransac_voting_gpu  # noqa: F401
 from . import decode  # noqa: F401
@@ -28,4 +32,5 @@ __all__ = [
     "ransac_voting_layer_v3_host", "install_as_reference_module", "ransac_voting", "ransac_voting_gpu",
     "decode_keypoint", "uncertainty_pnp_weights", "un_pnp", "uncertainty_pnp_batch", "p3p_init_batch",
     "uncertainty_pnp_from_votes", "parallel",
+    "nn", "find_nearest_point_idx", "nearest_point_idx", "add_metric_batch", "install_nn_as_reference_module",
 ]

@@ -63,6 +63,10 @@ SIGNATURES = {
     "pvb_uncertainty_pnp_from_votes": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32,
                                                       ctypes.c_int64, ctypes.c_int64, ctypes.c_void_p, _vp]),
     "pvb_uncertainty_pnp_init": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, ctypes.c_int64, ctypes.c_int64, _vp]),
+    "pvb_nearest_point_workspace_bytes": (_sz, [_i32, _i32, _i32]),
+    "pvb_nearest_point_idx": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _sz, _vp]),
+    "pvb_add_metric_workspace_bytes": (_sz, [_i32, _i32, _i32]),
+    "pvb_add_metric": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _sz, _vp]),
     "pvb_read_status": (ctypes.c_int, [_dp, _vp, _vp]),
     "pvb_host_scratch_bytes": (_sz, [_dp, _i32]),
     "pvb_ransac_voting_v3_host": (ctypes.c_int, [_dp, _vp, _vp, _vp, _i32, ctypes.c_uint32, _vp, _sz, _vp]),

@@ -487,6 +487,68 @@ PVB_API int pvb_uncertainty_pnp_init(const double *pts2d, const double *pts3d, c
     return e == cudaSuccess ? PVB_OK : cuda_fail(e, "p3p init kernel");
 }
 
+namespace {
+
+// the workspace checks of the nearest-neighbour entries; `need` may be 0 (then NULL is fine)
+int nn_check_workspace(size_t need, const void *workspace, size_t workspace_bytes)
+{
+    if (!need) return PVB_OK;
+    if (!workspace || workspace_bytes < need)
+        return fail(PVB_ERR_WORKSPACE, "workspace too small: need %zu bytes, got %zu", need, workspace ? workspace_bytes : 0);
+    if (reinterpret_cast<uintptr_t>(workspace) & 255u) return fail(PVB_ERR_WORKSPACE, "workspace must be 256-byte aligned");
+    return PVB_OK;
+}
+
+// CTAs of the widest launch; the grid is one-dimensional
+bool nn_grid_fits(int b, int pn1, int pn2)
+{
+    const NnPlan p = nn_plan(b, pn1, pn2);
+    return (long long)b * p.nsplit * p.qchunks <= 0x7fffffffll;
+}
+
+} // namespace
+
+PVB_API size_t pvb_nearest_point_workspace_bytes(int32_t b, int32_t pn1, int32_t pn2)
+{
+    if (b <= 0 || pn1 < 0 || pn2 <= 0) return 0;
+    return nn_workspace_bytes(b, pn1, pn2);
+}
+
+PVB_API int pvb_nearest_point_idx(const float *ref, const float *que, int32_t *idxs, int32_t b, int32_t pn1, int32_t pn2,
+                                  int32_t dim, int32_t exclude_self, void *workspace, size_t workspace_bytes,
+                                  pvb_stream_t stream)
+{
+    if (b < 0 || pn1 < 0 || pn2 < 0) return fail(PVB_ERR_INVALID, "negative size (b=%d pn1=%d pn2=%d)", b, pn1, pn2);
+    if (dim != 2 && dim != 3) return fail(PVB_ERR_INVALID, "dim must be 2 or 3 (got %d)", dim);
+    if (b == 0 || pn2 == 0) return PVB_OK;
+    if (!que || !idxs || (pn1 > 0 && !ref)) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (!nn_grid_fits(b, pn1, pn2)) return fail(PVB_ERR_INVALID, "b * pn2 too large");
+    if (int rc = nn_check_workspace(nn_workspace_bytes(b, pn1, pn2), workspace, workspace_bytes)) return rc;
+    cudaError_t e = launch_nearest_point(ref, que, idxs, b, pn1, pn2, dim, exclude_self != 0, workspace,
+                                         static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "nearest point kernels");
+}
+
+PVB_API size_t pvb_add_metric_workspace_bytes(int32_t n, int32_t pn, int32_t syn)
+{
+    if (n <= 0 || pn < 0 || (syn != 0 && syn != 1)) return 0;
+    return add_metric_workspace_bytes(n, pn, syn, nullptr);
+}
+
+PVB_API int pvb_add_metric(const double *model, const double *pose_pred, const double *pose_gt, double *mean_dist, int32_t n,
+                           int32_t pn, int32_t syn, void *workspace, size_t workspace_bytes, pvb_stream_t stream)
+{
+    if (n < 0 || pn < 0) return fail(PVB_ERR_INVALID, "negative size (n=%d pn=%d)", n, pn);
+    if (syn != 0 && syn != 1) return fail(PVB_ERR_INVALID, "syn must be 0 or 1 (got %d)", syn);
+    if (n == 0) return PVB_OK;
+    if (!pose_pred || !pose_gt || !mean_dist || (pn > 0 && !model)) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (!nn_grid_fits(n, pn, pn)) return fail(PVB_ERR_INVALID, "n * pn too large");
+    if (int rc = nn_check_workspace(add_metric_workspace_bytes(n, pn, syn, nullptr), workspace, workspace_bytes)) return rc;
+    cudaError_t e = launch_add_metric(model, pose_pred, pose_gt, mean_dist, n, pn, syn != 0, workspace,
+                                      static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "add metric kernels");
+}
+
 PVB_API int pvb_read_status(const pvb_desc *d, const void *workspace, pvb_stream_t stream)
 {
     pvb_layout L;

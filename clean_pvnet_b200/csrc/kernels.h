@@ -130,6 +130,21 @@ struct PnpArgs {
 };
 cudaError_t launch_pnp_batch(const PnpArgs &a, cudaStream_t st);
 
+// exact nearest neighbour and ADD / ADD-S (nn.cu).  A problem's pn2 queries go to `qchunks` CTAs, its pn1 reference points
+// to `nsplit` slices of `slice` points; nsplit > 1 (chosen from the shapes when b * qchunks CTAs cannot fill the GPU)
+// merges the slices through a 64-bit key per query in the workspace.
+struct NnPlan { int qchunks, nsplit, slice; };
+NnPlan nn_plan(int b, int pn1, int pn2);
+size_t nn_workspace_bytes(int b, int pn1, int pn2);
+// ADD-S keys [n][pn] (split path only), then the per-CTA partial sums [n][qchunks] at *partial_offset
+size_t add_metric_workspace_bytes(int n, int pn, int syn, size_t *partial_offset);
+// ref [b][pn1][dim], que [b][pn2][dim] fp32 -> idxs [b][pn2]
+cudaError_t launch_nearest_point(const float *ref, const float *que, int *idxs, int b, int pn1, int pn2, int dim,
+                                 bool exclude_self, void *workspace, cudaStream_t st);
+// model [pn][3], pose_pred / pose_gt [n][3][4] fp64 -> mean_dist [n] fp64
+cudaError_t launch_add_metric(const double *model, const double *pose_pred, const double *pose_gt, double *mean_dist, int n,
+                              int pn, bool syn, void *workspace, cudaStream_t st);
+
 // twins of the reference extension on its own layouts
 cudaError_t launch_compat_generate(const float *direct, const float *coords, const int32_t *idxs, float *hyp,
                                    int tn, int vn, int hn, bool vanishing, cudaStream_t st);

@@ -24,7 +24,6 @@ Extra keyword-only arguments (all optional; the reference call sites never pass 
 """
 import math
 import sys
-import types
 
 import torch
 
@@ -376,27 +375,9 @@ def install_as_reference_module():
     the clean-pvnet checkout on sys.path), so `lib.config`, `lib.networks`, `lib.csrc.nn`, `lib.csrc.uncertainty_pnp`
     keep importing.  A stand-in package is created only for a parent that does not exist anywhere on sys.path
     (using this module outside a clean-pvnet checkout).  Idempotent."""
-    import importlib
-    import importlib.util
+    from ._dropin import reference_package
     this = sys.modules[__name__]
-    parent = None
-    for name in ("lib", "lib.csrc", "lib.csrc.ransac_voting"):
-        mod = sys.modules.get(name)
-        if mod is None:
-            try:
-                found = importlib.util.find_spec(name) is not None
-            except (ImportError, ValueError, AttributeError):
-                found = False
-            if found:
-                mod = importlib.import_module(name)        # the real package; errors inside it propagate
-            else:
-                mod = types.ModuleType(name)
-                mod.__path__ = []                            # genuinely absent: namespace stand-in
-                mod.__pvb_stand_in__ = True
-                sys.modules[name] = mod
-        if parent is not None and not hasattr(parent, name.rsplit(".", 1)[1]):
-            setattr(parent, name.rsplit(".", 1)[1], mod)
-        parent = mod
+    parent = reference_package("lib.csrc.ransac_voting")
     sys.modules["lib.csrc.ransac_voting.ransac_voting_gpu"] = this
     sys.modules["lib.csrc.ransac_voting.ransac_voting"] = _ext
     parent.ransac_voting_gpu = this

@@ -22,6 +22,11 @@
  *   un_pnp_utils.py:25-31  cv2.solvePnP(..., SOLVEPNP_P3P)        pvb_uncertainty_pnp_init
  *   evaluators/linemod/pvnet.py:118-130 + un_pnp_utils.py:6-57     pvb_uncertainty_pnp_from_votes (all three, one launch)
  *
+ *   and the one native extension of the evaluators (lib/csrc/nn, cffi, imported by both):
+ *   lib/csrc/nn/src/ext.h  findNearestPointIdxLauncher(...)       pvb_nearest_point_idx (device pointers, batched)
+ *   evaluators/linemod/pvnet.py:68-82  add_metric distance,
+ *   evaluators/tless_test/pvnet.py:107-117  adi_metric distance   pvb_add_metric (n pose pairs per call)
+ *
  * Conventions
  *   - plain C: device pointers, sizes, strides (in ELEMENTS), a CUDA stream
  *     handle.  No torch types.  All work is enqueued on `stream`; no entry
@@ -224,6 +229,36 @@ PVB_API int pvb_uncertainty_pnp_from_votes(const float *kpt_2d, const float *cov
 PVB_API int pvb_uncertainty_pnp_init(const double *pts2d, const double *pts3d, const double *wgt2d, const double *K,
                                      double *init_rt, int32_t n, int32_t pn, int64_t pts3d_stride, int64_t k_stride,
                                      pvb_stream_t stream);
+
+/* Exact brute-force nearest neighbour, the batched device twin of the reference's
+ * `findNearestPointIdxLauncher(ref_pts, que_pts, idxs, b, pn1, pn2, dim, exclude_self)` (lib/csrc/nn/src/ext.h,
+ * nearest_neighborhood.cu:48-163, which takes host pointers and allocates, copies and frees on every call).
+ *   ref device fp32 [b,pn1,dim], que device fp32 [b,pn2,dim], idxs device int32 [b,pn2]; dim 2 or 3.
+ *   idxs[i][q] = the first p (scan order) minimising the reference's fp32 squared distance ref[i][p] - que[i][q]
+ *   (exclude_self != 0: p != q), with its rounding; NaN / inf / FLT_MAX distances never win, and a query without any
+ *   other distance gets 0.  Bit-equal to the reference kernel (DESIGN.md section 8b).
+ *   workspace: pvb_nearest_point_workspace_bytes(b, pn1, pn2) bytes of 256-byte aligned device memory (0 bytes -- and
+ *   NULL allowed -- when b * pn2 fills the GPU or pn1 is too short to split).  b == 0 or pn2 == 0 is a no-op.
+ * Bad arguments (NULL tensors, dim not 2 or 3, negative sizes) return PVB_ERR_INVALID, a missing or short workspace
+ * PVB_ERR_WORKSPACE, both before any CUDA call. */
+PVB_API size_t pvb_nearest_point_workspace_bytes(int32_t b, int32_t pn1, int32_t pn2);
+PVB_API int pvb_nearest_point_idx(const float *ref, const float *que, int32_t *idxs, int32_t b, int32_t pn1, int32_t pn2,
+                                  int32_t dim, int32_t exclude_self, void *workspace, size_t workspace_bytes,
+                                  pvb_stream_t stream);
+
+/* The distance of the evaluators' ADD / ADD-S metric for n pose pairs in one call (Evaluator.add_metric,
+ * lib/evaluators/linemod/pvnet.py:68-82; T-LESS's adi_metric, tless_test/pvnet.py:107-117, is its caller expanding the
+ * (prediction, ground truth) pairs into the n rows):
+ *   pred = model @ R_pred.T + t_pred, target = model @ R_gt.T + t_gt in fp64;
+ *   syn != 0 (ADD-S): for every target point its nearest predicted point, found like pvb_nearest_point_idx on both clouds
+ *   rounded to fp32 (what nn_utils.find_nearest_point_idx hands the reference kernel); syn == 0 (ADD): the same point;
+ *   mean_dist[i] = mean over the points of |pred[idx] - target| in fp64.
+ *   model device fp64 [pn,3] (shared by all pairs), pose_pred / pose_gt device fp64 [n,3,4] ([R|t]), mean_dist device
+ *   fp64 [n].  The `< 0.1 * diameter` test stays with the caller.  pn == 0 gives NaN (the mean of nothing), n == 0 is a
+ *   no-op.  workspace: pvb_add_metric_workspace_bytes(n, pn, syn) bytes of 256-byte aligned device memory. */
+PVB_API size_t pvb_add_metric_workspace_bytes(int32_t n, int32_t pn, int32_t syn);
+PVB_API int pvb_add_metric(const double *model, const double *pose_pred, const double *pose_gt, double *mean_dist, int32_t n,
+                           int32_t pn, int32_t syn, void *workspace, size_t workspace_bytes, pvb_stream_t stream);
 
 /* Reads the sticky status word of a workspace (synchronises `stream`). */
 PVB_API int pvb_read_status(const pvb_desc *d, const void *workspace, pvb_stream_t stream);
