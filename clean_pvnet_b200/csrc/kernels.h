@@ -72,9 +72,11 @@ struct PruneArgs {
 bool prune_setup(const VoteArgs &a, PruneArgs &q);
 // cell histograms + bounds + pass 1 + pass 2; counts must be zeroed (launch_generate)
 cudaError_t launch_vote_pruned(const VoteArgs &a, const PruneArgs &q, cudaStream_t st);
-// the vote kernel over hypothesis lists: slot s of (b,k) scores hypothesis list[(b*K+k)*hn + s], s < len[b*K+k], in slices
-// of 128 hypotheses (`narrow`: 64)
-cudaError_t launch_vote_list(const VoteArgs &a, const int *list, const int *len, int max_len, bool narrow, cudaStream_t st);
+// Both passes score hypothesis lists: entry s of (b,k) is hypothesis list[(b*K+k)*hn + s], s < len[b*K+k] <= max_len.
+// Pass 2: vote_list_kernel, pixels in registers, one CTA per (tile, k, b) over the whole list, which costs its real length.
+cudaError_t launch_vote_list(const VoteArgs &a, const int *list, const int *len, int max_len, cudaStream_t st);
+// Pass 1: vote_kernel, hypotheses in registers, in slices of 128 entries
+cudaError_t launch_vote_list_slices(const VoteArgs &a, const int *list, const int *len, int max_len, cudaStream_t st);
 void set_vote_tuning(int variant);   // tooling: pixel-tile size per CTA
 void set_gather_tuning(int mode);    // tooling: gather access pattern (select.cu)
 // argmax + winner refit -> out_kpt [B][K][2], win [B][K].  The pixels of one (image,keypoint) are split

@@ -12,7 +12,7 @@
 //   prune_plan_kernel   (k, b):         the PRUNE_M largest bounds -> list 0 (pass 1)
 //   vote_kernel         list 0
 //   prune_next_kernel   (k, b):         L = best pass-1 count; {h not in pass 1 : B(h) >= L} -> list 1 (pass 2)
-//   vote_kernel         list 1
+//   vote_list_kernel    list 1
 #include <cmath>
 #include <math_constants.h>
 #include "common.cuh"
@@ -329,7 +329,8 @@ bool prune_setup(const VoteArgs &a, PruneArgs &q)
     // below PRUNE_MIN_UNITS (image, keypoint) pairs the full vote is short of a wave and latency bound: the extra
     // launches cost more than the skipped tests save (H100, B=1, K=9: 0.104 ms per call in full, 0.151 ms pruned)
     if ((long long)a.B * a.K < PRUNE_MIN_UNITS) return false;
-    if ((long long)a.K * ((a.hn + 63) / 64) > 65535) return false;     // grid.y of pass 2's 64-hypothesis slices
+    // the list passes launch grid.y = K (pass 2) and K * 1 slice (pass 1), inside this bound; tests/prune_twin.py states it
+    if ((long long)a.K * ((a.hn + 63) / 64) > 65535) return false;
     // theta' >= every angle at which the reference can still count a vote: its fp32 cosine is within 9u of the exact one
     // (DESIGN.md 4.1), so a vote needs cos > t - 9u; 64u and 1e-5 rad on top cover the rounding of the bound itself
     const double u = ldexp(1.0, -24);
@@ -348,10 +349,10 @@ cudaError_t launch_vote_pruned(const VoteArgs &a, const PruneArgs &q, cudaStream
     prune_hist_kernel<<<dim3(nbands, a.K, a.B), HIST_THREADS, 0, st>>>(a, q);
     prune_bound_kernel<<<dim3((a.hn + BOUND_HYPS - 1) / BOUND_HYPS, a.K, a.B), BOUND_THREADS, 0, st>>>(a, q);
     prune_plan_kernel<<<dim3(a.K, a.B), PLAN_THREADS, 0, st>>>(a, q);
-    cudaError_t e = launch_vote_list(a, q.list, q.len, PRUNE_M, false, st);
+    cudaError_t e = launch_vote_list_slices(a, q.list, q.len, PRUNE_M, st);
     if (e != cudaSuccess) return e;
     prune_next_kernel<<<dim3(a.K, a.B), PLAN_THREADS, 0, st>>>(a, q);
-    return launch_vote_list(a, q.list + BK * a.hn, q.len + BK, a.hn - PRUNE_M, true, st);
+    return launch_vote_list(a, q.list + BK * a.hn, q.len + BK, a.hn - PRUNE_M, st);
 }
 
 } // namespace pvb

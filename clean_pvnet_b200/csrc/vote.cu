@@ -100,6 +100,76 @@ __device__ __forceinline__ float cone_margin(const float4 ra, const float2 rb, f
     return ap - fabsf(pp);
 }
 
+// Loads a tile's n pixels, pixel i = threadIdx.x + r*NT to slot r (zeros past n), and returns the tile-local origin (ox, oy),
+// the centre of the tile's bounding box, with cmax = max over the tile of |cx-ox|+|cy-oy|.  The guard band scales with
+// S = |h-o|_1 + cmax, so a local origin keeps it tight.  Every thread of the CTA calls it.
+template <int NT, int PPT>
+__device__ __forceinline__ void load_tile(const float2 *dk, const float2 *xy, int n, float2 (&v)[PPT], float2 (&c)[PPT],
+                                          float (*s_box)[NT / 32], float &ox, float &oy, float &cmax)
+{
+    constexpr int NW = NT / 32;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    float x0 = CUDART_INF_F, x1 = -CUDART_INF_F, y0 = CUDART_INF_F, y1 = -CUDART_INF_F;
+#pragma unroll
+    for (int r = 0; r < PPT; ++r) {
+        const int i = tid + r * NT;
+        v[r] = make_float2(0.f, 0.f); c[r] = make_float2(0.f, 0.f);
+        if (i < n) {
+            v[r] = __ldg(dk + i); c[r] = __ldg(xy + i);
+            x0 = fminf(x0, c[r].x); x1 = fmaxf(x1, c[r].x); y0 = fminf(y0, c[r].y); y1 = fmaxf(y1, c[r].y);
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        x0 = fminf(x0, __shfl_xor_sync(0xffffffffu, x0, o)); x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, o));
+        y0 = fminf(y0, __shfl_xor_sync(0xffffffffu, y0, o)); y1 = fmaxf(y1, __shfl_xor_sync(0xffffffffu, y1, o));
+    }
+    if (lane == 0) { s_box[0][warp] = x0; s_box[1][warp] = x1; s_box[2][warp] = y0; s_box[3][warp] = y1; }
+    __syncthreads();
+#pragma unroll
+    for (int w = 0; w < NW; ++w) {
+        x0 = fminf(x0, s_box[0][w]); x1 = fmaxf(x1, s_box[1][w]); y0 = fminf(y0, s_box[2][w]); y1 = fmaxf(y1, s_box[3][w]);
+    }
+    ox = 0.5f * (x0 + x1); oy = 0.5f * (y0 + y1);
+    // half extents, padded against the rounding of ox/oy
+    cmax = (0.5f * (x1 - x0) + 0.5f * (y1 - y0)) * 1.000001f + 1e-3f;
+}
+
+// Cone record (A1, A2, A3, B1), (B2, B3) of pixel (v, c) relative to the tile origin.  `pixel` false (padding) and a pixel the
+// reference never lets vote give margin -1e30 against every hypothesis: negative, never inside a finite band.  A pixel outside
+// the domain of the error analysis gives margin 0, always inside the band, so the exact path decides every one of its tests.
+__device__ __forceinline__ void cone_record(bool pixel, float2 v, float2 c, float ox, float oy, float cmax, float kappa,
+                                            float4 &ra, float2 &rb)
+{
+    ra = make_float4(0.f, 0.f, -1e30f, 0.f);
+    rb = make_float2(0.f, 0.f);
+    if (!pixel) return;
+    const float n1 = __fsqrt_rn(__fmaf_rn(v.x, v.x, __fmul_rn(v.y, v.y)));   // the reference's norm1
+    const float cxc = c.x - ox, cyc = c.y - oy;
+    if (!(n1 > below_1e6())) {
+        // (double)norm1 < 1e-6 or NaN: the reference never votes for this pixel (.cu:121)
+    } else if (!(n1 < 1e18f) || !(fabsf(cxc) + fabsf(cyc) <= cmax)) {
+        ra.z = 0.f;
+    } else {
+        const float inv = 1.0f / n1;
+        const float ux = v.x * inv, uy = v.y * inv;
+        const float a1 = kappa * ux, a2 = kappa * uy;
+        ra.x = a1; ra.y = a2; ra.z = -fmaf(a1, cxc, a2 * cyc);
+        ra.w = -uy; rb.x = ux; rb.y = fmaf(uy, cxc, -(ux * cyc));
+    }
+}
+
+// Hypothesis q relative to the tile origin, (hxc, hyc), and its guard band dl.  Non-finite or huge: (0, 0, inf), so every
+// test of it takes the exact path.
+__device__ __forceinline__ float3 hyp_frame(float2 q, float ox, float oy, float cmax, const ConeParams &cone)
+{
+    float xc = q.x - ox, yc = q.y - oy;
+    const float S = fabsf(xc) + fabsf(yc) + cmax;
+    float d = fmaxf(cone.band * S, cone.floor);    // the floor binds only for tiles narrower than ~0.4 px
+    if (!(S <= 1e15f) || !(d < CUDART_INF_F)) { xc = 0.f; yc = 0.f; d = CUDART_INF_F; }
+    return make_float3(xc, yc, d);
+}
+
 // WS = warps that together hold one hypothesis slice (HPT*WS*32 hypotheses).  With fewer than 512 hypotheses per
 // keypoint the remaining NT/32/WS warp teams of the CTA split the tile's 16-pixel blocks between them, so every
 // thread still owns HPT hypotheses and the inner loop keeps its instruction mix.
@@ -125,7 +195,7 @@ vote_kernel(const VoteK p)
     const int *lst = p.list ? p.list + bk * a.hn : nullptr;
     const int n = min(VOTE_TILE, tn - t0);
     const int npad = (n + VOTE_BLOCK - 1) / VOTE_BLOCK * VOTE_BLOCK;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x, lane = tid & 31;
     const float kappa = p.cone.kappa, thresh = p.cone.thresh;
     const float2 *hyp = a.hyp + bk * a.hn;
     const float2 *xy = a.xy + (size_t)b * a.cap + t0;
@@ -133,58 +203,19 @@ vote_kernel(const VoteK p)
     const int team = tid / TEAM;
     const int hbase = slice * (TEAM * HPT) + (tid - team * TEAM);
 
-    // ---- stage 1: load this tile's pixels, bounding box -> tile-local origin for the fast path.
-    // The guard band scales with S = |h-o|_1 + max|c-o|_1, so a local origin keeps it tight.
+    // ---- stage 1: load this tile's pixels -> tile-local origin for the fast path
     float2 v[PPT], c[PPT];
-    float x0 = CUDART_INF_F, x1 = -CUDART_INF_F, y0 = CUDART_INF_F, y1 = -CUDART_INF_F;
-#pragma unroll
-    for (int r = 0; r < PPT; ++r) {
-        const int i = tid + r * NT;
-        v[r] = make_float2(0.f, 0.f); c[r] = make_float2(0.f, 0.f);
-        if (i < n) {
-            v[r] = __ldg(dk + i); c[r] = __ldg(xy + i);
-            x0 = fminf(x0, c[r].x); x1 = fmaxf(x1, c[r].x); y0 = fminf(y0, c[r].y); y1 = fmaxf(y1, c[r].y);
-        }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        x0 = fminf(x0, __shfl_xor_sync(0xffffffffu, x0, o)); x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, o));
-        y0 = fminf(y0, __shfl_xor_sync(0xffffffffu, y0, o)); y1 = fmaxf(y1, __shfl_xor_sync(0xffffffffu, y1, o));
-    }
-    if (lane == 0) { s_box[0][warp] = x0; s_box[1][warp] = x1; s_box[2][warp] = y0; s_box[3][warp] = y1; }
-    __syncthreads();
-#pragma unroll
-    for (int w = 0; w < NW; ++w) {
-        x0 = fminf(x0, s_box[0][w]); x1 = fmaxf(x1, s_box[1][w]); y0 = fminf(y0, s_box[2][w]); y1 = fmaxf(y1, s_box[3][w]);
-    }
-    const float ox = 0.5f * (x0 + x1), oy = 0.5f * (y0 + y1);
-    // max over the tile of |cx-ox|+|cy-oy| (half extents, padded against the rounding of ox/oy)
-    const float cmax = (0.5f * (x1 - x0) + 0.5f * (y1 - y0)) * 1.000001f + 1e-3f;
+    float ox, oy, cmax;
+    load_tile<NT, PPT>(dk, xy, n, v, c, s_box, ox, oy, cmax);
 
     // ---- stage 2: cone records
 #pragma unroll
     for (int r = 0; r < PPT; ++r) {
         const int i = tid + r * NT;
         if (i < npad) {
-            // pad record == "never votes": margin -1e30, negative, never inside a finite band
-            float4 ra = make_float4(0.f, 0.f, -1e30f, 0.f);
-            float2 rb = make_float2(0.f, 0.f);
-            if (i < n) {
-                const float n1 = __fsqrt_rn(__fmaf_rn(v[r].x, v[r].x, __fmul_rn(v[r].y, v[r].y)));   // the reference's norm1
-                const float cxc = c[r].x - ox, cyc = c[r].y - oy;
-                if (!(n1 > below_1e6())) {
-                    // (double)norm1 < 1e-6 or NaN: the reference never votes for this pixel (.cu:121)
-                } else if (!(n1 < 1e18f) || !(fabsf(cxc) + fabsf(cyc) <= cmax)) {
-                    // outside the domain of the error analysis: force the exact path (m == 0 < delta)
-                    ra.z = 0.f;
-                } else {
-                    const float inv = 1.0f / n1;
-                    const float ux = v[r].x * inv, uy = v[r].y * inv;
-                    const float a1 = kappa * ux, a2 = kappa * uy;
-                    ra.x = a1; ra.y = a2; ra.z = -fmaf(a1, cxc, a2 * cyc);
-                    ra.w = -uy; rb.x = ux; rb.y = fmaf(uy, cxc, -(ux * cyc));
-                }
-            }
+            float4 ra;
+            float2 rb;
+            cone_record(i < n, v[r], c[r], ox, oy, cmax, kappa, ra, rb);
             s_a[i] = ra; s_b[i] = rb;
         }
     }
@@ -196,11 +227,8 @@ vote_kernel(const VoteK p)
     for (int j = 0; j < HPT; ++j) {
         const int s = hbase + j * TEAM;
         const float2 q = (s < nh) ? hyp[lst ? __ldg(lst + s) : s] : make_float2(0.f, 0.f);
-        float xc = q.x - ox, yc = q.y - oy;
-        const float S = fabsf(xc) + fabsf(yc) + cmax;
-        float d = fmaxf(p.cone.band * S, p.cone.floor);    // the floor binds only for tiles narrower than ~0.4 px
-        if (!(S <= 1e15f) || !(d < CUDART_INF_F)) { xc = 0.f; yc = 0.f; d = CUDART_INF_F; }   // exact path only
-        hxc[j] = xc; hyc[j] = yc; dl[j] = d;
+        const float3 f = hyp_frame(q, ox, oy, cmax, p.cone);
+        hxc[j] = f.x; hyc[j] = f.y; dl[j] = f.z;
         neg[j] = 0;
     }
     __syncthreads();
@@ -339,12 +367,144 @@ cudaError_t launch_vote(const VoteArgs &a, bool zero_counts, cudaStream_t st)
     return cudaGetLastError();
 }
 
-// The passes of the pruned v3 vote score (HPT*32)-hypothesis slices (WS = 1) whose four warps split the 1024-pixel tile,
-// so a pass scores its list in whole slices and CTAs past a list's end return at once.
-template <int HPT>
-static cudaError_t vote_list(const VoteArgs &a, const int *list, const int *len, int max_len, cudaStream_t st)
+// The pruned v3 vote's list kernel: vote_kernel turned inside out.  A CTA owns one (image, keypoint, 1024-pixel tile) and
+// the whole list; every thread keeps LIST_PPT pixels as cone records in registers, and the list's hypotheses stream
+// past as broadcasts from shared memory, staged LIST_CHUNK at a time.  The loop runs over the list's real length, so a list
+// of 63 hypotheses costs 63, not a padded slice, and a tile's records are built once for the whole list: the lists of pass 2
+// have any length from 0 to hn - PRUNE_M.  Records, origin and guard band are vote_kernel's (load_tile, cone_record,
+// hyp_frame), and so is every count.  One CTA per tile and list builds the records once (H100, cfg-2 pass 2: 122 us, against
+// 137 us for one CTA per 64 entries and 140 us for two CTAs per list).  A copy of the records in shared memory serves the
+// rare exact path (122 us, against 145 us when the path rebuilds the records from v and c).  96 registers, no spills, 5 CTAs per SM.
+constexpr int LIST_NT = 128;
+constexpr int LIST_PPT = 8;                          // pixels per thread
+constexpr int LIST_TILE = LIST_NT * LIST_PPT;
+constexpr int LIST_CHUNK = LIST_NT;                  // list entries staged at a time, one per thread
+constexpr int LIST_U = 2;                            // hypotheses per loop iteration
+static_assert(LIST_CHUNK % LIST_U == 0 && LIST_U % 2 == 0, "");
+
+// Rare: re-tests this thread's pixels whose margin against hypothesis q falls inside its guard band with the reference's exact
+// operation sequence (fast verdict = sign bit of m) and returns the correction to the thread's count of non-inliers.  The
+// records come from the CTA's copy in shared memory, so the path indexes no register array and finds the pixels inside the
+// band with one load and 5 instructions each; padding (i >= n) stays "not an inlier".
+__device__ __forceinline__ int list_exact(const float4 q, const float4 *s_a, const float2 *s_b, const float2 *hyp, const float2 *dk,
+                                          const float2 *xy, int n, float thresh)
 {
-    constexpr int NT = 128, TILE = 1024;
+    const float2 hq = __ldg(hyp + __float_as_int(q.w));
+    int d = 0;
+    for (int i = threadIdx.x; i < n; i += LIST_NT) {
+        const float m = cone_margin(s_a[i], s_b[i], q.x, q.y);
+        if (fabsf(m) < q.z) {
+            const float2 vv = __ldg(dk + i), cc = __ldg(xy + i);
+            d += (vote_exact(vv.x, vv.y, cc.x, cc.y, hq.x, hq.y, thresh) ? 0 : 1) - (int)(__float_as_uint(m) >> 31);
+        }
+    }
+    return d;
+}
+
+__global__ void __launch_bounds__(LIST_NT, 5)
+vote_list_kernel(const VoteArgs a, const ConeParams cone, const int *__restrict__ list, const int *__restrict__ len)
+{
+    constexpr int NW = LIST_NT / 32;
+    __shared__ __align__(16) float4 s_a[LIST_TILE];     // the records again, for the exact path
+    __shared__ __align__(16) float2 s_b[LIST_TILE];
+    __shared__ __align__(16) float4 s_h[LIST_CHUNK];    // (hxc, hyc, dl, hypothesis index bits)
+    __shared__ unsigned s_tally[NW][LIST_CHUNK / 2];    // inliers per warp of entries 2i, 2i+1 (16-bit halves)
+    __shared__ float s_box[4][NW];
+    const int b = blockIdx.z;
+    const int k = blockIdx.y;
+    const int tn = min(a.tn[b], a.cap);
+    const int t0 = blockIdx.x * LIST_TILE;
+    const size_t bk = (size_t)b * a.K + k;
+    const int nh = __ldg(len + bk);
+    if (t0 >= tn || nh <= 0) return;
+    const int n = min(LIST_TILE, tn - t0);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int *lst = list + bk * a.hn;
+    const float2 *hyp = a.hyp + bk * a.hn;
+    const float2 *xy = a.xy + (size_t)b * a.cap + t0;
+    const float2 *dk = a.dirs + bk * a.cap + t0;
+
+    int h = 0;                                          // this thread's first list entry, loaded while the pixels are
+    float2 hq = make_float2(0.f, 0.f);
+    if (tid < nh) { h = __ldg(lst + tid); hq = hyp[h]; }
+    float4 ra[LIST_PPT];
+    float2 rb[LIST_PPT];
+    float ox, oy, cmax;
+    {
+        float2 v[LIST_PPT], c[LIST_PPT];
+        load_tile<LIST_NT, LIST_PPT>(dk, xy, n, v, c, s_box, ox, oy, cmax);
+#pragma unroll
+        for (int r = 0; r < LIST_PPT; ++r) {
+            cone_record(tid + r * LIST_NT < n, v[r], c[r], ox, oy, cmax, cone.kappa, ra[r], rb[r]);
+            s_a[tid + r * LIST_NT] = ra[r]; s_b[tid + r * LIST_NT] = rb[r];
+        }
+    }
+    unsigned *tally = s_tally[warp];
+    for (int c0 = 0; c0 < nh; c0 += LIST_CHUNK) {
+        const int ns = min(LIST_CHUNK, nh - c0);
+        if (c0 > 0 && tid < ns) { h = __ldg(lst + c0 + tid); hq = hyp[h]; }
+        if (tid < ns) {
+            const float3 f = hyp_frame(hq, ox, oy, cmax, cone);
+            s_h[tid] = make_float4(f.x, f.y, f.z, __int_as_float(h));
+        } else {
+            s_h[tid] = make_float4(0.f, 0.f, 0.f, 0.f);   // rounds the loop up to LIST_U: band 0 is never re-tested
+        }
+        __syncthreads();
+        for (int s = 0; s < ns; s += LIST_U) {
+            float4 q[LIST_U];
+            int neg[LIST_U];            // tests whose margin is negative (sign bit) = non-inliers, padding included
+            float mn[LIST_U];           // smallest |margin|
+            bool flag = false;
+#pragma unroll
+            for (int u = 0; u < LIST_U; ++u) {
+                q[u] = s_h[s + u];
+                neg[u] = 0;
+                mn[u] = CUDART_INF_F;
+#pragma unroll
+                for (int r = 0; r < LIST_PPT; ++r) {
+                    const float m = cone_margin(ra[r], rb[r], q[u].x, q[u].y);
+                    neg[u] += (int)(__float_as_uint(m) >> 31);
+                    mn[u] = fminf(mn[u], fabsf(m));
+                }
+                flag |= mn[u] < q[u].z;
+            }
+            if (flag) {
+#pragma unroll
+                for (int u = 0; u < LIST_U; ++u)
+                    if (mn[u] < q[u].z) neg[u] += list_exact(q[u], s_a, s_b, hyp, dk, xy, n, cone.thresh);
+            }
+            // a thread's tally is at most LIST_PPT, a warp's at most 256: two fit one 32-bit reduction
+#pragma unroll
+            for (int u = 0; u < LIST_U; u += 2) {
+                const unsigned t = __reduce_add_sync(0xffffffffu, (unsigned)(LIST_PPT - neg[u]) | ((unsigned)(LIST_PPT - neg[u + 1]) << 16));
+                if (lane == 0) tally[(s + u) / 2] = t;
+            }
+        }
+        __syncthreads();
+        if (tid < ns) {
+            int cnt = 0;
+#pragma unroll
+            for (int w = 0; w < NW; ++w) cnt += (int)((s_tally[w][tid / 2] >> (16 * (tid & 1))) & 0xffffu);
+            if (cnt) atomicAdd(a.counts + bk * a.hn + __float_as_int(s_h[tid].w), cnt);
+        }
+        // the next chunk's staging writes only this thread's s_h slot; s_tally is rewritten after the barrier that follows it
+    }
+}
+
+cudaError_t launch_vote_list(const VoteArgs &a, const int *list, const int *len, int max_len, cudaStream_t st)
+{
+    if (max_len <= 0) return cudaSuccess;
+    dim3 g((a.cap + LIST_TILE - 1) / LIST_TILE, a.K, a.B);
+    vote_list_kernel<<<g, LIST_NT, 0, st>>>(a, make_cone(a.thresh), list, len);
+    return cudaGetLastError();
+}
+
+// Pass 1: vote_kernel over a full list, in (HPT*32)-hypothesis slices (WS = 1) whose four warps split the 1024-pixel tile.
+// With a whole slice per list it scores faster than vote_list_kernel (H100, cfg-2: 192 against 238 us).
+cudaError_t launch_vote_list_slices(const VoteArgs &a, const int *list, const int *len, int max_len, cudaStream_t st)
+{
+    constexpr int HPT = 4, NT = 128, TILE = 1024;
+    static_assert(HPT * 32 == PRUNE_M, "pass 1 is one slice");
     if (max_len <= 0) return cudaSuccess;
     VoteK p;
     p.a = a;
@@ -355,13 +515,6 @@ static cudaError_t vote_list(const VoteArgs &a, const int *list, const int *len,
     dim3 g((a.cap + TILE - 1) / TILE, a.K * slices, a.B);
     vote_kernel<HPT, NT, 8, TILE, 1><<<g, NT, 0, st>>>(p);
     return cudaGetLastError();
-}
-
-// Pass 1 is one 128-slice; pass 2 lists are mostly shorter than 128 (cfg-2: 0.13 hn on average), so it scores 64-slices
-cudaError_t launch_vote_list(const VoteArgs &a, const int *list, const int *len, int max_len, bool narrow, cudaStream_t st)
-{
-    static_assert(4 * 32 == PRUNE_M, "pass 1 is one slice");
-    return narrow ? vote_list<2>(a, list, len, max_len, st) : vote_list<4>(a, list, len, max_len, st);
 }
 
 // Multi-GPU exchange tail shared by the refit and the covariance kernel: one thread stores NV floats of unit `bk` into every
