@@ -8,10 +8,14 @@ Public surface (same names/signatures as the reference):
     parallel.ShardedVotingLayer (images sharded over the GPUs of one box, results exchanged over NVLink peer memory)
     nn.find_nearest_point_idx (twin of lib/csrc/nn/nn_utils.py), nearest_point_idx, add_metric_batch (the evaluators'
     ADD / ADD-S distance for n pose pairs), install_nn_as_reference_module
+    metrics.pose_metrics_batch (projection_2d / cm_degree_5 distances), mask_iou_batch, linemod_scores (the evaluator's four
+    per-image flags for a batch)
 """
 from . import _lib  # noqa: F401
 from . import nn  # noqa: F401
 from .nn import find_nearest_point_idx, nearest_point_idx, add_metric_batch, install_nn_as_reference_module  # noqa: F401
+from . import metrics  # noqa: F401
+from .metrics import pose_metrics_batch, mask_iou_batch, linemod_scores  # noqa: F401
 from . import ransac_voting  # noqa: F401
 from . import ransac_voting_gpu  # noqa: F401
 from . import decode  # noqa: F401
@@ -33,4 +37,5 @@ __all__ = [
     "decode_keypoint", "uncertainty_pnp_weights", "un_pnp", "uncertainty_pnp_batch", "p3p_init_batch",
     "uncertainty_pnp_from_votes", "parallel",
     "nn", "find_nearest_point_idx", "nearest_point_idx", "add_metric_batch", "install_nn_as_reference_module",
+    "metrics", "pose_metrics_batch", "mask_iou_batch", "linemod_scores",
 ]

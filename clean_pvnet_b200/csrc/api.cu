@@ -549,6 +549,51 @@ PVB_API int pvb_add_metric(const double *model, const double *pose_pred, const d
     return e == cudaSuccess ? PVB_OK : cuda_fail(e, "add metric kernels");
 }
 
+PVB_API size_t pvb_pose_metrics_workspace_bytes(int32_t n, int32_t pn)
+{
+    if (n <= 0 || pn < 0) return 0;
+    return pose_metrics_workspace_bytes(n, pn);
+}
+
+PVB_API int pvb_pose_metrics(const double *model, const double *pose_pred, const double *pose_gt, const double *K,
+                             int64_t k_stride, double *proj2d, double *trans_cm, double *angle_deg, int32_t n, int32_t pn,
+                             void *workspace, size_t workspace_bytes, pvb_stream_t stream)
+{
+    if (n < 0 || pn < 0) return fail(PVB_ERR_INVALID, "negative size (n=%d pn=%d)", n, pn);
+    if (n == 0) return PVB_OK;
+    if (!pose_pred || !pose_gt || !K || !proj2d || !trans_cm || !angle_deg || (pn > 0 && !model))
+        return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (k_stride < 0) return fail(PVB_ERR_INVALID, "negative stride");
+    if (!nn_grid_fits(n, pn, pn)) return fail(PVB_ERR_INVALID, "n * pn too large");
+    if (int rc = nn_check_workspace(pose_metrics_workspace_bytes(n, pn), workspace, workspace_bytes)) return rc;
+    cudaError_t e = launch_pose_metrics(model, pose_pred, pose_gt, K, k_stride, proj2d, trans_cm, angle_deg, n, pn, workspace,
+                                        static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "pose metric kernels");
+}
+
+PVB_API int pvb_mask_iou(const void *pred, int32_t pred_dtype, const int64_t *pred_stride, const void *gt, int32_t gt_dtype,
+                         const int64_t *gt_stride, int64_t *inter, int64_t *uni, int32_t B, int32_t H, int32_t W,
+                         pvb_stream_t stream)
+{
+    if (B < 0 || H < 0 || W < 0) return fail(PVB_ERR_INVALID, "negative size (B=%d H=%d W=%d)", B, H, W);
+    for (int32_t dt : {pred_dtype, gt_dtype})
+        if (dt < PVB_MASK_U8 || dt > PVB_MASK_I64)
+            return fail(PVB_ERR_INVALID, "mask dtypes must be integer pvb_mask_dtypes (U8..I64), got %d and %d", pred_dtype,
+                        gt_dtype);
+    if (B == 0) return PVB_OK;
+    if (!pred_stride || !gt_stride) return fail(PVB_ERR_INVALID, "NULL stride array");
+    const long long HW = (long long)H * W;
+    if (!inter || !uni || (HW > 0 && (!pred || !gt))) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (HW > 0x7fffffffll) return fail(PVB_ERR_INVALID, "image too large (H*W >= 2^31)");
+    for (int i = 0; i < 3; ++i)
+        if (pred_stride[i] < 0 || gt_stride[i] < 0) return fail(PVB_ERR_INVALID, "negative stride");
+    const long long ps[3] = {pred_stride[0], pred_stride[1], pred_stride[2]};
+    const long long gs[3] = {gt_stride[0], gt_stride[1], gt_stride[2]};
+    cudaError_t e = launch_mask_iou(pred, pred_dtype, ps, gt, gt_dtype, gs, reinterpret_cast<long long *>(inter),
+                                    reinterpret_cast<long long *>(uni), B, H, W, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "mask iou kernel");
+}
+
 PVB_API int pvb_read_status(const pvb_desc *d, const void *workspace, pvb_stream_t stream)
 {
     pvb_layout L;

@@ -146,6 +146,16 @@ cudaError_t launch_nearest_point(const float *ref, const float *que, int *idxs, 
 // model [pn][3], pose_pred / pose_gt [n][3][4] fp64 -> mean_dist [n] fp64
 cudaError_t launch_add_metric(const double *model, const double *pose_pred, const double *pose_gt, double *mean_dist, int n,
                               int pn, bool syn, void *workspace, cudaStream_t st);
+// projection_2d / cm_degree_5 (nn.cu): the per-CTA partial sums [n][ceil(pn / 2048)] of the reprojection distances
+size_t pose_metrics_workspace_bytes(int n, int pn);
+// model [pn][3], pose_pred / pose_gt [n][3][4], K [3][3] at K + pair * k_stride, fp64 -> proj2d, trans_cm, angle_deg [n]
+cudaError_t launch_pose_metrics(const double *model, const double *pose_pred, const double *pose_gt, const double *K,
+                                long long k_stride, double *proj2d, double *trans_cm, double *angle_deg, int n, int pn,
+                                void *workspace, cudaStream_t st);
+// mask_iou (select.cu): inter[b] = sum(pred & gt), uni[b] = sum(pred | gt) over [B,H,W] masks of integer pvb_mask_dtypes
+// with strides ps / gs (elements); zeroes both outputs first
+cudaError_t launch_mask_iou(const void *pred, int pred_dtype, const long long *ps, const void *gt, int gt_dtype,
+                            const long long *gs, long long *inter, long long *uni, int B, int H, int W, cudaStream_t st);
 
 // twins of the reference extension on its own layouts
 cudaError_t launch_compat_generate(const float *direct, const float *coords, const int32_t *idxs, float *hyp,

@@ -1,5 +1,6 @@
 // nn.cu -- exact brute-force nearest neighbour (the twin of lib/csrc/nn/src/nearest_neighborhood.cu:48-117) and the
-// ADD / ADD-S distance of lib/evaluators/linemod/pvnet.py:68-82 (tless_test/pvnet.py:107-117) built on it.
+// ADD / ADD-S distance of lib/evaluators/linemod/pvnet.py:68-82 (tless_test/pvnet.py:107-117) built on it, and the
+// evaluators' other two pose metrics, projection_2d and cm_degree_5 (:59-66, :84-94), on the same transform.
 //
 // The reference predicate, read from the PTX that `nvcc -O2 -arch=sm_52` (its setup.py) emits for the reference source:
 //   d? = RN(ref.? - que.?),  3-D: dist = fma(dz, dz, fma(dx, dx, RN(dy*dy))),  2-D: dist = fma(dx, dx, RN(dy*dy))
@@ -278,15 +279,93 @@ add_dist_kernel(AddArgs a)
     add_block_sum(s, a.partial + (size_t)pair * a.plan.qchunks + qc);
 }
 
+// the sum of one pair's per-CTA partials in a fixed order (on every lane of the calling warp)
+__device__ __forceinline__ double pair_partial_sum(const double *partial, int pair, int qchunks, int lane)
+{
+    double s = 0.0;
+    for (int c = lane; c < qchunks; c += 32) s += partial[(size_t)pair * qchunks + c];
+    return warp_sum(s);
+}
+
 // one warp per pair: mean = (sum of the partials, fixed order) / pn  (pn = 0 gives NaN, like np.mean of nothing)
 __global__ void add_mean_kernel(const double *partial, double *mean, int n, int qchunks, int pn)
 {
     const int pair = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (pair >= n) return;
-    double s = 0.0;
-    for (int c = lane; c < qchunks; c += 32) s += partial[(size_t)pair * qchunks + c];
-    s = warp_sum(s);
+    const double s = pair_partial_sum(partial, pair, qchunks, lane);
     if (lane == 0) mean[pair] = s / (double)pn;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// projection_2d and cm_degree_5 of n pose pairs (Evaluator.projection_2d / cm_degree_5_metric, linemod/pvnet.py:59-66 and
+// :84-94, on pvnet_pose_utils.project / cm_degree_5, pvnet_pose_utils.py:41-60), fp64:
+//   uv = ((model @ R.T + t) @ K.T)[:, :2] / z                   both poses, every product and sum rounded on its own
+//   proj2d = mean_i |uv_pred_i - uv_gt_i|                       z <= 0 gives what IEEE division gives (+-inf, NaN)
+//   trans_cm = |t_pred - t_gt| * 100
+//   trace = trace(R_pred @ R_gt.T); trace = trace if trace <= 3 else 3; trace = trace if trace >= -1 else -1
+//   angle_deg = rad2deg(arccos((trace - 1) / 2))                a NaN trace becomes 3, i.e. 0 degrees
+// proj_dist_kernel has add_dist_kernel's grid and per-CTA partial sums; pose_final_kernel adds them like add_mean_kernel
+// and computes the two pose distances, so a pair's three outputs do not depend on the batch or on scheduling.
+// ---------------------------------------------------------------------------------------------------------------------
+
+// uv of one camera-frame point: (x, y, z) @ K.T in the dot product's summation order, then divided by its z
+__device__ __forceinline__ void project_point(const double *K, double x, double y, double z, double &u, double &v)
+{
+    const double X = __dadd_rn(__dadd_rn(__dmul_rn(x, K[0]), __dmul_rn(y, K[1])), __dmul_rn(z, K[2]));
+    const double Y = __dadd_rn(__dadd_rn(__dmul_rn(x, K[3]), __dmul_rn(y, K[4])), __dmul_rn(z, K[5]));
+    const double Z = __dadd_rn(__dadd_rn(__dmul_rn(x, K[6]), __dmul_rn(y, K[7])), __dmul_rn(z, K[8]));
+    u = __ddiv_rn(X, Z);
+    v = __ddiv_rn(Y, Z);
+}
+
+// K of pair p at K + p * k_stride (0: shared)
+__global__ void __launch_bounds__(NN_THREADS, NN_MIN_CTAS)
+proj_dist_kernel(AddArgs a, const double *K, long long k_stride)
+{
+    __shared__ double s_pose[2][12];
+    __shared__ double s_K[9];
+    const int pair = blockIdx.x / a.plan.qchunks, qc = blockIdx.x % a.plan.qchunks;
+    if (threadIdx.x < 9) s_K[threadIdx.x] = K[(size_t)pair * k_stride + threadIdx.x];
+    load_poses(a, pair, s_pose);                          // its barrier also publishes s_K
+    double s = 0.0;
+#pragma unroll
+    for (int q = 0; q < NN_Q; ++q) {
+        const int i = qc * NN_QPB + q * NN_THREADS + (int)threadIdx.x;
+        if (i >= a.pn) continue;
+        double px, py, pz, gx, gy, gz, pu, pv, gu, gv;
+        pose_apply(s_pose[0], a.model + (size_t)i * 3, px, py, pz);
+        pose_apply(s_pose[1], a.model + (size_t)i * 3, gx, gy, gz);
+        project_point(s_K, px, py, pz, pu, pv);
+        project_point(s_K, gx, gy, gz, gu, gv);
+        const double du = __dsub_rn(pu, gu), dv = __dsub_rn(pv, gv);
+        s += __dsqrt_rn(__dadd_rn(__dmul_rn(du, du), __dmul_rn(dv, dv)));
+    }
+    add_block_sum(s, a.partial + (size_t)pair * a.plan.qchunks + qc);
+}
+
+// one warp per pair: proj2d from the partials (pn = 0 gives NaN), trans_cm and angle_deg from the two poses
+__global__ void pose_final_kernel(const double *partial, const double *pose_pred, const double *pose_gt, double *proj2d,
+                                  double *trans_cm, double *angle_deg, int n, int qchunks, int pn)
+{
+    const int pair = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (pair >= n) return;
+    const double s = pair_partial_sum(partial, pair, qchunks, lane);
+    if (lane != 0) return;
+    proj2d[pair] = s / (double)pn;
+    const double *P = pose_pred + (size_t)pair * 12, *G = pose_gt + (size_t)pair * 12;
+    const double d0 = __dsub_rn(P[3], G[3]), d1 = __dsub_rn(P[7], G[7]), d2 = __dsub_rn(P[11], G[11]);
+    const double sq = __dadd_rn(__dadd_rn(__dmul_rn(d0, d0), __dmul_rn(d1, d1)), __dmul_rn(d2, d2));
+    trans_cm[pair] = __dmul_rn(__dsqrt_rn(sq), 100.0);
+    double tr = 0.0;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {                         // (R_pred @ R_gt.T)[r][r] = row r of R_pred . row r of R_gt
+        const double *p = P + 4 * r, *g = G + 4 * r;
+        const double drr = __dadd_rn(__dadd_rn(__dmul_rn(p[0], g[0]), __dmul_rn(p[1], g[1])), __dmul_rn(p[2], g[2]));
+        tr = r == 0 ? drr : __dadd_rn(tr, drr);
+    }
+    tr = tr <= 3.0 ? tr : 3.0;                            // the reference's comparisons, which send NaN to 3
+    tr = tr >= -1.0 ? tr : -1.0;
+    angle_deg[pair] = __dmul_rn(acos(__ddiv_rn(__dsub_rn(tr, 1.0), 2.0)), 180.0 / 3.14159265358979323846);
 }
 
 } // namespace
@@ -320,6 +399,11 @@ size_t add_metric_workspace_bytes(int n, int pn, int syn, size_t *partial_offset
     const size_t keys = syn && p.nsplit > 1 ? ((size_t)n * pn * sizeof(unsigned long long) + 255) / 256 * 256 : 0;
     if (partial_offset) *partial_offset = keys;
     return keys + (size_t)n * p.qchunks * sizeof(double);
+}
+
+size_t pose_metrics_workspace_bytes(int n, int pn)
+{
+    return (size_t)n * ((pn + NN_QPB - 1) / NN_QPB) * sizeof(double);
 }
 
 cudaError_t launch_nearest_point(const float *ref, const float *que, int *idxs, int b, int pn1, int pn2, int dim,
@@ -368,6 +452,21 @@ cudaError_t launch_add_metric(const double *model, const double *pose_pred, cons
         }
     }
     add_mean_kernel<<<(n + 7) / 8, 256, 0, st>>>(a.partial, mean_dist, n, a.plan.qchunks, pn);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_pose_metrics(const double *model, const double *pose_pred, const double *pose_gt, const double *K,
+                                long long k_stride, double *proj2d, double *trans_cm, double *angle_deg, int n, int pn,
+                                void *workspace, cudaStream_t st)
+{
+    if (n <= 0) return cudaSuccess;
+    AddArgs a = {};
+    a.model = model; a.pose_pred = pose_pred; a.pose_gt = pose_gt; a.pn = pn;
+    a.plan.qchunks = (pn + NN_QPB - 1) / NN_QPB; a.plan.nsplit = 1; a.plan.slice = pn;
+    a.partial = static_cast<double *>(workspace);
+    if (pn > 0) proj_dist_kernel<<<(unsigned)((size_t)n * a.plan.qchunks), NN_THREADS, 0, st>>>(a, K, k_stride);
+    pose_final_kernel<<<(n + 7) / 8, 256, 0, st>>>(a.partial, pose_pred, pose_gt, proj2d, trans_cm, angle_deg, n,
+                                                  a.plan.qchunks, pn);
     return cudaGetLastError();
 }
 

@@ -14,6 +14,8 @@
 //
 // Both kernels are HBM/latency bound: the mask is read exactly once (mask_bits), the bitmap (1/256 of an int64 mask)
 // is what the second pass touches, and the vertex field is read only at selected pixels.
+//
+// The evaluator's mask_iou (mask_iou_kernel, at the end) streams a predicted and a ground-truth mask with the same loads.
 #include <atomic>
 #include "common.cuh"
 #include "kernels.h"
@@ -444,6 +446,141 @@ cudaError_t launch_select(const SelectArgs &a, cudaStream_t st)
                                                   make_uint2((uint32_t)a.seed, (uint32_t)(a.seed >> 32)), a.tag_sel, a.img_base,
                                                   (a.rowwise_gather || gmode == 2) ? 1 : 0);
     return cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// mask_iou of the LINEMOD evaluator (lib/evaluators/linemod/pvnet.py:96-100) for B images:
+//   inter[b] = sum(pred & gt), uni[b] = sum(pred | gt)
+// It sums the VALUES of the bitwise ops, not pixel counts.  numpy promotes both operands to a common integer type; here
+// both are widened to int64 by value (sign-extended if signed, zero-extended if not), which gives the same value, because
+// the bits above a narrower promoted result are copies of its top bit in both operands.  The sums are exact modulo 2^64
+// like numpy's int64 sum, so the atomics cannot change the result.
+// A warp takes IOU_TILE elements at a time.  When both images are contiguous and 16-byte aligned, each operand's tile is
+// staged in shared memory with 16-byte evict-first loads (sizeof(T) of them per lane, consecutive lanes on consecutive
+// 16 bytes) whatever the two element sizes are; then lane l combines elements l, l + 32, ...  Strided views and the last,
+// partial tile of an image are read element by element in the same order.
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int IOU_WARPS = 4;
+constexpr int IOU_TILE = 32 * 16;                // elements per warp tile: 16 per lane
+
+__device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v)
+{
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+template <typename TP, typename TG>
+__device__ __forceinline__ void iou_add(TP p, TG g, unsigned long long &si, unsigned long long &su)
+{
+    const long long a = (long long)p, c = (long long)g;
+    si += (unsigned long long)(a & c);
+    su += (unsigned long long)(a | c);
+}
+
+template <typename TP, typename TG>
+__global__ void __launch_bounds__(IOU_WARPS * 32)
+mask_iou_kernel(const TP *__restrict__ pred, long long psb, long long psy, long long psx, const TG *__restrict__ gt,
+                long long gsb, long long gsy, long long gsx, int B, int H, int W, unsigned long long *__restrict__ inter,
+                unsigned long long *__restrict__ uni)
+{
+    __shared__ uint4 s_p[IOU_WARPS][IOU_TILE * sizeof(TP) / 16];
+    __shared__ uint4 s_g[IOU_WARPS][IOU_TILE * sizeof(TG) / 16];
+    __shared__ unsigned long long s_red[2][IOU_WARPS];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int HW = H * W, ntiles = (HW + IOU_TILE - 1) / IOU_TILE;
+    const bool contig = psx == 1 && psy == W && gsx == 1 && gsy == W;
+    for (int b = blockIdx.y; b < B; b += gridDim.y) {
+        const TP *pb = pred + (long long)b * psb;
+        const TG *gb = gt + (long long)b * gsb;
+        const bool vec = contig && ((reinterpret_cast<uintptr_t>(pb) | reinterpret_cast<uintptr_t>(gb)) & 15u) == 0;
+        unsigned long long si = 0, su = 0;
+        for (int t = blockIdx.x * IOU_WARPS + warp; t < ntiles; t += gridDim.x * IOU_WARPS) {
+            const int e0 = t * IOU_TILE;
+            if (vec && e0 + IOU_TILE <= HW) {
+                const uint4 *qp = reinterpret_cast<const uint4 *>(pb + e0), *qg = reinterpret_cast<const uint4 *>(gb + e0);
+                uint4 vp[sizeof(TP)], vg[sizeof(TG)];
+#pragma unroll
+                for (int j = 0; j < (int)sizeof(TP); ++j) vp[j] = ld_stream16(qp + j * 32 + lane);
+#pragma unroll
+                for (int j = 0; j < (int)sizeof(TG); ++j) vg[j] = ld_stream16(qg + j * 32 + lane);
+#pragma unroll
+                for (int j = 0; j < (int)sizeof(TP); ++j) s_p[warp][j * 32 + lane] = vp[j];
+#pragma unroll
+                for (int j = 0; j < (int)sizeof(TG); ++j) s_g[warp][j * 32 + lane] = vg[j];
+                __syncwarp();
+                const TP *sp = reinterpret_cast<const TP *>(s_p[warp]);
+                const TG *sg = reinterpret_cast<const TG *>(s_g[warp]);
+#pragma unroll
+                for (int k = 0; k < IOU_TILE / 32; ++k) iou_add(sp[k * 32 + lane], sg[k * 32 + lane], si, su);
+                __syncwarp();                            // read before the next tile overwrites it
+            } else {
+#pragma unroll 4
+                for (int k = 0; k < IOU_TILE / 32; ++k) {
+                    const int e = e0 + k * 32 + lane;
+                    if (e >= HW) break;
+                    const int y = e / W, x = e - y * W;
+                    iou_add(__ldg(pb + y * psy + x * psx), __ldg(gb + y * gsy + x * gsx), si, su);
+                }
+            }
+        }
+        si = warp_sum_u64(si);
+        su = warp_sum_u64(su);
+        if (lane == 0) { s_red[0][warp] = si; s_red[1][warp] = su; }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            si = su = 0;
+#pragma unroll
+            for (int w = 0; w < IOU_WARPS; ++w) { si += s_red[0][w]; su += s_red[1][w]; }
+            if (si) atomicAdd(inter + b, si);
+            if (su) atomicAdd(uni + b, su);
+        }
+        __syncthreads();                                 // s_red is reused by the next image
+    }
+}
+
+template <typename TP, typename TG>
+void launch_mask_iou_typed(const void *pred, const long long *ps, const void *gt, const long long *gs, long long *inter,
+                           long long *uni, int B, int H, int W, cudaStream_t st)
+{
+    const int ntiles = (int)(((long long)H * W + IOU_TILE - 1) / IOU_TILE);
+    const dim3 grid((unsigned)((ntiles + IOU_WARPS - 1) / IOU_WARPS), (unsigned)(B < 65535 ? B : 65535));
+    mask_iou_kernel<TP, TG><<<grid, IOU_WARPS * 32, 0, st>>>(
+        static_cast<const TP *>(pred), ps[0], ps[1], ps[2], static_cast<const TG *>(gt), gs[0], gs[1], gs[2], B, H, W,
+        reinterpret_cast<unsigned long long *>(inter), reinterpret_cast<unsigned long long *>(uni));
+}
+
+template <typename TP>
+bool launch_mask_iou_gt(const void *pred, const long long *ps, const void *gt, int gt_dtype, const long long *gs,
+                        long long *inter, long long *uni, int B, int H, int W, cudaStream_t st)
+{
+    switch (gt_dtype) {
+    case PVB_MASK_U8: launch_mask_iou_typed<TP, uint8_t>(pred, ps, gt, gs, inter, uni, B, H, W, st); return true;
+    case PVB_MASK_I8: launch_mask_iou_typed<TP, int8_t>(pred, ps, gt, gs, inter, uni, B, H, W, st); return true;
+    case PVB_MASK_I16: launch_mask_iou_typed<TP, int16_t>(pred, ps, gt, gs, inter, uni, B, H, W, st); return true;
+    case PVB_MASK_I32: launch_mask_iou_typed<TP, int32_t>(pred, ps, gt, gs, inter, uni, B, H, W, st); return true;
+    case PVB_MASK_I64: launch_mask_iou_typed<TP, long long>(pred, ps, gt, gs, inter, uni, B, H, W, st); return true;
+    default: return false;
+    }
+}
+
+cudaError_t launch_mask_iou(const void *pred, int pred_dtype, const long long *ps, const void *gt, int gt_dtype,
+                            const long long *gs, long long *inter, long long *uni, int B, int H, int W, cudaStream_t st)
+{
+    if (B <= 0) return cudaSuccess;
+    cudaError_t e = cudaMemsetAsync(inter, 0, (size_t)B * sizeof(long long), st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(uni, 0, (size_t)B * sizeof(long long), st);
+    if (e != cudaSuccess || (long long)H * W == 0) return e;
+    bool ok = false;
+    switch (pred_dtype) {
+    case PVB_MASK_U8: ok = launch_mask_iou_gt<uint8_t>(pred, ps, gt, gt_dtype, gs, inter, uni, B, H, W, st); break;
+    case PVB_MASK_I8: ok = launch_mask_iou_gt<int8_t>(pred, ps, gt, gt_dtype, gs, inter, uni, B, H, W, st); break;
+    case PVB_MASK_I16: ok = launch_mask_iou_gt<int16_t>(pred, ps, gt, gt_dtype, gs, inter, uni, B, H, W, st); break;
+    case PVB_MASK_I32: ok = launch_mask_iou_gt<int32_t>(pred, ps, gt, gt_dtype, gs, inter, uni, B, H, W, st); break;
+    case PVB_MASK_I64: ok = launch_mask_iou_gt<long long>(pred, ps, gt, gt_dtype, gs, inter, uni, B, H, W, st); break;
+    default: break;
+    }
+    return ok ? cudaGetLastError() : cudaErrorInvalidValue;
 }
 
 } // namespace pvb

@@ -27,6 +27,12 @@
  *   evaluators/linemod/pvnet.py:68-82  add_metric distance,
  *   evaluators/tless_test/pvnet.py:107-117  adi_metric distance   pvb_add_metric (n pose pairs per call)
  *
+ *   and the evaluators' other per-image metrics:
+ *   evaluators/linemod/pvnet.py:59-66  projection_2d,
+ *   evaluators/linemod/pvnet.py:84-94  cm_degree_5_metric,
+ *   evaluators/tless_test/pvnet.py:119-125  cm_degree_5_metric     pvb_pose_metrics (n pose pairs per call)
+ *   evaluators/linemod/pvnet.py:96-100  mask_iou                   pvb_mask_iou (B images per call)
+ *
  * Conventions
  *   - plain C: device pointers, sizes, strides (in ELEMENTS), a CUDA stream
  *     handle.  No torch types.  All work is enqueued on `stream`; no entry
@@ -259,6 +265,43 @@ PVB_API int pvb_nearest_point_idx(const float *ref, const float *que, int32_t *i
 PVB_API size_t pvb_add_metric_workspace_bytes(int32_t n, int32_t pn, int32_t syn);
 PVB_API int pvb_add_metric(const double *model, const double *pose_pred, const double *pose_gt, double *mean_dist, int32_t n,
                            int32_t pn, int32_t syn, void *workspace, size_t workspace_bytes, pvb_stream_t stream);
+
+/* projection_2d + cm_degree_5 of the LINEMOD / T-LESS evaluators for n (prediction, ground truth) pose pairs
+ * (Evaluator.projection_2d, lib/evaluators/linemod/pvnet.py:59-66, on pvnet_pose_utils.project, pvnet_pose_utils.py:41-50;
+ * cm_degree_5_metric, linemod/pvnet.py:84-94 and pvnet_pose_utils.cm_degree_5:53-60), in fp64 with every product and sum
+ * rounded on its own:
+ *   uv = ((model @ R.T + t) @ K.T)[:, :2] / z for both poses;  proj2d[i] = mean over the points of |uv_pred - uv_gt|
+ *   (z <= 0 gives what IEEE division gives; pn == 0 gives NaN, the mean of nothing)
+ *   trans_cm[i] = |t_pred - t_gt| * 100
+ *   angle_deg[i] = rad2deg(arccos((trace - 1) / 2)), trace = trace(R_pred R_gt^T) clamped like the reference:
+ *   `trace if trace <= 3 else 3`, then `trace if trace >= -1 else -1`, so a NaN trace gives 0 degrees.
+ *   model device fp64 [pn,3] (shared by all pairs), pose_pred / pose_gt device fp64 [n,3,4] ([R|t]), K device fp64 [3,3]
+ *   row-major for pair i at K + i * k_stride (in doubles; 0 = one K for all), outputs device fp64 [n].  The thresholds
+ *   (< 5 pixels; < 5 cm and < 5 degrees) stay with the caller.  T-LESS's any-of-all-pairs cm_degree_5_metric
+ *   (tless_test/pvnet.py:119-125) is the caller expanding the (prediction, ground truth) pairs into the n rows.
+ *   A pair's outputs do not depend on the other pairs.  workspace: pvb_pose_metrics_workspace_bytes(n, pn) bytes of
+ *   256-byte aligned device memory (0 -- and NULL allowed -- when pn == 0).  n == 0 is a no-op.
+ * Bad arguments return PVB_ERR_INVALID, a missing or short workspace PVB_ERR_WORKSPACE, both before any CUDA call. */
+PVB_API size_t pvb_pose_metrics_workspace_bytes(int32_t n, int32_t pn);
+PVB_API int pvb_pose_metrics(const double *model, const double *pose_pred, const double *pose_gt, const double *K,
+                             int64_t k_stride, double *proj2d, double *trans_cm, double *angle_deg, int32_t n, int32_t pn,
+                             void *workspace, size_t workspace_bytes, pvb_stream_t stream);
+
+/* mask_iou of the LINEMOD evaluator (lib/evaluators/linemod/pvnet.py:96-100) for B images:
+ *   inter[b] = sum (pred & gt), uni[b] = sum (pred | gt)
+ * the sums of the VALUES of the bitwise ops, as numpy computes them (with more than two classes, 2 & 1 = 0 and 2 | 1 = 3);
+ * both operands are widened to int64 by value, and the int64 sums are exact (modulo 2^64, like numpy's).
+ *   pred, gt  device [B,H,W] with element strides pred_stride / gt_stride (HOST int64[3]); pred_dtype / gt_dtype are
+ *             integer pvb_mask_dtypes (U8, also for bool, I8, I16, I32, I64); F32 / F64 are rejected, as numpy's `&`
+ *             rejects floats.  The evaluator's pair, an int64 prediction and a uint8 ground truth, both contiguous, is
+ *             streamed with 16-byte loads.
+ *   inter, uni device int64 [B], zeroed by the call itself in stream order (no workspace).  iou = inter / uni is the
+ *   caller's (0 / 0 is NaN, as in numpy).  B == 0 is a no-op.
+ * Bad arguments (negative sizes, NULL tensors or stride arrays, negative strides, other dtypes, H*W >= 2^31) return
+ * PVB_ERR_INVALID before any CUDA call. */
+PVB_API int pvb_mask_iou(const void *pred, int32_t pred_dtype, const int64_t *pred_stride, const void *gt, int32_t gt_dtype,
+                         const int64_t *gt_stride, int64_t *inter, int64_t *uni, int32_t B, int32_t H, int32_t W,
+                         pvb_stream_t stream);
 
 /* Reads the sticky status word of a workspace (synchronises `stream`). */
 PVB_API int pvb_read_status(const pvb_desc *d, const void *workspace, pvb_stream_t stream);
