@@ -10,6 +10,8 @@ Public surface (same names/signatures as the reference):
     ADD / ADD-S distance for n pose pairs), install_nn_as_reference_module
     metrics.pose_metrics_batch (projection_2d / cm_degree_5 distances), mask_iou_batch, linemod_scores (the evaluator's four
     per-image flags for a batch)
+    pose.pnp (twin of lib/utils/pvnet/pvnet_pose_utils.py's cv2.solvePnP ITERATIVE step), pnp_batch (n problems, one launch:
+    the pose step of the default un_pnp=False path)
 """
 from . import _lib  # noqa: F401
 from . import nn  # noqa: F401
@@ -23,6 +25,8 @@ from . import parallel  # noqa: F401
 from .decode import decode_keypoint, uncertainty_pnp_weights  # noqa: F401
 from . import uncertainty_pnp as un_pnp  # noqa: F401
 from .uncertainty_pnp import uncertainty_pnp_batch, p3p_init_batch, uncertainty_pnp_from_votes  # noqa: F401
+from . import pose  # noqa: F401
+from .pose import pnp_batch  # noqa: F401
 from .ransac_voting_gpu import (  # noqa: F401
     estimate_voting_distribution_with_mean,
     ransac_voting_layer,
@@ -35,7 +39,7 @@ __all__ = [
     "ransac_voting_layer", "ransac_voting_layer_v3", "estimate_voting_distribution_with_mean",
     "ransac_voting_layer_v3_host", "install_as_reference_module", "ransac_voting", "ransac_voting_gpu",
     "decode_keypoint", "uncertainty_pnp_weights", "un_pnp", "uncertainty_pnp_batch", "p3p_init_batch",
-    "uncertainty_pnp_from_votes", "parallel",
+    "uncertainty_pnp_from_votes", "pose", "pnp_batch", "parallel",
     "nn", "find_nearest_point_idx", "nearest_point_idx", "add_metric_batch", "install_nn_as_reference_module",
     "metrics", "pose_metrics_batch", "mask_iou_batch", "linemod_scores",
 ]

@@ -14,6 +14,7 @@ PVB_HOST_STAGE_VERTEX, PVB_HOST_INPLACE_MASK = 2, 4
 PVB_IPC_HANDLE_BYTES = 64
 (PVB_MASK_U8, PVB_MASK_I8, PVB_MASK_I16, PVB_MASK_I32, PVB_MASK_I64, PVB_MASK_F32, PVB_MASK_F64) = range(7)
 PVB_SELECT_BYTE, PVB_SELECT_EQ1 = 0, 1
+(PVB_PNP_OK, PVB_PNP_ITERATION_LIMIT, PVB_PNP_TOO_FEW_POINTS, PVB_PNP_PLANAR, PVB_PNP_DEGENERATE) = range(5)
 
 
 class PvbDesc(ctypes.Structure):
@@ -63,6 +64,7 @@ SIGNATURES = {
     "pvb_uncertainty_pnp_from_votes": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32,
                                                       ctypes.c_int64, ctypes.c_int64, ctypes.c_void_p, _vp]),
     "pvb_uncertainty_pnp_init": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, ctypes.c_int64, ctypes.c_int64, _vp]),
+    "pvb_pnp_iterative": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, ctypes.c_int64, ctypes.c_int64, _vp]),
     "pvb_nearest_point_workspace_bytes": (_sz, [_i32, _i32, _i32]),
     "pvb_nearest_point_idx": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _sz, _vp]),
     "pvb_add_metric_workspace_bytes": (_sz, [_i32, _i32, _i32]),

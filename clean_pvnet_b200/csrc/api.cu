@@ -487,6 +487,20 @@ PVB_API int pvb_uncertainty_pnp_init(const double *pts2d, const double *pts3d, c
     return e == cudaSuccess ? PVB_OK : cuda_fail(e, "p3p init kernel");
 }
 
+PVB_API int pvb_pnp_iterative(const double *pts2d, const double *pts3d, const double *K, double *pose, double *rt,
+                              int32_t *info, int32_t n, int32_t pn, int64_t pts3d_stride, int64_t k_stride,
+                              pvb_stream_t stream)
+{
+    if (n < 0) return fail(PVB_ERR_INVALID, "n < 0");
+    if (pn < 1) return fail(PVB_ERR_INVALID, "pn must be >= 1 (got %d)", pn);
+    if (int rc = pnp_check_inputs(n, pts2d && pts3d && K && pose, pts3d_stride, k_stride)) return rc;
+    PnpArgs a = {};
+    a.pts2d = pts2d; a.pts3d = pts3d; a.K = K; a.pose = pose; a.result_rt = rt; a.info = info;
+    a.n = n; a.pn = pn; a.pts3d_stride = pts3d_stride; a.k_stride = k_stride;
+    cudaError_t e = launch_pnp_iterative(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "iterative pnp kernel");
+}
+
 namespace {
 
 // the workspace checks of the nearest-neighbour entries; `need` may be 0 (then NULL is fine)

@@ -126,11 +126,15 @@ struct PnpArgs {
     double *init_out;         // optional [n][6]: the initial pose that was used
     double *result_rt;        // [n][6]: the refined pose; NULL: the P3P start alone (fp64 inputs, into init_out)
     int *info;                // optional [n][2]: iterations, termination code
+    double *pose;             // [n][3][4]: the pose of pvb_pnp_iterative (launch_pnp_iterative only)
     int n, pn;
     long long pts3d_stride, k_stride;
     PnpOptions opt;
 };
 cudaError_t launch_pnp_batch(const PnpArgs &a, cudaStream_t st);
+// PVNet's default pose step, cv2.solvePnP(..., SOLVEPNP_ITERATIVE) (pnp.cu, pnp_iter_core.cuh): reads pts2d, pts3d, K and
+// the strides; writes pose [n][3][4], result_rt (optional) and info (optional: iterations, pvb_pnp_status).
+cudaError_t launch_pnp_iterative(const PnpArgs &a, cudaStream_t st);
 
 // exact nearest neighbour and ADD / ADD-S (nn.cu).  A problem's pn2 queries go to `qchunks` CTAs, its pn1 reference points
 // to `nsplit` slices of `slice` points; nsplit > 1 (chosen from the shapes when b * qchunks CTAs cannot fill the GPU)

@@ -11,6 +11,7 @@
 #include "kernels.h"
 #include "pnp_core.cuh"
 #include "p3p_core.cuh"
+#include "pnp_iter_core.cuh"
 
 namespace pvb {
 
@@ -35,20 +36,28 @@ cudaError_t launch_pnp_weights(const float *cov, float *w, int n, cudaStream_t s
     return cudaGetLastError();
 }
 
+// sum of C numbers over the warp by an XOR butterfly, in place: every lane ends with the same bits
+struct PnpWarpSum {
+    template <int C> __device__ __forceinline__ void sum(double *v) const
+    {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+#pragma unroll
+            for (int q = 0; q < C; ++q) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
+        }
+    }
+};
+
 // normal equations of one problem at `pose`: lane i owns points i, i+32, ...; butterfly sum -> every lane holds the same bits
 __device__ __forceinline__ void pnp_warp_normal_at(const double *pose, const double *p2, const double *p3, const double *w,
                                                    const double *cam, int pn, int lane, PnpNormal &n)
 {
     pnp_normal_zero(n);
     for (int i = lane; i < pn; i += 32) pnp_accumulate_point(pose, p3 + 3 * i, p2 + 2 * i, w + 3 * i, cam, n);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-#pragma unroll
-        for (int q = 0; q < 21; ++q) n.H[q] += __shfl_xor_sync(0xffffffffu, n.H[q], o);
-#pragma unroll
-        for (int q = 0; q < 6; ++q) n.g[q] += __shfl_xor_sync(0xffffffffu, n.g[q], o);
-        n.cost += __shfl_xor_sync(0xffffffffu, n.cost, o);
-    }
+    const PnpWarpSum red;
+    red.sum<21>(n.H);
+    red.sum<6>(n.g);
+    red.sum<1>(&n.cost);
 }
 
 // Problem `prob`'s camera (fx, fy, px, py) and model points: one for the batch (stride 0) or one per problem
@@ -132,6 +141,40 @@ p3p_start_kernel(PnpArgs a)
     p3p_start(a.pts2d + (size_t)prob * a.pn * 2, p3, a.wgt2d + (size_t)prob * a.pn * 3, a.pn, cam, rt);
 #pragma unroll
     for (int i = 0; i < 6; ++i) a.init_out[(size_t)prob * 6 + i] = rt[i];
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// PVNet's default pose step, cv2.solvePnP(..., SOLVEPNP_ITERATIVE) (pnp_iter_core.cuh): one warp per problem like
+// pnp_batch_kernel.  Lane i owns points i, i+32, ...; every sum over points (the centroid and scatter of the model, the 78
+// entries of L^T L, the 28 numbers of J^T J / J^T e / |e|^2) is an XOR butterfly, so every lane holds the same bits and runs
+// the identical DLT and Levenberg-Marquardt code without divergence.  No shared memory, no workspace; a problem's result
+// depends on nothing but its own inputs.
+// ---------------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(PNP_WARPS * 32)
+pnp_iter_kernel(PnpArgs a)
+{
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const int prob = blockIdx.x * PNP_WARPS + wid;
+    if (prob >= a.n) return;
+    double cam[4], rt[6], pose[12];
+    const double *p3 = pnp_model_camera(a, prob, cam);
+    int iterations;
+    const int status = pnp_iter_solve(a.pts2d + (size_t)prob * a.pn * 2, p3, cam, a.pn, lane, 32, PnpWarpSum(), rt, iterations);
+    pnp_iter_pose(rt, pose);
+#pragma unroll
+    for (int i = 0; i < 12; ++i) if (lane == i) a.pose[(size_t)prob * 12 + i] = pose[i];
+    if (a.result_rt) {
+#pragma unroll
+        for (int i = 0; i < 6; ++i) if (lane == 12 + i) a.result_rt[(size_t)prob * 6 + i] = rt[i];
+    }
+    if (a.info && lane == 31) { a.info[2 * prob] = iterations; a.info[2 * prob + 1] = status; }
+}
+
+cudaError_t launch_pnp_iterative(const PnpArgs &a, cudaStream_t st)
+{
+    if (a.n <= 0) return cudaSuccess;
+    pnp_iter_kernel<<<(a.n + PNP_WARPS - 1) / PNP_WARPS, PNP_WARPS * 32, 0, st>>>(a);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_pnp_batch(const PnpArgs &a, cudaStream_t st)

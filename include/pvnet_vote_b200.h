@@ -21,6 +21,7 @@
  *   lib/csrc/uncertainty_pnp/src/ext.h  uncertainty_pnp(...)      pvb_uncertainty_pnp (batched)
  *   un_pnp_utils.py:25-31  cv2.solvePnP(..., SOLVEPNP_P3P)        pvb_uncertainty_pnp_init
  *   evaluators/linemod/pvnet.py:118-130 + un_pnp_utils.py:6-57     pvb_uncertainty_pnp_from_votes (all three, one launch)
+ *   pvnet_pose_utils.py:5-38  pnp(...) = cv2.solvePnP(ITERATIVE)  pvb_pnp_iterative (batched; the default un_pnp=False path)
  *
  *   and the one native extension of the evaluators (lib/csrc/nn, cffi, imported by both):
  *   lib/csrc/nn/src/ext.h  findNearestPointIdxLauncher(...)       pvb_nearest_point_idx (device pointers, batched)
@@ -235,6 +236,31 @@ PVB_API int pvb_uncertainty_pnp_from_votes(const float *kpt_2d, const float *cov
 PVB_API int pvb_uncertainty_pnp_init(const double *pts2d, const double *pts3d, const double *wgt2d, const double *K,
                                      double *init_rt, int32_t n, int32_t pn, int64_t pts3d_stride, int64_t k_stride,
                                      pvb_stream_t stream);
+
+/* PVNet's default pose step for n problems: `pnp(points_3d, points_2d, camera_matrix)` of lib/utils/pvnet/
+ * pvnet_pose_utils.py:5-38, i.e. cv2.solvePnP(..., zero distortion, flags=cv2.SOLVEPNP_ITERATIVE) followed by
+ * [cv2.Rodrigues(rvec) | tvec], which both evaluators call once per image when cfg.test.un_pnp is False
+ * (lib/evaluators/linemod/pvnet.py:188, tless_test/pvnet.py:239).  OpenCV's own method, step for step: its DLT start and
+ * its 20-iteration Levenberg-Marquardt loop with OpenCV's damping schedule and stop rule (csrc/pnp_iter_core.cuh).  Pinned
+ * against cv2.solvePnP 4.13 itself: rvec and tvec within 1e-8 relative wherever OpenCV's own answer is stable under a
+ * 1e-13 relative change of the image points (tests/test_pnp_iter_host_core.py, tests/golden/pnp_iterative.npz).  One warp
+ * per problem, fp64, no workspace.
+ *   All pointers are DEVICE memory: pts2d [n,pn,2] pixels; pts3d [pn,3] and K [3,3] (row-major; fx, fy, cx, cy are read,
+ *   skew and bottom row ignored like OpenCV) per problem at pts3d + p*pts3d_stride / K + p*k_stride (strides in doubles;
+ *   0 = shared); pose [n,3,4] = [R | t]; rt optional [n,6] = (rvec, tvec); info optional int32 [n,2] = (LM iterations,
+ *   pvb_pnp_status).  Every status but PVB_PNP_OK and PVB_PNP_ITERATION_LIMIT writes an all-NaN pose (and rt).  pn >= 1;
+ *   n == 0 is a no-op.  Bad arguments return PVB_ERR_INVALID before any CUDA call. */
+typedef enum pvb_pnp_status {
+    PVB_PNP_OK = 0,                 /* stopped by |p - p_prev| / (|p_prev| + DBL_EPSILON) < FLT_EPSILON           */
+    PVB_PNP_ITERATION_LIMIT = 1,    /* stopped after 20 iterations (OpenCV returns that pose too)                   */
+    PVB_PNP_TOO_FEW_POINTS = 2,     /* pn < 4, or a non-planar model with pn < 6: OpenCV raises                     */
+    PVB_PNP_PLANAR = 3,             /* W[2]/W[1] < 1e-3: OpenCV's homography start, not built here                   */
+    PVB_PNP_DEGENERATE = 4          /* non-finite input, all image points equal, |RR|_F <= DBL_EPSILON, or a step
+                                       whose damped system is not positive definite                                 */
+} pvb_pnp_status;
+PVB_API int pvb_pnp_iterative(const double *pts2d, const double *pts3d, const double *K, double *pose, double *rt,
+                              int32_t *info, int32_t n, int32_t pn, int64_t pts3d_stride, int64_t k_stride,
+                              pvb_stream_t stream);
 
 /* Exact brute-force nearest neighbour, the batched device twin of the reference's
  * `findNearestPointIdxLauncher(ref_pts, que_pts, idxs, b, pn1, pn2, dim, exclude_self)` (lib/csrc/nn/src/ext.h,
