@@ -12,6 +12,9 @@ Public surface (same names/signatures as the reference):
     per-image flags for a batch)
     pose.pnp (twin of lib/utils/pvnet/pvnet_pose_utils.py's cv2.solvePnP ITERATIVE step), pnp_batch (n problems, one launch:
     the pose step of the default un_pnp=False path)
+    vote_loss.vote_loss (the trainer's vote loss and its gradient from the mask and the keypoints), vote_target_batch (twin
+    of lib/utils/pvnet/pvnet_data_utils.py's compute_vertex), NetworkWrapper (twin of lib/train/trainers/pvnet.py),
+    install_vote_loss_as_reference
 """
 from . import _lib  # noqa: F401
 from . import nn  # noqa: F401
@@ -27,6 +30,7 @@ from . import uncertainty_pnp as un_pnp  # noqa: F401
 from .uncertainty_pnp import uncertainty_pnp_batch, p3p_init_batch, uncertainty_pnp_from_votes  # noqa: F401
 from . import pose  # noqa: F401
 from .pose import pnp_batch  # noqa: F401
+from .vote_loss import vote_loss, vote_target_batch, NetworkWrapper, install_vote_loss_as_reference  # noqa: F401
 from .ransac_voting_gpu import (  # noqa: F401
     estimate_voting_distribution_with_mean,
     ransac_voting_layer,
@@ -42,4 +46,5 @@ __all__ = [
     "uncertainty_pnp_from_votes", "pose", "pnp_batch", "parallel",
     "nn", "find_nearest_point_idx", "nearest_point_idx", "add_metric_batch", "install_nn_as_reference_module",
     "metrics", "pose_metrics_batch", "mask_iou_batch", "linemod_scores",
+    "vote_loss", "vote_target_batch", "NetworkWrapper", "install_vote_loss_as_reference",
 ]

@@ -73,6 +73,12 @@ SIGNATURES = {
     "pvb_pose_metrics": (ctypes.c_int, [_vp, _vp, _vp, _vp, ctypes.c_int64, _vp, _vp, _vp, _i32, _i32, _vp, _sz, _vp]),
     "pvb_mask_iou": (ctypes.c_int, [_vp, _i32, ctypes.POINTER(ctypes.c_int64), _vp, _i32, ctypes.POINTER(ctypes.c_int64),
                                     _vp, _vp, _i32, _i32, _i32, _vp]),
+    "pvb_vote_target": (ctypes.c_int, [_vp, _i32, ctypes.POINTER(ctypes.c_int64), _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
+    "pvb_vote_loss_workspace_bytes": (_sz, [_i32, _i32, _i32]),
+    "pvb_vote_loss_forward": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int64), _vp, _i32, ctypes.POINTER(ctypes.c_int64),
+                                             _vp, _vp, _i32, _i32, _i32, _i32, _vp, _sz, _vp]),
+    "pvb_vote_loss_backward": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int64), _vp, _i32, ctypes.POINTER(ctypes.c_int64),
+                                              _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _sz, _vp]),
     "pvb_read_status": (ctypes.c_int, [_dp, _vp, _vp]),
     "pvb_host_scratch_bytes": (_sz, [_dp, _i32]),
     "pvb_ransac_voting_v3_host": (ctypes.c_int, [_dp, _vp, _vp, _vp, _i32, ctypes.c_uint32, _vp, _sz, _vp]),

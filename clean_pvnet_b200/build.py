@@ -12,7 +12,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-SOURCES = ["api.cu", "select.cu", "vote.cu", "prune.cu", "compat.cu", "pnp.cu", "exchange.cu", "nn.cu"]
+SOURCES = ["api.cu", "select.cu", "vote.cu", "prune.cu", "compat.cu", "pnp.cu", "exchange.cu", "nn.cu", "loss.cu"]
 # every header a translation unit includes (pnp.cu: pnp_core.cuh, p3p_core.cuh), found by globbing
 HEADERS = sorted(f for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + [os.path.join("..", "..", "include", "pvnet_vote_b200.h")]
 LIB = os.path.join(HERE, "libpvnet_vote_b200.so")

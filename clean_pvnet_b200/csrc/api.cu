@@ -608,6 +608,112 @@ PVB_API int pvb_mask_iou(const void *pred, int32_t pred_dtype, const int64_t *pr
     return e == cudaSuccess ? PVB_OK : cuda_fail(e, "mask iou kernel");
 }
 
+namespace {
+
+constexpr int VOTE_LOSS_MAX_K = 1024;      // the image's keypoints live in 16 KB of shared memory
+
+// the arguments every vote-loss entry shares; fills the mask, keypoint and size fields of `a`
+int vote_loss_common(VoteLossArgs &a, const void *mask, int32_t mask_dtype, const int64_t *mask_stride, const double *kpt_2d,
+                     int32_t B, int32_t H, int32_t W, int32_t K)
+{
+    if (B < 0 || H < 0 || W < 0) return fail(PVB_ERR_INVALID, "negative size (B=%d H=%d W=%d)", B, H, W);
+    if (K < 1 || K > VOTE_LOSS_MAX_K) return fail(PVB_ERR_INVALID, "K must be in [1, %d], got %d", VOTE_LOSS_MAX_K, K);
+    if (B > 65535) return fail(PVB_ERR_INVALID, "B must be at most 65535, got %d", B);
+    if ((long long)H * W > 0x7fffffffll) return fail(PVB_ERR_INVALID, "image too large (H*W >= 2^31)");
+    if (mask_dtype < PVB_MASK_U8 || mask_dtype > PVB_MASK_I64)
+        return fail(PVB_ERR_INVALID, "mask dtype must be an integer pvb_mask_dtype (U8..I64), got %d", mask_dtype);
+    if (!mask_stride) return fail(PVB_ERR_INVALID, "NULL stride array");
+    for (int i = 0; i < 3; ++i)
+        if (mask_stride[i] < 0) return fail(PVB_ERR_INVALID, "negative stride");
+    if ((long long)B * H * W > 0 && (!mask || !kpt_2d)) return fail(PVB_ERR_INVALID, "NULL tensor");
+    a = VoteLossArgs{};
+    a.mask = mask; a.mask_dtype = mask_dtype;
+    a.msb = mask_stride[0]; a.msy = mask_stride[1]; a.msx = mask_stride[2];
+    a.kpt = kpt_2d;
+    a.B = B; a.H = H; a.W = W; a.K = K;
+    return PVB_OK;
+}
+
+int vote_loss_pred(VoteLossArgs &a, const float *pred, const int64_t *pred_stride)
+{
+    if (!pred_stride) return fail(PVB_ERR_INVALID, "NULL stride array");
+    for (int i = 0; i < 4; ++i) {
+        if (pred_stride[i] < 0) return fail(PVB_ERR_INVALID, "negative stride");
+        a.ps[i] = pred_stride[i];
+    }
+    if ((long long)a.B * a.H * a.W > 0 && !pred) return fail(PVB_ERR_INVALID, "NULL tensor");
+    a.pred = pred;
+    return PVB_OK;
+}
+
+// fills the workspace fields of `a` from a checked workspace
+int vote_loss_workspace(VoteLossArgs &a, const void *workspace, size_t workspace_bytes)
+{
+    size_t po = 0, wo = 0;
+    const size_t need = vote_loss_workspace_bytes(a.B, a.H, a.W, &po, &wo);
+    if (!workspace || workspace_bytes < need)
+        return fail(PVB_ERR_WORKSPACE, "workspace too small: need %zu bytes, got %zu", need, workspace ? workspace_bytes : 0);
+    if (reinterpret_cast<uintptr_t>(workspace) & 255u) return fail(PVB_ERR_WORKSPACE, "workspace must be 256-byte aligned");
+    char *ws = static_cast<char *>(const_cast<void *>(workspace));
+    a.wsum = reinterpret_cast<float *>(ws);
+    a.partial = reinterpret_cast<double *>(ws + po);
+    a.wpart = reinterpret_cast<long long *>(ws + wo);
+    return PVB_OK;
+}
+
+} // namespace
+
+// pvnet_data_utils.py:30-44 compute_vertex
+PVB_API int pvb_vote_target(const void *mask, int32_t mask_dtype, const int64_t *mask_stride, const double *kpt_2d,
+                            float *vertex, int32_t B, int32_t H, int32_t W, int32_t K, pvb_stream_t stream)
+{
+    VoteLossArgs a;
+    if (int rc = vote_loss_common(a, mask, mask_dtype, mask_stride, kpt_2d, B, H, W, K)) return rc;
+    if ((long long)B * H * W > 0 && !vertex) return fail(PVB_ERR_INVALID, "NULL tensor");
+    a.out = vertex;
+    cudaError_t e = launch_vote_target(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "vote target kernel");
+}
+
+PVB_API size_t pvb_vote_loss_workspace_bytes(int32_t B, int32_t H, int32_t W)
+{
+    if (B < 0 || H < 0 || W < 0) return 0;
+    return vote_loss_workspace_bytes(B, H, W, nullptr, nullptr);
+}
+
+// lib/train/trainers/pvnet.py:25-27, the forward pass
+PVB_API int pvb_vote_loss_forward(const float *pred, const int64_t *pred_stride, const void *mask, int32_t mask_dtype,
+                                  const int64_t *mask_stride, const double *kpt_2d, float *loss, int32_t B, int32_t H,
+                                  int32_t W, int32_t K, void *workspace, size_t workspace_bytes, pvb_stream_t stream)
+{
+    VoteLossArgs a;
+    if (int rc = vote_loss_common(a, mask, mask_dtype, mask_stride, kpt_2d, B, H, W, K)) return rc;
+    if (int rc = vote_loss_pred(a, pred, pred_stride)) return rc;
+    if (!loss) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (int rc = vote_loss_workspace(a, workspace, workspace_bytes)) return rc;
+    a.loss = loss;
+    cudaError_t e = launch_vote_loss_forward(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "vote loss forward kernels");
+}
+
+// lib/train/trainers/pvnet.py:25-27, autograd's backward pass of it
+PVB_API int pvb_vote_loss_backward(const float *pred, const int64_t *pred_stride, const void *mask, int32_t mask_dtype,
+                                   const int64_t *mask_stride, const double *kpt_2d, const float *grad_loss,
+                                   float *grad_pred, int32_t B, int32_t H, int32_t W, int32_t K, const void *workspace,
+                                   size_t workspace_bytes, pvb_stream_t stream)
+{
+    VoteLossArgs a;
+    if (int rc = vote_loss_common(a, mask, mask_dtype, mask_stride, kpt_2d, B, H, W, K)) return rc;
+    if (int rc = vote_loss_pred(a, pred, pred_stride)) return rc;
+    if ((long long)B * H * W == 0) return PVB_OK;
+    if (!grad_loss || !grad_pred) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (int rc = vote_loss_workspace(a, workspace, workspace_bytes)) return rc;
+    a.grad_loss = grad_loss;
+    a.out = grad_pred;
+    cudaError_t e = launch_vote_loss_backward(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "vote loss backward kernel");
+}
+
 PVB_API int pvb_read_status(const pvb_desc *d, const void *workspace, pvb_stream_t stream)
 {
     pvb_layout L;

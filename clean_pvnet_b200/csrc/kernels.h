@@ -161,6 +161,30 @@ cudaError_t launch_pose_metrics(const double *model, const double *pose_pred, co
 cudaError_t launch_mask_iou(const void *pred, int pred_dtype, const long long *ps, const void *gt, int gt_dtype,
                             const long long *gs, long long *inter, long long *uni, int B, int H, int W, cudaStream_t st);
 
+// PVNet's vote loss (loss.cu, DESIGN.md 8e): the target field of compute_vertex, the trainer's smooth-l1 vote loss and its
+// gradient, from the mask and the keypoints.  One thread per pixel over a (ceil(H*W / 256), B) grid; the image's keypoints
+// are staged in shared memory.
+struct VoteLossArgs {
+    const float *pred;        // [B][2K][H][W] at element strides ps (forward, backward)
+    long long ps[4];
+    const void *mask;         // [B][H][W] integer pvb_mask_dtype at element strides msb, msy, msx
+    int mask_dtype;
+    long long msb, msy, msx;
+    const double *kpt;        // [B][K][2] contiguous, (x, y) per keypoint
+    int B, H, W, K;
+    float *out;               // contiguous [B][2K][H][W]: the target field (target) or grad_pred (backward)
+    double *partial;          // [B * ceil(H*W / 256)] per-CTA sums of the smooth-l1 terms (forward)
+    long long *wpart;         // [B * ceil(H*W / 256)] per-CTA sums of the mask values (forward)
+    float *wsum;              // fp32 weight sum: written by the forward pass, read by the backward pass
+    float *loss;              // the scalar loss (forward)
+    const float *grad_loss;   // the scalar upstream gradient (backward)
+};
+// workspace: wsum at offset 0, then the two partial arrays, each 256-byte aligned
+size_t vote_loss_workspace_bytes(int B, int H, int W, size_t *partial_offset, size_t *wpart_offset);
+cudaError_t launch_vote_target(const VoteLossArgs &a, cudaStream_t st);
+cudaError_t launch_vote_loss_forward(const VoteLossArgs &a, cudaStream_t st);
+cudaError_t launch_vote_loss_backward(const VoteLossArgs &a, cudaStream_t st);
+
 // twins of the reference extension on its own layouts
 cudaError_t launch_compat_generate(const float *direct, const float *coords, const int32_t *idxs, float *hyp,
                                    int tn, int vn, int hn, bool vanishing, cudaStream_t st);

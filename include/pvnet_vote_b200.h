@@ -34,6 +34,10 @@
  *   evaluators/tless_test/pvnet.py:119-125  cm_degree_5_metric     pvb_pose_metrics (n pose pairs per call)
  *   evaluators/linemod/pvnet.py:96-100  mask_iou                   pvb_mask_iou (B images per call)
  *
+ *   and the training side of the vote field:
+ *   utils/pvnet/pvnet_data_utils.py:30-44  compute_vertex          pvb_vote_target (B images per call)
+ *   train/trainers/pvnet.py:25-27  vote loss                       pvb_vote_loss_forward / pvb_vote_loss_backward
+ *
  * Conventions
  *   - plain C: device pointers, sizes, strides (in ELEMENTS), a CUDA stream
  *     handle.  No torch types.  All work is enqueued on `stream`; no entry
@@ -328,6 +332,45 @@ PVB_API int pvb_pose_metrics(const double *model, const double *pose_pred, const
 PVB_API int pvb_mask_iou(const void *pred, int32_t pred_dtype, const int64_t *pred_stride, const void *gt, int32_t gt_dtype,
                          const int64_t *gt_stride, int64_t *inter, int64_t *uni, int32_t B, int32_t H, int32_t W,
                          pvb_stream_t stream);
+
+/* ---- training: PVNet's vote loss from the mask and the keypoints (DESIGN.md section 8e) ----------------------------
+ * The trainer supervises the unit-vector field with a dense target that every dataset builds on the host
+ * (pvnet_data_utils.py:30-44 compute_vertex, called by lib/datasets/{linemod,custom}/pvnet.py:53 and
+ * tless_train/pvnet.py:117).  These entries compute that target, and the loss and gradient that consume it, on the device.
+ * Shared arguments:
+ *   mask       device [B,H,W] of an integer pvb_mask_dtype (U8, also for bool, I8, I16, I32, I64) at element strides
+ *              mask_stride (HOST int64[3]).  The target is non-zero only where mask == 1; the loss weight is float(mask).
+ *   kpt_2d     device fp64 [B,K,2] contiguous, (x = column, y = row) per keypoint.
+ *   B <= 65535, 1 <= K <= 1024, H*W < 2^31.  The target of channel 2k / 2k+1 at (x, y), where mask == 1, is compute_vertex's
+ *   bit for bit: d = kpt - (x, y), n = sqrt(RN(dx*dx) + RN(dy*dy)), n < 1e-3 -> n + 1e-3, (dx / n, dy / n) rounded to fp32.
+ * Bad arguments (negative sizes, K out of range, NULL pointers or stride arrays, negative strides, other dtypes) return
+ * PVB_ERR_INVALID, a missing, short or misaligned workspace PVB_ERR_WORKSPACE, both before any CUDA call.  No entry
+ * synchronises with the host. */
+
+/* pvnet_data_utils.py:30-44 compute_vertex for a batch: vertex device fp32 [B,2K,H,W] contiguous, fully written.
+ * B, H or W == 0 is a no-op. */
+PVB_API int pvb_vote_target(const void *mask, int32_t mask_dtype, const int64_t *mask_stride, const double *kpt_2d,
+                            float *vertex, int32_t B, int32_t H, int32_t W, int32_t K, pvb_stream_t stream);
+
+/* The vote loss of lib/train/trainers/pvnet.py:25-27 with batch['vertex'] = compute_vertex(mask, kpt_2d), never built:
+ *   w = float(mask);  loss = smooth_l1(pred * w, tgt * w, reduction='sum') / w.sum() / 2K
+ * pred device fp32 [B,2K,H,W] at element strides pred_stride (HOST int64[4]), read at every pixel (a NaN or inf prediction
+ * where w = 0 gives a NaN loss, as in the reference).  The terms are summed in fp64 and added in a fixed order, so the loss
+ * is reproducible bit for bit; w.sum() is the exact int64 sum of the mask values rounded to fp32 (the reference's fp32 sum
+ * agrees while its partial sums stay below 2^24).  loss: device fp32 scalar.  workspace:
+ * pvb_vote_loss_workspace_bytes(B, H, W) bytes of 256-byte aligned device memory; it keeps the fp32 weight sum for
+ * pvb_vote_loss_backward, so pass the same workspace to both.  B, H or W == 0 gives the reference's NaN (0 / 0). */
+PVB_API size_t pvb_vote_loss_workspace_bytes(int32_t B, int32_t H, int32_t W);
+PVB_API int pvb_vote_loss_forward(const float *pred, const int64_t *pred_stride, const void *mask, int32_t mask_dtype,
+                                  const int64_t *mask_stride, const double *kpt_2d, float *loss, int32_t B, int32_t H,
+                                  int32_t W, int32_t K, void *workspace, size_t workspace_bytes, pvb_stream_t stream);
+/* autograd's gradient of that loss with respect to pred, bit for bit: grad_loss is the device fp32 upstream gradient
+ * (read on the device, never by the host), grad_pred device fp32 [B,2K,H,W] contiguous, fully written.  The workspace is
+ * the forward call's, after it.  B, H or W == 0 is a no-op. */
+PVB_API int pvb_vote_loss_backward(const float *pred, const int64_t *pred_stride, const void *mask, int32_t mask_dtype,
+                                   const int64_t *mask_stride, const double *kpt_2d, const float *grad_loss,
+                                   float *grad_pred, int32_t B, int32_t H, int32_t W, int32_t K, const void *workspace,
+                                   size_t workspace_bytes, pvb_stream_t stream);
 
 /* Reads the sticky status word of a workspace (synchronises `stream`). */
 PVB_API int pvb_read_status(const pvb_desc *d, const void *workspace, pvb_stream_t stream);
