@@ -188,6 +188,7 @@ int make_plan(const pvb_desc *d, const void *mask, const float *vertex, const in
     P->prune.key = reinterpret_cast<int *>(w + L.prune_key);
     P->prune.list = reinterpret_cast<int *>(w + L.prune_list);
     P->prune.len = reinterpret_cast<int *>(w + L.prune_len);
+    P->prune.ticket = P->refit.ticket;               // the bound step leaves it at 0 for the refit
     P->prune.ncx = (d->W + PRUNE_CELL - 1) / PRUNE_CELL;
     P->prune.ncells = L.prune_ncells;
     P->prune.cos_w = P->prune.sin_w = 0.f;

@@ -56,7 +56,7 @@ constexpr int PRUNE_CELL = 32;              // histogram cells are PRUNE_CELL x 
 constexpr int PRUNE_NBIN = 128;             // pseudo-angle bins per cell
 constexpr int PRUNE_REC = 4 + PRUNE_NBIN / 2;   // words per (image, keypoint, cell): box, 16-bit inclusive prefix counts
 constexpr int PRUNE_M = 128;                // pass-1 hypotheses = one slice of the pruned vote shape
-constexpr int PRUNE_MAX_HN = 2048;          // the plan kernel holds two hypotheses per thread
+constexpr int PRUNE_MAX_HN = 2048;          // pass 1 is picked from every bound staged in shared memory
 constexpr int PRUNE_MIN_UNITS = 32;         // fewer (image, keypoint) pairs: the full vote is faster
 static_assert(PRUNE_CELL * PRUNE_CELL < 65536, "a cell's prefix counts fit 16 bits");
 struct PruneArgs {
@@ -64,6 +64,7 @@ struct PruneArgs {
     int *key;            // [B][K][hn]  bound, or -1 for pass-1 hypotheses
     int *list;           // [2][B][K][hn]
     int *len;            // [2][B][K]
+    int *ticket;         // [B][K] arrival counter of the bound CTAs: 0 at the start of the call, and left 0
     int ncx, ncells;     // ceil(W / PRUNE_CELL), ceil(H / PRUNE_CELL) * ncx
     float cos_w, sin_w;  // rotation by the widened cone half-angle theta'
 };

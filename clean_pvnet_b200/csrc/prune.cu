@@ -8,8 +8,8 @@
 // count of any hypothesis, cannot be the first maximum.  DESIGN.md 4.2 has the argument, including the slack theta' - theta.
 //
 //   prune_hist_kernel   (band, k, b):   per cell of a 32-row band: bounding box + prefix histogram of direction pseudo-angles
-//   prune_bound_kernel  (h group, k, b): B(h), one thread per hypothesis -> key
-//   prune_plan_kernel   (k, b):         the PRUNE_M largest bounds -> list 0 (pass 1)
+//   prune_bound_kernel  (h group, k, b): B(h), three threads per hypothesis -> key; the last CTA of (k, b) takes the
+//                                       PRUNE_M largest bounds -> list 0 (pass 1)
 //   vote_kernel         list 0
 //   prune_next_kernel   (k, b):         L = best pass-1 count; {h not in pass 1 : B(h) >= L} -> list 1 (pass 2)
 //   vote_list_kernel    list 1
@@ -178,57 +178,198 @@ __device__ void count_bound(const PruneArgs &q, const int *rec, int nt, float hx
     }
 }
 
-constexpr int BOUND_HYPS = 128;                // hypotheses per CTA
-constexpr int BOUND_SPLIT = 3;                 // threads per hypothesis, each over a third of the records: one thread per
-                                               // hypothesis leaves ~4 warps per scheduler, too few to hide the latency
+constexpr int BOUND_HYPS = 64;                 // hypotheses per CTA
+constexpr int BOUND_SPLIT = 3;                 // threads per hypothesis, each over a third of every staged chunk: one
+                                               // thread per hypothesis leaves too few warps to hide the latency
 constexpr int BOUND_THREADS = BOUND_HYPS * BOUND_SPLIT;
-constexpr int BOUND_CELLS = 64;                // non-empty cell records staged in shared memory at a time (17 KB)
+constexpr int BOUND_WARPS = BOUND_THREADS / 32;
+constexpr int BOUND_SCAN = 3 * BOUND_THREADS;  // cell totals read per listing round, three per thread
+constexpr int BOUND_CELLS = 32;                // non-empty cell records per staged chunk; two chunks in flight (17 KB)
+constexpr int REC_V4 = PRUNE_REC / 4;          // 16-byte pieces of a record
+static_assert(PRUNE_REC % 4 == 0, "records are staged in 16-byte pieces");
+static_assert(PRUNE_MAX_HN + 256 <= 2 * BOUND_CELLS * PRUNE_REC, "the pass-1 selection fits in the record buffers");
 
-__global__ void __launch_bounds__(BOUND_THREADS)
+__device__ __forceinline__ void cp_async16(void *smem, const void *gmem)
+{
+    const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" :: "r"(s), "l"(gmem) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
+template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" :: "n"(N) : "memory"); }
+
+// Pass 1 of (b, k): the PRUNE_M largest bounds, ties in index order, listed in index order; their keys become -1.
+// Called by every thread of the CTA once all of the (image, keypoint)'s bounds are in q.key.  s_key holds hn ints,
+// s_cnt 256, s_w 2 x BOUND_WARPS, s_sel 2.
+__device__ void plan_pass1(const VoteArgs &a, const PruneArgs &q, size_t bk, int *s_key, int *s_cnt, int *s_w, int *s_sel)
+{
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int hn = a.hn, M = min(PRUNE_M, hn);
+    int *key = q.key + bk * hn;
+    int top = 0;
+    for (int h = tid; h < hn; h += BOUND_THREADS) {
+        const int v = __ldcg(key + h);                    // written by the other CTAs of (b, k)
+        s_key[h] = v;
+        top = max(top, v);
+    }
+    top = __reduce_max_sync(0xffffffffu, top);
+    if (lane == 0) s_w[warp] = top;
+    __syncthreads();
+    for (int w = 0; w < BOUND_WARPS; ++w) top = max(top, s_w[w]);
+    // thr = the M-th largest bound (bounds are >= 0), by radix selection, at most 8 bits a round from the top: bits
+    // [hi, 31] of thr are fixed, and `need` of the M lie among the bounds that agree with thr there
+    int thr = 0, need = M;
+    for (int hi = 32 - __clz(top | 1); hi > 0;) {
+        const int lo = max(0, hi - 8);
+        for (int i = tid; i < 256; i += BOUND_THREADS) s_cnt[i] = 0;
+        __syncthreads();
+        for (int h = tid; h < hn; h += BOUND_THREADS) {
+            const int v = s_key[h];
+            if ((v >> hi) == (thr >> hi)) atomicAdd(&s_cnt[(v >> lo) & ((1 << (hi - lo)) - 1)], 1);
+        }
+        __syncthreads();
+        if (warp == 0) {                                  // the digit d of thr: the largest with #{digit >= d} >= need
+            int c[8], own = 0;
+#pragma unroll
+            for (int e = 0; e < 8; ++e) { c[e] = s_cnt[8 * lane + e]; own += c[e]; }
+            int suf = own;                                // digits >= 8 * lane
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int t = __shfl_down_sync(0xffffffffu, suf, o);
+                if (lane + o < 32) suf += t;
+            }
+            const unsigned ok = __ballot_sync(0xffffffffu, suf >= need);   // lane 0 always: every match counts
+            if (lane == 31 - __clz(ok)) {
+                int above = suf - own;
+#pragma unroll
+                for (int e = 7; e >= 0; --e) {
+                    if (above + c[e] >= need) { s_sel[0] = 8 * lane + e; s_sel[1] = need - above; break; }
+                    above += c[e];
+                }
+            }
+        }
+        __syncthreads();
+        thr |= s_sel[0] << lo;
+        need = s_sel[1];
+        hi = lo;
+    }
+    // every bound > thr and the first `need` equal to it, in index order: each warp takes a contiguous range
+    const int per = (hn + 32 * BOUND_WARPS - 1) / (32 * BOUND_WARPS) * 32;
+    const int h0 = warp * per, h1 = min(hn, h0 + per);
+    int gt = 0, eq = 0;
+    for (int h = h0 + lane; h - lane < h1; h += 32) {
+        const int v = h < h1 ? s_key[h] : -1;
+        gt += __popc(__ballot_sync(0xffffffffu, v > thr));
+        eq += __popc(__ballot_sync(0xffffffffu, v == thr));
+    }
+    int *s_gt = s_w, *s_eq = s_w + BOUND_WARPS;
+    __syncthreads();                                      // s_w was read above
+    if (lane == 0) { s_gt[warp] = gt; s_eq[warp] = eq; }
+    __syncthreads();
+    gt = eq = 0;
+    for (int w = 0; w < warp; ++w) { gt += s_gt[w]; eq += s_eq[w]; }
+    int *list = q.list + bk * hn;
+    const unsigned below = (1u << lane) - 1u;
+    for (int h = h0 + lane; h - lane < h1; h += 32) {
+        const int v = h < h1 ? s_key[h] : -1;
+        const unsigned mg = __ballot_sync(0xffffffffu, v > thr), me = __ballot_sync(0xffffffffu, v == thr);
+        const int g = gt + __popc(mg & below), e = eq + __popc(me & below);
+        if (v > thr || (v == thr && e < need)) {
+            list[g + min(e, need)] = h;
+            key[h] = -1;
+        }
+        gt += __popc(mg);
+        eq += __popc(me);
+    }
+    if (tid == 0) q.len[bk] = M;
+}
+
+// One CTA per (BOUND_HYPS hypotheses, k, b).  The CTA lists the non-empty cells (an empty one adds nothing), stages
+// their records in shared memory a chunk ahead of the one it computes on, and sums B(h) over them; the last CTA of
+// (b, k) to finish then picks pass 1 (plan_pass1), so no launch waits for the slowest one.
+__global__ void __launch_bounds__(BOUND_THREADS, 10)
 prune_bound_kernel(VoteArgs a, PruneArgs q)
 {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int part = tid / BOUND_HYPS;
-    const int h = blockIdx.x * BOUND_HYPS + tid % BOUND_HYPS, k = blockIdx.y, b = blockIdx.z;
+    const int part = tid / BOUND_HYPS, hl = tid % BOUND_HYPS;
+    const int h = blockIdx.x * BOUND_HYPS + hl, k = blockIdx.y, b = blockIdx.z;
     const size_t bk = (size_t)b * a.K + k;
     const int tn = max(0, min(a.tn[b], a.cap));
-    __shared__ int s_rec[BOUND_CELLS * PRUNE_REC];
-    __shared__ int s_idx[BOUND_CELLS];
-    __shared__ int s_bound[BOUND_HYPS];
-    __shared__ int s_n, s_next;
-    if (tid < BOUND_HYPS) s_bound[tid] = 0;
+    __shared__ __align__(16) int s_rec[2][BOUND_CELLS * PRUNE_REC];
+    __shared__ int s_idx[BOUND_SCAN];
+    __shared__ int s_part[BOUND_SPLIT][BOUND_HYPS];
+    __shared__ int s_w[2 * BOUND_WARPS];
+    __shared__ int s_sel[2];
     const float2 hp = (h < a.hn) ? a.hyp[bk * a.hn + h] : make_float2(0.f, 0.f);
     const int *rec = q.cells + bk * q.ncells * PRUNE_REC;
     int bound = 0;
-    for (int c0 = 0; c0 < q.ncells;) {
-        if (warp == 0) {                                  // the next non-empty cells: an empty one adds nothing
-            int m = 0, c = c0;
-            for (; c < q.ncells && m <= BOUND_CELLS - 32; c += 32) {
-                const bool f = c + lane < q.ncells && cell_total(rec + (size_t)(c + lane) * PRUNE_REC) > 0;
-                const unsigned bal = __ballot_sync(0xffffffffu, f);
-                if (f) s_idx[m + __popc(bal & ((1u << lane) - 1u))] = c + lane;
-                m += __popc(bal);
-            }
-            if (lane == 0) { s_n = m; s_next = c; }
+    for (int c0 = 0; c0 < q.ncells; c0 += BOUND_SCAN) {
+        bool f[3];
+        unsigned bal[3];
+        int cnt = 0;
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            const int c = c0 + j * BOUND_THREADS + tid;
+            f[j] = c < q.ncells && cell_total(rec + (size_t)c * PRUNE_REC) > 0;
+        }
+#pragma unroll
+        for (int j = 0; j < 3; ++j) { bal[j] = __ballot_sync(0xffffffffu, f[j]); cnt += __popc(bal[j]); }
+        if (lane == 0) s_w[warp] = cnt;
+        __syncthreads();
+        int base = 0, m = 0;
+        for (int w = 0; w < BOUND_WARPS; ++w) {
+            const int c = s_w[w];
+            base += (w < warp) ? c : 0;
+            m += c;
+        }
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {                     // the order of the list does not change an integer sum
+            if (f[j]) s_idx[base + __popc(bal[j] & ((1u << lane) - 1u))] = c0 + j * BOUND_THREADS + tid;
+            base += __popc(bal[j]);
         }
         __syncthreads();
-        const int m = s_n;
-        c0 = s_next;
-        for (int r = warp; r < m; r += BOUND_THREADS / 32)
-            for (int w = lane; w < PRUNE_REC; w += 32) s_rec[r * PRUNE_REC + w] = __ldg(rec + (size_t)s_idx[r] * PRUNE_REC + w);
-        __syncthreads();
-        const int r0 = part * m / BOUND_SPLIT, r1 = (part + 1) * m / BOUND_SPLIT;
-        count_bound(q, s_rec + r0 * PRUNE_REC, r1 - r0, hp.x, hp.y, bound);
-        __syncthreads();                                  // s_idx, s_rec, s_n, s_next are rewritten
+        const int nch = (m + BOUND_CELLS - 1) / BOUND_CELLS;
+        auto stage = [&](int ch) {
+            const int r0 = ch * BOUND_CELLS, n = min(BOUND_CELLS, m - r0);
+            int *dst = s_rec[ch & 1];
+            for (int i = tid; i < n * REC_V4; i += BOUND_THREADS) {
+                const int r = i / REC_V4, w = (i - r * REC_V4) * 4;
+                cp_async16(dst + r * PRUNE_REC + w, rec + (size_t)s_idx[r0 + r] * PRUNE_REC + w);
+            }
+            cp_async_commit();
+        };
+        if (nch > 0) stage(0);
+        for (int ch = 0; ch < nch; ++ch) {
+            if (ch + 1 < nch) { stage(ch + 1); cp_async_wait<1>(); }
+            else cp_async_wait<0>();
+            __syncthreads();
+            const int n = min(BOUND_CELLS, m - ch * BOUND_CELLS);
+            const int r0 = part * n / BOUND_SPLIT, r1 = (part + 1) * n / BOUND_SPLIT;
+            count_bound(q, s_rec[ch & 1] + r0 * PRUNE_REC, r1 - r0, hp.x, hp.y, bound);
+            __syncthreads();                              // the buffer is restaged two chunks on; s_idx, s_w next round
+        }
     }
-    if (part > 0) atomicAdd(&s_bound[tid % BOUND_HYPS], bound);
+    if (part > 0) s_part[part][hl] = bound;
     __syncthreads();
-    // non-finite or huge: not bounded
-    if (part == 0 && h < a.hn) q.key[bk * a.hn + h] = (fabsf(hp.x) + fabsf(hp.y) <= 1e15f) ? bound + s_bound[tid] : tn;
+    if (part == 0 && h < a.hn) {
+#pragma unroll
+        for (int p = 1; p < BOUND_SPLIT; ++p) bound += s_part[p][hl];
+        // non-finite or huge: not bounded
+        q.key[bk * a.hn + h] = (fabsf(hp.x) + fabsf(hp.y) <= 1e15f) ? bound : tn;
+    }
+    // q.ticket[bk] is 0 when the call starts (it lies in the workspace header) and is left 0 for the refit
+    __threadfence();
+    __syncthreads();
+    if (tid == 0) {
+        s_sel[0] = (atomicAdd(q.ticket + bk, 1) == (int)gridDim.x - 1);
+        if (s_sel[0]) q.ticket[bk] = 0;
+    }
+    __syncthreads();
+    if (!s_sel[0]) return;
+    __threadfence();
+    plan_pass1(a, q, bk, &s_rec[0][0], &s_rec[0][0] + PRUNE_MAX_HN, s_w, s_sel);
 }
 
 constexpr int PLAN_THREADS = 1024;
-constexpr int PLAN_HPT = PRUNE_MAX_HN / PLAN_THREADS;
 
 // exclusive prefix of `flag` over the CTA in thread order; returns it, *total gets the sum.  Every thread calls it.
 __device__ __forceinline__ int cta_scan(bool flag, int *s_warp, int *total)
@@ -246,49 +387,6 @@ __device__ __forceinline__ int cta_scan(bool flag, int *s_warp, int *total)
     }
     *total = tot;
     return before + __popc(m & ((1u << lane) - 1u));
-}
-
-__global__ void __launch_bounds__(PLAN_THREADS)
-prune_plan_kernel(VoteArgs a, PruneArgs q)
-{
-    const int k = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
-    const size_t bk = (size_t)b * a.K + k;
-    const int tn = max(0, min(a.tn[b], a.cap));
-    __shared__ int s_warp[PLAN_THREADS / 32];
-    int bnd[PLAN_HPT];
-#pragma unroll
-    for (int j = 0; j < PLAN_HPT; ++j) {
-        const int h = j * PLAN_THREADS + tid;
-        bnd[j] = (h < a.hn) ? q.key[bk * a.hn + h] : -1;  // no hypothesis: -1, never selected
-    }
-    // pass 1: the M largest bounds (ties in index order).  thr = largest v with #{B >= v} >= M, by bisection over [0, tn]
-    const int M = min(PRUNE_M, a.hn);
-    int lo = 0, hi = tn + 1;
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        int c = 0;
-#pragma unroll
-        for (int j = 0; j < PLAN_HPT; ++j) c += __syncthreads_count(bnd[j] >= mid);
-        if (c >= M) lo = mid; else hi = mid;
-    }
-    int gt = 0;
-#pragma unroll
-    for (int j = 0; j < PLAN_HPT; ++j) gt += __syncthreads_count(bnd[j] > lo);
-    int *list = q.list + bk * a.hn;
-    int base_eq = 0, base_sel = 0;
-#pragma unroll
-    for (int j = 0; j < PLAN_HPT; ++j) {
-        const int h = j * PLAN_THREADS + tid;
-        int n_eq, n_sel;
-        const int r = base_eq + cta_scan(bnd[j] == lo, s_warp, &n_eq);
-        const bool sel = bnd[j] > lo || (bnd[j] == lo && r < M - gt);
-        const int pos = base_sel + cta_scan(sel, s_warp, &n_sel);
-        if (sel) list[pos] = h;
-        if (h < a.hn && sel) q.key[bk * a.hn + h] = -1;
-        base_eq += n_eq;
-        base_sel += n_sel;
-    }
-    if (tid == 0) q.len[bk] = M;
 }
 
 __global__ void __launch_bounds__(PLAN_THREADS)
@@ -348,7 +446,6 @@ cudaError_t launch_vote_pruned(const VoteArgs &a, const PruneArgs &q, cudaStream
     const int nbands = (a.H + PRUNE_CELL - 1) / PRUNE_CELL;
     prune_hist_kernel<<<dim3(nbands, a.K, a.B), HIST_THREADS, 0, st>>>(a, q);
     prune_bound_kernel<<<dim3((a.hn + BOUND_HYPS - 1) / BOUND_HYPS, a.K, a.B), BOUND_THREADS, 0, st>>>(a, q);
-    prune_plan_kernel<<<dim3(a.K, a.B), PLAN_THREADS, 0, st>>>(a, q);
     cudaError_t e = launch_vote_list_slices(a, q.list, q.len, PRUNE_M, st);
     if (e != cudaSuccess) return e;
     prune_next_kernel<<<dim3(a.K, a.B), PLAN_THREADS, 0, st>>>(a, q);
