@@ -122,6 +122,9 @@ int make_layout(const pvb_desc *d, pvb_layout *L)
     L->prune_key = take(B * K * hn * sizeof(int));
     L->prune_list = take(2 * B * K * hn * sizeof(int));
     L->prune_len = take(2 * B * K * sizeof(int));
+    // not in pvb_layout (its fields are ABI): the sub-cell records and the pass-2 refinement's bounds follow prune_len
+    take(B * K * ncells * 4 * PRUNE_REC * sizeof(int));
+    take(B * K * hn * sizeof(int));
     L->total = off;
     L->nwords = nwords;
     L->nblocks = nblocks;
@@ -188,6 +191,10 @@ int make_plan(const pvb_desc *d, const void *mask, const float *vertex, const in
     P->prune.key = reinterpret_cast<int *>(w + L.prune_key);
     P->prune.list = reinterpret_cast<int *>(w + L.prune_list);
     P->prune.len = reinterpret_cast<int *>(w + L.prune_len);
+    const size_t BK = (size_t)d->B * d->K;
+    const size_t prune_sub = align_up(L.prune_len + 2 * BK * sizeof(int));
+    P->prune.sub = reinterpret_cast<int *>(w + prune_sub);
+    P->prune.b2 = reinterpret_cast<int *>(w + align_up(prune_sub + BK * L.prune_ncells * 4 * PRUNE_REC * sizeof(int)));
     P->prune.ticket = P->refit.ticket;               // the bound step leaves it at 0 for the refit
     P->prune.ncx = (d->W + PRUNE_CELL - 1) / PRUNE_CELL;
     P->prune.ncells = L.prune_ncells;

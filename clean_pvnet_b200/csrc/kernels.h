@@ -51,8 +51,10 @@ cudaError_t launch_vote(const VoteArgs &a, bool zero_counts, cudaStream_t st);
 
 // Pruned v3 vote (prune.cu, DESIGN.md 4.2): only hypotheses that can still be the first maximum are scored.  A bound
 // B(h) >= count(h) comes from per-cell direction histograms; pass 1 scores the PRUNE_M largest bounds, pass 2 every other
-// hypothesis whose bound reaches pass 1's best count.  The others keep count 0, below the winner's.
+// hypothesis whose bound reaches pass 1's best count and whose bound over the cells' four sub-cells reaches it too.  The
+// others keep count 0, below the winner's.
 constexpr int PRUNE_CELL = 32;              // histogram cells are PRUNE_CELL x PRUNE_CELL pixels of the image
+constexpr int PRUNE_SUB = PRUNE_CELL / 2;   // each split into 2 x 2 sub-cells, which refine pass 2
 constexpr int PRUNE_NBIN = 128;             // pseudo-angle bins per cell
 constexpr int PRUNE_REC = 4 + PRUNE_NBIN / 2;   // words per (image, keypoint, cell): box, 16-bit inclusive prefix counts
 constexpr int PRUNE_M = 128;                // pass-1 hypotheses = one slice of the pruned vote shape
@@ -61,7 +63,11 @@ constexpr int PRUNE_MIN_UNITS = 32;         // fewer (image, keypoint) pairs: th
 static_assert(PRUNE_CELL * PRUNE_CELL < 65536, "a cell's prefix counts fit 16 bits");
 struct PruneArgs {
     int *cells;          // [B][K][ncells][PRUNE_REC], cell (row band y, column x) at y * ncx + x
+    int *sub;            // [B][K][ncells][4][PRUNE_REC], the sub-cells of each cell: top left, top right, bottom left,
+                         // bottom right; a cell's record is their union.  Of an empty one only the last word (0) is written
     int *key;            // [B][K][hn]  bound, or -1 for pass-1 hypotheses
+    int *b2;             // [B][K][hn]  bound over the sub-cells of pass-2 candidates: zeroed by the bound step, summed by
+                         // prune_next_kernel
     int *list;           // [2][B][K][hn]
     int *len;            // [2][B][K]
     int *ticket;         // [B][K] arrival counter of the bound CTAs: 0 at the start of the call, and left 0

@@ -5,13 +5,17 @@
 // h-c (c in Q) lies in the angular interval [psi_lo, psi_hi] that Q subtends from h (convexity: the extremes are corners),
 // so at most #{c in set : angle(u_c) in [psi_lo - theta', psi_hi + theta']} of its pixels vote for h.  The sets are the
 // 32x32-pixel cells of the image; summed over the cells this is B(h) >= count(h).  A hypothesis with B(h) < L, L the exact
-// count of any hypothesis, cannot be the first maximum.  DESIGN.md 4.2 has the argument, including the slack theta' - theta.
+// count of any hypothesis, cannot be the first maximum.  The argument holds for any partition of the pixels, so pass 2 also
+// requires B2(h) >= L, the same bound over the 16x16-pixel sub-cells, which is tighter for cells near h.  DESIGN.md 4.2
+// has the argument, including the slack theta' - theta.
 //
-//   prune_hist_kernel   (band, k, b):   per cell of a 32-row band: bounding box + prefix histogram of direction pseudo-angles
+//   prune_hist_kernel   (band, k, b):   per sub-cell and cell of a 32-row band: bounding box + prefix histogram of
+//                                       direction pseudo-angles
 //   prune_bound_kernel  (h group, k, b): B(h), three threads per hypothesis -> key; the last CTA of (k, b) takes the
 //                                       PRUNE_M largest bounds -> list 0 (pass 1)
 //   vote_kernel         list 0
-//   prune_next_kernel   (k, b):         L = best pass-1 count; {h not in pass 1 : B(h) >= L} -> list 1 (pass 2)
+//   prune_next_kernel   (sub-cells, k, b): L = best pass-1 count; B2(h) of {h not in pass 1 : B(h) >= L}; the last CTA
+//                                       of (k, b) lists those with B2(h) >= L -> list 1 (pass 2)
 //   vote_list_kernel    list 1
 #include <cmath>
 #include <math_constants.h>
@@ -49,10 +53,15 @@ __device__ int first_row_at(const float2 *xy, int n, float y)
 }
 
 constexpr int HIST_THREADS = 256;
-constexpr int HIST_CELLS = 32;                 // cells of a band histogrammed at a time (16 KB of shared memory)
+constexpr int HIST_CELLS = 32;                 // cells of a band histogrammed at a time
+constexpr int HIST_SUBX = 2 * HIST_CELLS;      // their sub-cell columns; two sub-cell rows per band
+constexpr int HIST_SUBS = 2 * HIST_SUBX;       // 128 sub-cells x 64 words of two 16-bit bin counts: 32 KB
+static_assert(PRUNE_SUB * PRUNE_SUB < 65536, "a sub-cell's bin counts fit 16 bits");
 
 // One CTA per (band of PRUNE_CELL pixel rows, k, b).  The selected-pixel list is in raster (torch.nonzero) order, so the
-// band's pixels are one contiguous segment of it.  Every cell of the band gets a record, empty ones with total 0.
+// band's pixels are one contiguous segment of it.  The histogram and box are taken per sub-cell; every sub-cell and
+// every cell of the band gets a record, empty ones with total 0, and a cell's record is the union of its sub-cells'
+// (box: min / max of the same float bits; counts: sums), so it is what a histogram over the whole cell gives.
 __global__ void __launch_bounds__(HIST_THREADS)
 prune_hist_kernel(VoteArgs a, PruneArgs q)
 {
@@ -61,8 +70,9 @@ prune_hist_kernel(VoteArgs a, PruneArgs q)
     const size_t bk = (size_t)b * a.K + k;
     const float2 *xy = a.xy + (size_t)b * a.cap;
     const float2 *dk = a.dirs + bk * a.cap;
-    __shared__ __align__(16) int s_hist[HIST_CELLS][PRUNE_NBIN];
-    __shared__ int s_box[HIST_CELLS][4];                 // float bits of x0, x1, y0, y1: coordinates are >= 0
+    // [sub-cell row][sub-cell column][bin / 2]: bin 2j in the low half of word j, bin 2j + 1 in the high half
+    __shared__ __align__(16) int s_hist[2][HIST_SUBX][PRUNE_NBIN / 2];
+    __shared__ int s_box[2][HIST_SUBX][4];               // float bits of x0, x1, y0, y1: coordinates are >= 0
     __shared__ int s_seg[2];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     if (warp < 2) {
@@ -71,8 +81,10 @@ prune_hist_kernel(VoteArgs a, PruneArgs q)
     }
     for (int cx0 = 0; cx0 < q.ncx; cx0 += HIST_CELLS) {
         const int nc = min(HIST_CELLS, q.ncx - cx0);
-        for (int i = tid; i < HIST_CELLS * PRUNE_NBIN; i += HIST_THREADS) (&s_hist[0][0])[i] = 0;
-        if (tid < HIST_CELLS * 4) (&s_box[0][0])[tid] = __float_as_int((tid & 1) ? -CUDART_INF_F : CUDART_INF_F);
+        for (int i = tid; i < HIST_SUBS * PRUNE_NBIN / 8; i += HIST_THREADS)
+            reinterpret_cast<int4 *>(&s_hist[0][0][0])[i] = make_int4(0, 0, 0, 0);
+        for (int i = tid; i < HIST_SUBS * 4; i += HIST_THREADS)
+            (&s_box[0][0][0])[i] = __float_as_int((i & 1) ? -CUDART_INF_F : CUDART_INF_F);
         __syncthreads();
         const int s0 = s_seg[0], s1 = s_seg[1];
         float2 cn = make_float2(0.f, 0.f), vn = make_float2(0.f, 0.f);
@@ -81,59 +93,84 @@ prune_hist_kernel(VoteArgs a, PruneArgs q)
             const int i = i0 + lane;
             const float2 c = cn, v = vn;
             if (i + HIST_THREADS < s1) { cn = __ldg(xy + i + HIST_THREADS); vn = __ldg(dk + i + HIST_THREADS); }
-            int key = -1, hkey = -1, cx = 0;
+            int key = -1, hkey = -1, sc = 0;
             if (i < s1) {
-                cx = (int)c.x / PRUNE_CELL - cx0;
+                const int sx = (int)c.x / PRUNE_SUB - 2 * cx0, row = (int)c.y - band * PRUNE_CELL;
                 // the reference never lets a pixel vote whose norm1 is below 1e-6 or NaN (.cu:121), nor one whose norm1
                 // overflows (its cosine is then 0 or NaN): such pixels are left out of the box and the histogram
                 const float n1 = __fsqrt_rn(__fmaf_rn(v.x, v.x, __fmul_rn(v.y, v.y)));
-                if (cx >= 0 && cx < nc && n1 > below_1e6() && n1 < CUDART_INF_F) {
+                if (sx >= 0 && sx < 2 * nc && n1 > below_1e6() && n1 < CUDART_INF_F) {
                     const int bin = min(PRUNE_NBIN - 1, (int)(pseudo_angle<true>(v.x, v.y) * (PRUNE_NBIN / 4)));
-                    key = ((int)c.y - band * PRUNE_CELL) * HIST_CELLS + cx;
-                    hkey = cx * PRUNE_NBIN + bin;
+                    sc = (row / PRUNE_SUB) * HIST_SUBX + sx;
+                    key = row * HIST_SUBX + sx;
+                    hkey = sc * PRUNE_NBIN + bin;
                 }
             }
-            // neighbouring pixels mostly share a cell and a bin, and shared atomics on one address serialise: each run
-            // of lanes with equal (cell, bin) adds its length once
+            // neighbouring pixels mostly share a sub-cell and a bin, and shared atomics on one address serialise: each
+            // run of lanes with equal (sub-cell, bin) adds its length once, to its half of the word
             const int hprev = __shfl_up_sync(0xffffffffu, hkey, 1);
             const unsigned heads = __ballot_sync(0xffffffffu, lane == 0 || hprev != hkey);
             if (hkey >= 0 && (lane == 0 || hprev != hkey)) {
                 const unsigned later = heads & ~((2u << lane) - 1u);
-                atomicAdd(&(&s_hist[0][0])[hkey], (later ? __ffs(later) - 1 : 32) - lane);
+                atomicAdd(&(&s_hist[0][0][0])[hkey >> 1], ((later ? __ffs(later) - 1 : 32) - lane) << (16 * (hkey & 1)));
             }
-            // in raster order the lanes of one (row, cell) form runs sorted by x: only a run's first and last lane update
-            // the box
+            // in raster order the lanes of one (row, sub-cell) form runs sorted by x: only a run's first and last lane
+            // update the box
+            int *box = &s_box[0][0][0] + 4 * sc;
             const int prev = __shfl_up_sync(0xffffffffu, key, 1), next = __shfl_down_sync(0xffffffffu, key, 1);
             if (key >= 0 && (lane == 0 || prev != key)) {
-                atomicMin(&s_box[cx][0], __float_as_int(c.x));
-                atomicMin(&s_box[cx][2], __float_as_int(c.y));
+                atomicMin(box + 0, __float_as_int(c.x));
+                atomicMin(box + 2, __float_as_int(c.y));
             }
             if (key >= 0 && (lane == 31 || next != key)) {
-                atomicMax(&s_box[cx][1], __float_as_int(c.x));
-                atomicMax(&s_box[cx][3], __float_as_int(c.y));
+                atomicMax(box + 1, __float_as_int(c.x));
+                atomicMax(box + 3, __float_as_int(c.y));
             }
         }
         __syncthreads();
-        // one warp per cell: inclusive prefix of the 128 bins, four per lane, stored as 16-bit counts two per word
+        // one warp per cell: inclusive prefix of the 128 bins of each sub-cell, four per lane, stored as 16-bit counts two
+        // per word; the cell's record is their sum and the union of their boxes
         for (int cc = warp; cc < nc; cc += HIST_THREADS / 32) {
-            const int4 h = reinterpret_cast<const int4 *>(s_hist[cc])[lane];
-            int s = h.x + h.y + h.z + h.w;
+            const size_t cell = bk * q.ncells + (size_t)band * q.ncx + cx0 + cc;
+            int4 sum = make_int4(0, 0, 0, 0);
+            int bx = lane & 1 ? __float_as_int(-CUDART_INF_F) : __float_as_int(CUDART_INF_F);
 #pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int t = __shfl_up_sync(0xffffffffu, s, o);
-                if (lane >= o) s += t;
+            for (int j = 0; j < 4; ++j) {
+                const int sr = j >> 1, sx = 2 * cc + (j & 1);
+                const int2 w = reinterpret_cast<const int2 *>(s_hist[sr][sx])[lane];
+                const int h0 = w.x & 0xffff, h1 = (unsigned)w.x >> 16, h2 = w.y & 0xffff, h3 = (unsigned)w.y >> 16;
+                int s = h0 + h1 + h2 + h3;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    const int t = __shfl_up_sync(0xffffffffu, s, o);
+                    if (lane >= o) s += t;
+                }
+                const int4 p = make_int4(s - h3 - h2 - h1, s - h3 - h2, s - h3, s);
+                int *rec = q.sub + (cell * 4 + j) * PRUNE_REC;
+                // most sub-cells of an image are empty: their record is the last word alone (total 0), which is all
+                // that prune_next_kernel reads of them
+                const bool empty = __shfl_sync(0xffffffffu, s, 31) == 0;
+                if (!empty || lane == 31)
+                    reinterpret_cast<int2 *>(rec + 4)[lane] = make_int2(p.x | (p.y << 16), p.z | (p.w << 16));
+                if (lane < 4) {
+                    const int v = s_box[sr][sx][lane];
+                    if (!empty) rec[lane] = v;
+                    bx = lane & 1 ? max(bx, v) : min(bx, v);
+                }
+                sum.x += p.x; sum.y += p.y; sum.z += p.z; sum.w += p.w;
             }
-            const int p1 = s - h.w - h.z, p0 = p1 - h.y;
-            int *rec = q.cells + (bk * q.ncells + (size_t)band * q.ncx + cx0 + cc) * PRUNE_REC;
-            rec[4 + 2 * lane] = p0 | (p1 << 16);
-            rec[4 + 2 * lane + 1] = (s - h.w) | (s << 16);
-            if (lane < 4) rec[lane] = s_box[cc][lane];
+            int *rec = q.cells + cell * PRUNE_REC;
+            reinterpret_cast<int2 *>(rec + 4)[lane] = make_int2(sum.x | (sum.y << 16), sum.z | (sum.w << 16));
+            if (lane < 4) rec[lane] = bx;
         }
         __syncthreads();                                  // s_hist / s_box are reset for the next cells
     }
 }
 
 __device__ __forceinline__ int cell_total(const int *rec) { return (int)((unsigned)rec[PRUNE_REC - 1] >> 16); }
+
+// false for non-finite or huge hypotheses, which get no bound (B(h) = tn)
+__device__ __forceinline__ bool bounded(float2 h) { return fabsf(h.x) + fabsf(h.y) <= 1e15f; }
 
 // Pixels of a cell whose direction bin lies in [blo, bhi] (bins taken modulo PRUNE_NBIN; bhi - blo + 1 < PRUNE_NBIN)
 __device__ __forceinline__ int bins_between(const unsigned short *P, int blo, int bhi, int tot)
@@ -353,8 +390,8 @@ prune_bound_kernel(VoteArgs a, PruneArgs q)
     if (part == 0 && h < a.hn) {
 #pragma unroll
         for (int p = 1; p < BOUND_SPLIT; ++p) bound += s_part[p][hl];
-        // non-finite or huge: not bounded
-        q.key[bk * a.hn + h] = (fabsf(hp.x) + fabsf(hp.y) <= 1e15f) ? bound : tn;
+        q.key[bk * a.hn + h] = bounded(hp) ? bound : tn;
+        q.b2[bk * a.hn + h] = 0;                          // prune_next_kernel's CTAs add their sub-cells' parts to it
     }
     // q.ticket[bk] is 0 when the call starts (it lies in the workspace header) and is left 0 for the refit
     __threadfence();
@@ -369,7 +406,8 @@ prune_bound_kernel(VoteArgs a, PruneArgs q)
     plan_pass1(a, q, bk, &s_rec[0][0], &s_rec[0][0] + PRUNE_MAX_HN, s_w, s_sel);
 }
 
-constexpr int PLAN_THREADS = 1024;
+constexpr int NEXT_THREADS = 256;
+constexpr int NEXT_SUBS = 64;                  // sub-cells per CTA of prune_next_kernel, staged at once (17 KB)
 
 // exclusive prefix of `flag` over the CTA in thread order; returns it, *total gets the sum.  Every thread calls it.
 __device__ __forceinline__ int cta_scan(bool flag, int *s_warp, int *total)
@@ -380,7 +418,7 @@ __device__ __forceinline__ int cta_scan(bool flag, int *s_warp, int *total)
     if (lane == 0) s_warp[warp] = __popc(m);
     __syncthreads();
     int before = 0, tot = 0;
-    for (int w = 0; w < PLAN_THREADS / 32; ++w) {
+    for (int w = 0; w < NEXT_THREADS / 32; ++w) {
         const int c = s_warp[w];
         before += (w < warp) ? c : 0;
         tot += c;
@@ -389,29 +427,102 @@ __device__ __forceinline__ int cta_scan(bool flag, int *s_warp, int *total)
     return before + __popc(m & ((1u << lane) - 1u));
 }
 
-__global__ void __launch_bounds__(PLAN_THREADS)
+// One CTA per (NEXT_SUBS sub-cells, k, b).  L = the best exact count of pass 1; the candidates of pass 2 are the
+// hypotheses not in pass 1 with B(h) >= L.  Each CTA adds, for every candidate, the bound over the non-empty sub-cells
+// of its slice to b2 (count_bound over a finer partition of the same pixels: DESIGN.md 4.2); the last CTA of (b, k) to
+// finish lists pass 2 = {candidates with B2(h) >= L} in index order.  L = 0 excludes nothing and skips the sums.
+__global__ void __launch_bounds__(NEXT_THREADS)
 prune_next_kernel(VoteArgs a, PruneArgs q)
 {
-    const int k = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+    const int k = blockIdx.y, b = blockIdx.z, tid = threadIdx.x;
     const size_t bk = (size_t)b * a.K + k;
     const size_t BK = (size_t)a.B * a.K;
-    __shared__ int s_warp[PLAN_THREADS / 32];
-    __shared__ int s_max[PLAN_THREADS / 32];
-    const int *counts = a.counts + bk * a.hn;
+    const int hn = a.hn;
+    __shared__ __align__(16) int s_rec[NEXT_SUBS * PRUNE_REC];
+    __shared__ int s_cand[PRUNE_MAX_HN];
+    __shared__ int s_b2[PRUNE_MAX_HN];
+    __shared__ int s_idx[NEXT_SUBS];
+    __shared__ int s_warp[NEXT_THREADS / 32];
+    __shared__ int s_last;
+    const int *key = q.key + bk * hn;
+    const float2 *hyp = a.hyp + bk * hn;
+    int *b2 = q.b2 + bk * hn;
     // L = the best exact count of pass 1 (0 when nothing was scored: then nothing is excluded)
-    int best = 0;
-    const int n1 = q.len[bk];
-    for (int s = tid; s < n1; s += PLAN_THREADS) best = max(best, counts[q.list[bk * a.hn + s]]);
-    best = __reduce_max_sync(0xffffffffu, best);
-    if ((tid & 31) == 0) s_max[tid >> 5] = best;
+    auto pass1_best = [&]() {
+        const int *counts = a.counts + bk * hn;
+        int best = 0;
+        const int n1 = q.len[bk];
+        for (int s = tid; s < n1; s += NEXT_THREADS) best = max(best, counts[q.list[bk * hn + s]]);
+        best = __reduce_max_sync(0xffffffffu, best);
+        __syncthreads();                                  // s_warp is free
+        if ((tid & 31) == 0) s_warp[tid >> 5] = best;
+        __syncthreads();
+        int L = 0;
+        for (int w = 0; w < NEXT_THREADS / 32; ++w) L = max(L, s_warp[w]);
+        return L;
+    };
+    // the slice's non-empty sub-cells, staged while L and the candidates are found; a slice without any (most of an
+    // image) has nothing to add
+    const int *sub = q.sub + bk * q.ncells * 4 * PRUNE_REC;
+    const int c = blockIdx.x * NEXT_SUBS + tid;
+    const bool fc = tid < NEXT_SUBS && c < 4 * q.ncells && cell_total(sub + (size_t)c * PRUNE_REC) > 0;
+    int m;
+    const int pc = cta_scan(fc, s_warp, &m);
+    if (fc) s_idx[pc] = c;
+    int L = -1;
+    if (m > 0) {
+        __syncthreads();
+        for (int i = tid; i < m * REC_V4; i += NEXT_THREADS) {
+            const int r = i / REC_V4, w = (i - r * REC_V4) * 4;
+            cp_async16(s_rec + r * PRUNE_REC + w, sub + (size_t)s_idx[r] * PRUNE_REC + w);
+        }
+        cp_async_commit();
+        L = pass1_best();
+        // the candidates that have a bound (the others stay in pass 2)
+        int nc = 0;
+        for (int h0 = 0; h0 < hn && L > 0; h0 += NEXT_THREADS) {
+            const int h = h0 + tid;
+            const bool f = h < hn && key[h] >= L && bounded(hyp[h]);
+            int n;
+            const int pos = nc + cta_scan(f, s_warp, &n);
+            if (f) { s_cand[pos] = h; s_b2[pos] = 0; }
+            nc += n;
+        }
+        cp_async_wait<0>();
+        __syncthreads();
+        if (nc > 0) {
+            // P threads per candidate, each over a contiguous part of the staged records
+            const int P = max(1, NEXT_THREADS / nc);
+            for (int it = tid; it < nc * P; it += NEXT_THREADS) {
+                const int j = it % nc, p = it / nc;
+                const int r0 = p * m / P, r1 = (p + 1) * m / P;
+                if (r1 == r0) continue;
+                const float2 hp = hyp[s_cand[j]];
+                int bound = 0;
+                count_bound(q, s_rec + r0 * PRUNE_REC, r1 - r0, hp.x, hp.y, bound);
+                if (bound) atomicAdd(&s_b2[j], bound);
+            }
+            __syncthreads();
+            for (int j = tid; j < nc; j += NEXT_THREADS)
+                if (s_b2[j]) atomicAdd(&b2[s_cand[j]], s_b2[j]);
+        }
+    }
+    // q.ticket[bk] is 0 here (the bound step leaves it so) and is left 0 for the refit
+    __threadfence();
     __syncthreads();
-    int L = 0;
-    for (int w = 0; w < PLAN_THREADS / 32; ++w) L = max(L, s_max[w]);
-    int *list = q.list + (BK + bk) * a.hn;
+    if (tid == 0) {
+        s_last = (atomicAdd(q.ticket + bk, 1) == (int)gridDim.x - 1);
+        if (s_last) q.ticket[bk] = 0;
+    }
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    if (L < 0) L = pass1_best();
+    int *list = q.list + (BK + bk) * hn;
     int base = 0;
-    for (int h0 = 0; h0 < a.hn; h0 += PLAN_THREADS) {
+    for (int h0 = 0; h0 < hn; h0 += NEXT_THREADS) {
         const int h = h0 + tid;
-        const bool f = h < a.hn && q.key[bk * a.hn + h] >= L;
+        const bool f = h < hn && key[h] >= L && (L == 0 || !bounded(hyp[h]) || __ldcg(b2 + h) >= L);
         int n;
         const int pos = base + cta_scan(f, s_warp, &n);
         if (f) list[pos] = h;
@@ -448,7 +559,7 @@ cudaError_t launch_vote_pruned(const VoteArgs &a, const PruneArgs &q, cudaStream
     prune_bound_kernel<<<dim3((a.hn + BOUND_HYPS - 1) / BOUND_HYPS, a.K, a.B), BOUND_THREADS, 0, st>>>(a, q);
     cudaError_t e = launch_vote_list_slices(a, q.list, q.len, PRUNE_M, st);
     if (e != cudaSuccess) return e;
-    prune_next_kernel<<<dim3(a.K, a.B), PLAN_THREADS, 0, st>>>(a, q);
+    prune_next_kernel<<<dim3((4 * q.ncells + NEXT_SUBS - 1) / NEXT_SUBS, a.K, a.B), NEXT_THREADS, 0, st>>>(a, q);
     return launch_vote_list(a, q.list + BK * a.hn, q.len + BK, a.hn - PRUNE_M, st);
 }
 

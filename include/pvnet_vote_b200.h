@@ -140,7 +140,11 @@ typedef struct pvb_layout {
                              histogram of their direction pseudo-angles as uint16 */
     size_t prune_key;     /* int32[B][K][hn] angular upper bound of each hypothesis's count, -1 if scored in pass 1 */
     size_t prune_list;    /* int32[2][B][K][hn] hypotheses scored by pass 1 / pass 2 of the pruned v3 vote */
-    size_t prune_len;     /* int32[2][B][K] lengths of those lists */
+    size_t prune_len;     /* int32[2][B][K] lengths of those lists; followed, at the next multiple of 256 bytes, by
+                             int32[B][K][prune_ncells][4][68]: the records of each cell's four 16x16-pixel sub-cells (top
+                             left, top right, bottom left, bottom right), laid out as prune_cells except that only the
+                             last word (0) of an empty one is written; then, at the next multiple of 256 bytes,
+                             int32[B][K][hn]: for the pass-2 candidates, the bound over the sub-cells */
     int32_t nwords;  /* ceil(H*W/32) */
     int32_t nblocks; /* ceil(nwords/128) */
     int32_t capacity;
