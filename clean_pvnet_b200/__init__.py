@@ -15,6 +15,8 @@ Public surface (same names/signatures as the reference):
     vote_loss.vote_loss (the trainer's vote loss and its gradient from the mask and the keypoints), vote_target_batch (twin
     of lib/utils/pvnet/pvnet_data_utils.py's compute_vertex), NetworkWrapper (twin of lib/train/trainers/pvnet.py),
     install_vote_loss_as_reference
+    render.render_depth_batch (the depth image the T-LESS evaluator's OpenGL DepthRender renders, n poses per launch),
+    vsd_batch (T-LESS's VSD error for n pose pairs), install_depth_renderer_as_reference
 """
 from . import _lib  # noqa: F401
 from . import nn  # noqa: F401
@@ -30,6 +32,8 @@ from . import uncertainty_pnp as un_pnp  # noqa: F401
 from .uncertainty_pnp import uncertainty_pnp_batch, p3p_init_batch, uncertainty_pnp_from_votes  # noqa: F401
 from . import pose  # noqa: F401
 from .pose import pnp_batch  # noqa: F401
+from . import render  # noqa: F401
+from .render import render_depth_batch, vsd_batch, install_depth_renderer_as_reference  # noqa: F401
 from .vote_loss import vote_loss, vote_target_batch, NetworkWrapper, install_vote_loss_as_reference  # noqa: F401
 from .ransac_voting_gpu import (  # noqa: F401
     estimate_voting_distribution_with_mean,
@@ -47,4 +51,5 @@ __all__ = [
     "nn", "find_nearest_point_idx", "nearest_point_idx", "add_metric_batch", "install_nn_as_reference_module",
     "metrics", "pose_metrics_batch", "mask_iou_batch", "linemod_scores",
     "vote_loss", "vote_target_batch", "NetworkWrapper", "install_vote_loss_as_reference",
+    "render", "render_depth_batch", "vsd_batch", "install_depth_renderer_as_reference",
 ]

@@ -73,7 +73,13 @@ SIGNATURES = {
     "pvb_pose_metrics": (ctypes.c_int, [_vp, _vp, _vp, _vp, ctypes.c_int64, _vp, _vp, _vp, _i32, _i32, _vp, _sz, _vp]),
     "pvb_mask_iou": (ctypes.c_int, [_vp, _i32, ctypes.POINTER(ctypes.c_int64), _vp, _i32, ctypes.POINTER(ctypes.c_int64),
                                     _vp, _vp, _i32, _i32, _i32, _vp]),
-    "pvb_vote_target": (ctypes.c_int, [_vp, _i32, ctypes.POINTER(ctypes.c_int64), _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
+    "pvb_render_depth_workspace_bytes": (_sz, [_i32, _i32]),
+    "pvb_render_depth": (ctypes.c_int, [_vp, _i32, _vp, _i32, _vp, _i32, _vp, ctypes.c_int64, _vp, _i32, _i32,
+                                        ctypes.c_double, ctypes.c_double, _vp, _sz, _vp]),
+    "pvb_vsd_workspace_bytes": (_sz, [_i32]),
+    "pvb_vsd": (ctypes.c_int, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _vp, _i32, _vp, ctypes.c_int64, _i32, _i32,
+                               ctypes.c_double, ctypes.c_double, _vp, _vp, _sz, _vp]),
+    "pvb_vote_target":(ctypes.c_int, [_vp, _i32, ctypes.POINTER(ctypes.c_int64), _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
     "pvb_vote_loss_workspace_bytes": (_sz, [_i32, _i32, _i32]),
     "pvb_vote_loss_forward": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int64), _vp, _i32, ctypes.POINTER(ctypes.c_int64),
                                              _vp, _vp, _i32, _i32, _i32, _i32, _vp, _sz, _vp]),

@@ -616,6 +616,62 @@ PVB_API int pvb_mask_iou(const void *pred, int32_t pred_dtype, const int64_t *pr
     return e == cudaSuccess ? PVB_OK : cuda_fail(e, "mask iou kernel");
 }
 
+PVB_API size_t pvb_render_depth_workspace_bytes(int32_t n, int32_t F)
+{
+    if (n <= 0 || F <= 0 || (long long)n * F > 0x7fffffffll) return 0;
+    return render_workspace_bytes(n, F);
+}
+
+PVB_API int pvb_render_depth(const float *pts, int32_t V, const int32_t *faces, int32_t F, const double *poses, int32_t n,
+                             const double *K, int64_t k_stride, float *depth, int32_t H, int32_t W, double clip_near,
+                             double clip_far, void *workspace, size_t workspace_bytes, pvb_stream_t stream)
+{
+    if (n < 0 || V < 0 || F < 0 || H < 0 || W < 0)
+        return fail(PVB_ERR_INVALID, "negative size (n=%d V=%d F=%d H=%d W=%d)", n, V, F, H, W);
+    if (!(clip_near > 0.0) || !(clip_far >= clip_near) || !std::isfinite(clip_far))
+        return fail(PVB_ERR_INVALID, "need 0 < near <= far < inf (got %g, %g)", clip_near, clip_far);
+    if ((long long)H * W > 0x7fffffffll) return fail(PVB_ERR_INVALID, "image too large (H*W >= 2^31)");
+    if ((long long)n * F > 0x7fffffffll) return fail(PVB_ERR_INVALID, "n * F too large (>= 2^31)");
+    if (n > 65535) return fail(PVB_ERR_INVALID, "n must be <= 65535 (got %d)", n);
+    if (n == 0 || (long long)H * W == 0) return PVB_OK;
+    if (!poses || !K || !depth || (F > 0 && (!faces || (V > 0 && !pts)))) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (k_stride < 0) return fail(PVB_ERR_INVALID, "negative stride");
+    if (F > 0)
+        if (int rc = nn_check_workspace(render_workspace_bytes(n, F), workspace, workspace_bytes)) return rc;
+    cudaError_t e = launch_render_depth(pts, V, faces, F, poses, n, K, k_stride, depth, H, W, clip_near, clip_far, workspace,
+                                        static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "depth render kernels");
+}
+
+PVB_API size_t pvb_vsd_workspace_bytes(int32_t n)
+{
+    if (n <= 0) return 0;
+    return vsd_workspace_bytes(n);
+}
+
+PVB_API int pvb_vsd(const float *depth_test, int32_t B, const float *depth_est, int32_t n_est, int32_t est_base,
+                    const float *depth_gt, int32_t n_gt, int32_t gt_base, const int32_t *pairs, int32_t n, const double *K,
+                    int64_t k_stride, int32_t H, int32_t W, double delta, double tau, double *e, void *workspace,
+                    size_t workspace_bytes, pvb_stream_t stream)
+{
+    if (n < 0 || B < 0 || n_est < 0 || n_gt < 0 || H < 0 || W < 0)
+        return fail(PVB_ERR_INVALID, "negative size (n=%d B=%d n_est=%d n_gt=%d H=%d W=%d)", n, B, n_est, n_gt, H, W);
+    if ((long long)H * W > 0x7fffffffll) return fail(PVB_ERR_INVALID, "image too large (H*W >= 2^31)");
+    if (std::isnan(delta) || std::isnan(tau)) return fail(PVB_ERR_INVALID, "delta and tau must not be NaN");
+    if (n == 0) return PVB_OK;
+    const bool px = (long long)H * W > 0;
+    if (!pairs || !e || !K || (px && ((B > 0 && !depth_test) || (n_est > 0 && !depth_est) || (n_gt > 0 && !depth_gt))))
+        return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (k_stride < 0) return fail(PVB_ERR_INVALID, "negative stride");
+    if (int rc = nn_check_workspace(vsd_workspace_bytes(n), workspace, workspace_bytes)) return rc;
+    VsdArgs a;
+    a.depth_test = depth_test; a.depth_est = depth_est; a.depth_gt = depth_gt; a.pairs = pairs; a.K = K;
+    a.k_stride = k_stride; a.n = n; a.B = B; a.n_est = n_est; a.n_gt = n_gt; a.est_base = est_base; a.gt_base = gt_base;
+    a.H = H; a.W = W; a.delta = delta; a.tau = tau; a.e = e;
+    cudaError_t err = launch_vsd(a, workspace, static_cast<cudaStream_t>(stream));
+    return err == cudaSuccess ? PVB_OK : cuda_fail(err, "vsd kernels");
+}
+
 namespace {
 
 constexpr int VOTE_LOSS_MAX_K = 1024;      // the image's keypoints live in 16 KB of shared memory

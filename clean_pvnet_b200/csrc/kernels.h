@@ -168,6 +168,25 @@ cudaError_t launch_pose_metrics(const double *model, const double *pose_pred, co
 cudaError_t launch_mask_iou(const void *pred, int pred_dtype, const long long *ps, const void *gt, int gt_dtype,
                             const long long *gs, long long *inter, long long *uni, int B, int H, int W, cudaStream_t st);
 
+// T-LESS's VSD (render.cu, DESIGN.md 8f).  Depth rasterizer: pts [V][3] fp32, faces [F][3] int32, poses [n][3][4] fp64,
+// K [3][3] fp64 at K + pose * k_stride -> depth [n][H][W] fp32.  Workspace: a queue counter, then n * F queue entries.
+size_t render_workspace_bytes(int n, int F);
+cudaError_t launch_render_depth(const float *pts, int V, const int *faces, int F, const double *poses, int n,
+                                const double *K, long long k_stride, float *depth, int H, int W, double znear,
+                                double zfar, void *workspace, cudaStream_t st);
+struct VsdArgs {
+    const float *depth_test, *depth_est, *depth_gt;  // [B][H][W], [n_est][H][W], [n_gt][H][W]
+    const int *pairs;                                // [n][3]: est index, gt index, image index
+    const double *K;                                 // [3][3] per image at K + image * k_stride
+    long long k_stride;
+    int n, B, n_est, n_gt, est_base, gt_base, H, W;  // rows use est in [est_base, est_base + n_est), likewise gt
+    double delta, tau;
+    double *e;                                       // [n]: written only for rows within the windows
+};
+// workspace: the integer counts of the n rows
+size_t vsd_workspace_bytes(int n);
+cudaError_t launch_vsd(const VsdArgs &a, void *workspace, cudaStream_t st);
+
 // PVNet's vote loss (loss.cu, DESIGN.md 8e): the target field of compute_vertex, the trainer's smooth-l1 vote loss and its
 // gradient, from the mask and the keypoints.  One thread per pixel over a (ceil(H*W / 256), B) grid; the image's keypoints
 // are staged in shared memory.

@@ -33,6 +33,9 @@
  *   evaluators/linemod/pvnet.py:84-94  cm_degree_5_metric,
  *   evaluators/tless_test/pvnet.py:119-125  cm_degree_5_metric     pvb_pose_metrics (n pose pairs per call)
  *   evaluators/linemod/pvnet.py:96-100  mask_iou                   pvb_mask_iou (B images per call)
+ *   utils/renderer/opengl_utils.py:405-490  DepthRender.render     pvb_render_depth (n poses per call, no OpenGL)
+ *   utils/vsd/vsd_utils.py:5-48  vsd (cost 'step'), as
+ *   evaluators/tless_test/pvnet.py:66-105  vsd_metric calls it     pvb_vsd (n pose pairs per call)
  *
  *   and the training side of the vote field:
  *   utils/pvnet/pvnet_data_utils.py:30-44  compute_vertex          pvb_vote_target (B images per call)
@@ -336,6 +339,49 @@ PVB_API int pvb_pose_metrics(const double *model, const double *pose_pred, const
 PVB_API int pvb_mask_iou(const void *pred, int32_t pred_dtype, const int64_t *pred_stride, const void *gt, int32_t gt_dtype,
                          const int64_t *gt_stride, int64_t *inter, int64_t *uni, int32_t B, int32_t H, int32_t W,
                          pvb_stream_t stream);
+
+/* ---- T-LESS's VSD without OpenGL (DESIGN.md section 8f) ------------------------------------------------------------
+ * Depth rendering: replaces lib/utils/renderer/opengl_utils.py:405-490 (DepthRender.render, which the T-LESS evaluator
+ * calls as render((720, 540), 100, 10000, K, R, t * 1000) at tless_test/pvnet.py:85, :93) and the depth mode of
+ * lib/utils/vsd/renderer.py's render.  For each of n poses:
+ *   R, t are rounded to fp32 (the shader's float32 view matrix), model points go to the camera frame in fp64, and pixel
+ *   (row r, column c) samples the ray through (u, v) = (c + 0.5, r + 0.5), u = fx X/Z + s Y/Z + cx, v = fy Y/Z + cy.  The
+ *   pixel holds the camera-frame Z of the nearest triangle along that ray with clip_near <= Z <= clip_far, rounded to fp32,
+ *   or 0.  No culling; triangles crossing the near plane or behind the camera are clipped, never projected through 0.
+ *   Coverage is watertight: a pixel centre on an edge or vertex shared by triangles is covered by one of them.
+ *   pts device fp32 [V,3], faces device int32 [F,3] (a face with an index outside [0, V) is skipped), poses device fp64
+ *   [n,3,4] ([R|t], in the units of pts), K device fp64 [3,3] row-major for pose i at K + i * k_stride (0 = shared; only
+ *   fx, s, cx, fy, cy are read, like _compute_calib_proj), depth device fp32 [n,H,W], fully written.  The result is
+ *   bit-identical run to run and a pose's image does not depend on the other poses.
+ *   n <= 65535, n * F < 2^31, H * W < 2^31, 0 < clip_near <= clip_far < inf.  workspace:
+ *   pvb_render_depth_workspace_bytes(n, F) bytes of 256-byte aligned device memory (0 -- and NULL allowed -- when F == 0).
+ * Bad arguments return PVB_ERR_INVALID, a missing or short workspace PVB_ERR_WORKSPACE, both before any CUDA call. */
+PVB_API size_t pvb_render_depth_workspace_bytes(int32_t n, int32_t F);
+PVB_API int pvb_render_depth(const float *pts, int32_t V, const int32_t *faces, int32_t F, const double *poses, int32_t n,
+                             const double *K, int64_t k_stride, float *depth, int32_t H, int32_t W, double clip_near,
+                             double clip_far, void *workspace, size_t workspace_bytes, pvb_stream_t stream);
+
+/* VSD: replaces vsd_utils.vsd (lib/utils/vsd/vsd_utils.py:5-48) with cost 'step', together with the distance images
+ * (misc.depth_im_to_dist_im, lib/utils/vsd/misc.py:42-60) and visibility masks (lib/utils/vsd/visibility.py:6-29) that
+ * Evaluator.vsd_metric (tless_test/pvnet.py:66-105) builds for it, for n rows (est, gt, image) of `pairs`:
+ *   dist = sqrt((X*X + Y*Y) + Z*Z), X = ((c - cx) * Z) * (1/fx), Y = ((r - cy) * Z) * (1/fy) in fp64, each step rounded on
+ *   its own as numpy does, at the integer pixel coordinate (c, r);
+ *   vg = dist_test > 0 & dist_gt > 0 & float(dist_gt) - float(dist_test) <= float(delta)
+ *   ve = (dist_test > 0 & dist_est > 0 & float(dist_est) - float(dist_test) <= float(delta)) | (vg & dist_est > 0)
+ *   e  = (#(vg & ve & |dist_gt - dist_est| >= tau) + #(vg | ve) - #(vg & ve)) / #(vg | ve), 1.0 for an empty union.
+ *   depth_test device fp32 [B,H,W] (the evaluator's load_depth(path) * 0.1), depth_est fp32 [n_est,H,W] and depth_gt fp32
+ *   [n_gt,H,W] (pvb_render_depth), pairs device int32 [n,3], K device fp64 [3,3] of image b at K + b * k_stride.  Row i
+ *   uses depth_est[pairs[i][0] - est_base] and depth_gt[pairs[i][1] - gt_base]; a row whose indices fall outside
+ *   [est_base, est_base + n_est), [gt_base, gt_base + n_gt) or [0, B) is left untouched in e (device fp64 [n]), so a
+ *   caller can render the poses in windows and call once per window pair.  No distance image or mask is stored; the
+ *   counts are integers, so e is exact and deterministic.  The `e < 0.3` test and the any-of over an image's rows stay
+ *   with the caller.  workspace: pvb_vsd_workspace_bytes(n) bytes of 256-byte aligned device memory.  n == 0 is a no-op.
+ * Bad arguments return PVB_ERR_INVALID, a missing or short workspace PVB_ERR_WORKSPACE, both before any CUDA call. */
+PVB_API size_t pvb_vsd_workspace_bytes(int32_t n);
+PVB_API int pvb_vsd(const float *depth_test, int32_t B, const float *depth_est, int32_t n_est, int32_t est_base,
+                    const float *depth_gt, int32_t n_gt, int32_t gt_base, const int32_t *pairs, int32_t n, const double *K,
+                    int64_t k_stride, int32_t H, int32_t W, double delta, double tau, double *e, void *workspace,
+                    size_t workspace_bytes, pvb_stream_t stream);
 
 /* ---- training: PVNet's vote loss from the mask and the keypoints (DESIGN.md section 8e) ----------------------------
  * The trainer supervises the unit-vector field with a dense target that every dataset builds on the host
