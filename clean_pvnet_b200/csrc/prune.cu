@@ -24,14 +24,19 @@
 
 namespace pvb {
 
-// Monotone pseudo-angle of a non-zero direction, in [0, 4] counter-clockwise from +x (one unit per quadrant).  The bound
-// divides approximately; the histogram divides with IEEE rounding (EXACT), so its bins are reproducible bit for bit.
+// Monotone pseudo-angle of a non-zero direction, in [0, 4] counter-clockwise from +x (one unit per quadrant): y / (x + y),
+// 1 + -x / (y - x), 2 + -y / (-x - y), 3 + x / (x - y).  The denominator is |x| + |y| and the numerator |y| or |x| in
+// every quadrant, the same values bit for bit, so the quadrant only selects them and the offset and one division follows:
+// no branch, which matters where a warp's directions lie in different quadrants.  (Quadrant 0 can give +0 where the
+// per-quadrant form gives -0; every caller maps both to bin 0.)  The bound divides approximately; the histogram divides
+// with IEEE rounding (EXACT), so its bins are reproducible bit for bit.
 template <bool EXACT = false>
 __device__ __forceinline__ float pseudo_angle(float x, float y)
 {
-    auto div = [](float a, float b) { return EXACT ? __fdiv_rn(a, b) : __fdividef(a, b); };
-    if (y >= 0.f) return x >= 0.f ? div(y, x + y) : 1.f + div(-x, y - x);
-    return x < 0.f ? 2.f + div(-y, -x - y) : 3.f + div(x, x - y);
+    const bool xn = x < 0.f, yn = y < 0.f;
+    const float num = (xn == yn) ? fabsf(y) : fabsf(x), den = fabsf(x) + fabsf(y);
+    const float off = yn ? (xn ? 2.f : 3.f) : (xn ? 1.f : 0.f);
+    return off + (EXACT ? __fdiv_rn(num, den) : __fdividef(num, den));
 }
 
 // First index i in [0, n) with xy[i].y >= y (n if none); xy is sorted by y.  Warp-cooperative 32-ary search: three rounds
@@ -175,16 +180,19 @@ __device__ __forceinline__ bool bounded(float2 h) { return fabsf(h.x) + fabsf(h.
 // Pixels of a cell whose direction bin lies in [blo, bhi] (bins taken modulo PRUNE_NBIN; bhi - blo + 1 < PRUNE_NBIN)
 __device__ __forceinline__ int bins_between(const unsigned short *P, int blo, int bhi, int tot)
 {
-    // C(j) = pixels with (unwrapped) bin < j = P[j mod NB - 1] + tot * floor(j / NB)
+    // C(j) = pixels with (unwrapped) bin < j = P[j mod NB - 1] + tot * floor(j / NB); on two's complement the floor
+    // division and the modulo are a shift and a mask
+    static_assert(PRUNE_NBIN == 128, "bins_between shifts by log2(PRUNE_NBIN)");
     auto C = [&](int j) {
-        const int w = (j >= 0) ? j / PRUNE_NBIN : -((PRUNE_NBIN - 1 - j) / PRUNE_NBIN);
-        const int r = j - w * PRUNE_NBIN;
-        return (r ? (int)P[r - 1] : 0) + tot * w;
+        const int r = j & (PRUNE_NBIN - 1);
+        return (r ? (int)P[r - 1] : 0) + tot * (j >> 7);
     };
     return C(bhi + 1) - C(blo);
 }
 
-// Adds to `bound` the bound of h over nt cell records `rec` (shared memory)
+// Adds to `bound` the bound of h over nt cell records `rec` (shared memory).  The window is computed for every record and
+// the two whole-record cases (h inside the box, a window of every bin) select the total afterwards, so a warp whose
+// hypotheses fall in different cases does not diverge; the window's table reads stay inside the record for any input.
 __device__ void count_bound(const PruneArgs &q, const int *rec, int nt, float hx, float hy, int &bound)
 {
     const float c = q.cos_w, s = q.sin_w;
@@ -193,9 +201,9 @@ __device__ void count_bound(const PruneArgs &q, const int *rec, int nt, float hx
         const float x0 = __int_as_float(rec[0]), x1 = __int_as_float(rec[1]);
         const float y0 = __int_as_float(rec[2]), y1 = __int_as_float(rec[3]);
         const int tot = cell_total(rec);
-        if (hx >= x0 - 0.5f && hx <= x1 + 0.5f && hy >= y0 - 0.5f && hy <= y1 + 0.5f) { bound += tot; continue; }
-        // h is at least half a pixel outside the box: the directions h - corner lie in an open half-plane, where
-        // "counter-clockwise of" (cross product > 0) orders them; lo / hi are the extreme ones
+        const bool inside = hx >= x0 - 0.5f && hx <= x1 + 0.5f && hy >= y0 - 0.5f && hy <= y1 + 0.5f;
+        // unless inside, h is at least half a pixel outside the box: the directions h - corner lie in an open
+        // half-plane, where "counter-clockwise of" (cross product > 0) orders them; lo / hi are the extreme ones
         float lx = hx - x0, ly = hy - y0, ux = lx, uy = ly;
         const float cx[3] = {x1, x0, x1}, cy[3] = {y0, y1, y1};
 #pragma unroll
@@ -208,23 +216,22 @@ __device__ void count_bound(const PruneArgs &q, const int *rec, int nt, float hx
         const float plo = pseudo_angle(c * lx + s * ly, c * ly - s * lx);
         float phi = pseudo_angle(c * ux - s * uy, c * uy + s * ux);
         if (phi < plo) phi += 4.f;
-        const int blo = (int)floorf((plo - EPS) * (PRUNE_NBIN / 4));
-        const int bhi = (int)floorf((phi + EPS) * (PRUNE_NBIN / 4));
-        bound += (bhi - blo + 1 >= PRUNE_NBIN)
-                     ? tot : bins_between(reinterpret_cast<const unsigned short *>(rec + 4), blo, bhi, tot);
+        const int blo = __float2int_rd((plo - EPS) * (PRUNE_NBIN / 4));
+        const int bhi = __float2int_rd((phi + EPS) * (PRUNE_NBIN / 4));
+        const int win = bins_between(reinterpret_cast<const unsigned short *>(rec + 4), blo, bhi, tot);
+        bound += (inside || bhi - blo + 1 >= PRUNE_NBIN) ? tot : win;
     }
 }
 
 constexpr int BOUND_HYPS = 64;                 // hypotheses per CTA
-constexpr int BOUND_SPLIT = 3;                 // threads per hypothesis, each over a third of every staged chunk: one
+constexpr int BOUND_SPLIT = 4;                 // threads per hypothesis, each over a quarter of every staged chunk: one
                                                // thread per hypothesis leaves too few warps to hide the latency
 constexpr int BOUND_THREADS = BOUND_HYPS * BOUND_SPLIT;
 constexpr int BOUND_WARPS = BOUND_THREADS / 32;
-constexpr int BOUND_SCAN = 3 * BOUND_THREADS;  // cell totals read per listing round, three per thread
-constexpr int BOUND_CELLS = 32;                // non-empty cell records per staged chunk; two chunks in flight (17 KB)
+constexpr int STAGE_RECS = 32;                 // non-empty records per staged chunk; two chunks in flight (17 KB)
 constexpr int REC_V4 = PRUNE_REC / 4;          // 16-byte pieces of a record
 static_assert(PRUNE_REC % 4 == 0, "records are staged in 16-byte pieces");
-static_assert(PRUNE_MAX_HN + 256 <= 2 * BOUND_CELLS * PRUNE_REC, "the pass-1 selection fits in the record buffers");
+static_assert(PRUNE_MAX_HN + 256 <= 2 * STAGE_RECS * PRUNE_REC, "the pass-1 selection fits in the record buffers");
 
 __device__ __forceinline__ void cp_async16(void *smem, const void *gmem)
 {
@@ -233,6 +240,63 @@ __device__ __forceinline__ void cp_async16(void *smem, const void *gmem)
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" :: "n"(N) : "memory"); }
+
+// Streams the non-empty ones of the records rec + c * stride (c < nrec; an empty one adds nothing to a bound) through
+// shared memory and calls use(records, n) with every thread of the CTA for each chunk of n <= STAGE_RECS of them.  The
+// CTA lists the non-empty records 3 x THREADS at a time (empty ones cost one word read), then stages their records with
+// cp.async one chunk ahead of the chunk in use.  Within a listing round the order is not the index order, which no
+// integer sum over the records sees.  s_rec holds 2 x STAGE_RECS records, s_idx 3 x THREADS ints, s_w THREADS / 32.
+template <int THREADS, typename Use>
+__device__ __forceinline__ void stream_records(const int *rec, int stride, int nrec, int *s_rec, int *s_idx, int *s_w,
+                                               Use use)
+{
+    constexpr int WARPS = THREADS / 32, SCAN = 3 * THREADS;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    for (int c0 = 0; c0 < nrec; c0 += SCAN) {
+        bool f[3];
+        unsigned bal[3];
+        int cnt = 0;
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            const int c = c0 + j * THREADS + tid;
+            f[j] = c < nrec && cell_total(rec + (size_t)c * stride) > 0;
+        }
+#pragma unroll
+        for (int j = 0; j < 3; ++j) { bal[j] = __ballot_sync(0xffffffffu, f[j]); cnt += __popc(bal[j]); }
+        if (lane == 0) s_w[warp] = cnt;
+        __syncthreads();
+        int base = 0, m = 0;
+        for (int w = 0; w < WARPS; ++w) {
+            const int c = s_w[w];
+            base += (w < warp) ? c : 0;
+            m += c;
+        }
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            if (f[j]) s_idx[base + __popc(bal[j] & ((1u << lane) - 1u))] = c0 + j * THREADS + tid;
+            base += __popc(bal[j]);
+        }
+        __syncthreads();
+        const int nch = (m + STAGE_RECS - 1) / STAGE_RECS;
+        auto stage = [&](int ch) {
+            const int r0 = ch * STAGE_RECS, n = min(STAGE_RECS, m - r0);
+            int *dst = s_rec + (ch & 1) * STAGE_RECS * PRUNE_REC;
+            for (int i = tid; i < n * REC_V4; i += THREADS) {
+                const int r = i / REC_V4, w = (i - r * REC_V4) * 4;
+                cp_async16(dst + r * PRUNE_REC + w, rec + (size_t)s_idx[r0 + r] * stride + w);
+            }
+            cp_async_commit();
+        };
+        if (nch > 0) stage(0);
+        for (int ch = 0; ch < nch; ++ch) {
+            if (ch + 1 < nch) { stage(ch + 1); cp_async_wait<1>(); }
+            else cp_async_wait<0>();
+            __syncthreads();
+            use(s_rec + (ch & 1) * STAGE_RECS * PRUNE_REC, min(STAGE_RECS, m - ch * STAGE_RECS));
+            __syncthreads();                              // the buffer is restaged two chunks on; s_idx, s_w next round
+        }
+    }
+}
 
 // Pass 1 of (b, k): the PRUNE_M largest bounds, ties in index order, listed in index order; their keys become -1.
 // Called by every thread of the CTA once all of the (image, keypoint)'s bounds are in q.key.  s_key holds hn ints,
@@ -320,71 +384,28 @@ __device__ void plan_pass1(const VoteArgs &a, const PruneArgs &q, size_t bk, int
     if (tid == 0) q.len[bk] = M;
 }
 
-// One CTA per (BOUND_HYPS hypotheses, k, b).  The CTA lists the non-empty cells (an empty one adds nothing), stages
-// their records in shared memory a chunk ahead of the one it computes on, and sums B(h) over them; the last CTA of
-// (b, k) to finish then picks pass 1 (plan_pass1), so no launch waits for the slowest one.
-__global__ void __launch_bounds__(BOUND_THREADS, 10)
+// One CTA per (BOUND_HYPS hypotheses, k, b).  The CTA streams the non-empty cells' records (stream_records) and sums
+// B(h) over them; the last CTA of (b, k) to finish then picks pass 1 (plan_pass1), so no launch waits for the slowest one.
+__global__ void __launch_bounds__(BOUND_THREADS, 2048 / BOUND_THREADS)
 prune_bound_kernel(VoteArgs a, PruneArgs q)
 {
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const int part = tid / BOUND_HYPS, hl = tid % BOUND_HYPS;
     const int h = blockIdx.x * BOUND_HYPS + hl, k = blockIdx.y, b = blockIdx.z;
     const size_t bk = (size_t)b * a.K + k;
     const int tn = max(0, min(a.tn[b], a.cap));
-    __shared__ __align__(16) int s_rec[2][BOUND_CELLS * PRUNE_REC];
-    __shared__ int s_idx[BOUND_SCAN];
+    __shared__ __align__(16) int s_rec[2][STAGE_RECS * PRUNE_REC];
+    __shared__ int s_idx[3 * BOUND_THREADS];
     __shared__ int s_part[BOUND_SPLIT][BOUND_HYPS];
     __shared__ int s_w[2 * BOUND_WARPS];
     __shared__ int s_sel[2];
     const float2 hp = (h < a.hn) ? a.hyp[bk * a.hn + h] : make_float2(0.f, 0.f);
-    const int *rec = q.cells + bk * q.ncells * PRUNE_REC;
     int bound = 0;
-    for (int c0 = 0; c0 < q.ncells; c0 += BOUND_SCAN) {
-        bool f[3];
-        unsigned bal[3];
-        int cnt = 0;
-#pragma unroll
-        for (int j = 0; j < 3; ++j) {
-            const int c = c0 + j * BOUND_THREADS + tid;
-            f[j] = c < q.ncells && cell_total(rec + (size_t)c * PRUNE_REC) > 0;
-        }
-#pragma unroll
-        for (int j = 0; j < 3; ++j) { bal[j] = __ballot_sync(0xffffffffu, f[j]); cnt += __popc(bal[j]); }
-        if (lane == 0) s_w[warp] = cnt;
-        __syncthreads();
-        int base = 0, m = 0;
-        for (int w = 0; w < BOUND_WARPS; ++w) {
-            const int c = s_w[w];
-            base += (w < warp) ? c : 0;
-            m += c;
-        }
-#pragma unroll
-        for (int j = 0; j < 3; ++j) {                     // the order of the list does not change an integer sum
-            if (f[j]) s_idx[base + __popc(bal[j] & ((1u << lane) - 1u))] = c0 + j * BOUND_THREADS + tid;
-            base += __popc(bal[j]);
-        }
-        __syncthreads();
-        const int nch = (m + BOUND_CELLS - 1) / BOUND_CELLS;
-        auto stage = [&](int ch) {
-            const int r0 = ch * BOUND_CELLS, n = min(BOUND_CELLS, m - r0);
-            int *dst = s_rec[ch & 1];
-            for (int i = tid; i < n * REC_V4; i += BOUND_THREADS) {
-                const int r = i / REC_V4, w = (i - r * REC_V4) * 4;
-                cp_async16(dst + r * PRUNE_REC + w, rec + (size_t)s_idx[r0 + r] * PRUNE_REC + w);
-            }
-            cp_async_commit();
-        };
-        if (nch > 0) stage(0);
-        for (int ch = 0; ch < nch; ++ch) {
-            if (ch + 1 < nch) { stage(ch + 1); cp_async_wait<1>(); }
-            else cp_async_wait<0>();
-            __syncthreads();
-            const int n = min(BOUND_CELLS, m - ch * BOUND_CELLS);
-            const int r0 = part * n / BOUND_SPLIT, r1 = (part + 1) * n / BOUND_SPLIT;
-            count_bound(q, s_rec[ch & 1] + r0 * PRUNE_REC, r1 - r0, hp.x, hp.y, bound);
-            __syncthreads();                              // the buffer is restaged two chunks on; s_idx, s_w next round
-        }
-    }
+    stream_records<BOUND_THREADS>(q.cells + bk * q.ncells * PRUNE_REC, PRUNE_REC, q.ncells, &s_rec[0][0], s_idx, s_w,
+                                  [&](const int *rec, int n) {
+        const int r0 = part * n / BOUND_SPLIT, r1 = (part + 1) * n / BOUND_SPLIT;
+        count_bound(q, rec + r0 * PRUNE_REC, r1 - r0, hp.x, hp.y, bound);
+    });
     if (part > 0) s_part[part][hl] = bound;
     __syncthreads();
     if (part == 0 && h < a.hn) {
@@ -407,7 +428,11 @@ prune_bound_kernel(VoteArgs a, PruneArgs q)
 }
 
 constexpr int NEXT_THREADS = 256;
-constexpr int NEXT_SUBS = 64;                  // sub-cells per CTA of prune_next_kernel, staged at once (17 KB)
+constexpr int NEXT_CTAS = 8;                   // CTAs per (image, keypoint): CTA x takes the sub-cells s = x mod NEXT_CTAS
+                                               // (with 4 sub-cells per cell, one quadrant of every cell or every other)
+// per candidate of pass 2 in prune_next_kernel's dynamic shared memory: its hypothesis, its B2 part and its index
+constexpr int NEXT_CAND_BYTES = sizeof(float2) + sizeof(int) + sizeof(unsigned short);
+static_assert(PRUNE_MAX_HN <= 65536, "candidate indices fit 16 bits");
 
 // exclusive prefix of `flag` over the CTA in thread order; returns it, *total gets the sum.  Every thread calls it.
 __device__ __forceinline__ int cta_scan(bool flag, int *s_warp, int *total)
@@ -427,85 +452,73 @@ __device__ __forceinline__ int cta_scan(bool flag, int *s_warp, int *total)
     return before + __popc(m & ((1u << lane) - 1u));
 }
 
-// One CTA per (NEXT_SUBS sub-cells, k, b).  L = the best exact count of pass 1; the candidates of pass 2 are the
-// hypotheses not in pass 1 with B(h) >= L.  Each CTA adds, for every candidate, the bound over the non-empty sub-cells
-// of its slice to b2 (count_bound over a finer partition of the same pixels: DESIGN.md 4.2); the last CTA of (b, k) to
-// finish lists pass 2 = {candidates with B2(h) >= L} in index order.  L = 0 excludes nothing and skips the sums.
+// NEXT_CTAS CTAs per (k, b); dynamic shared memory: NEXT_CAND_BYTES x (hn - PRUNE_M).  L = the best exact count of
+// pass 1; the candidates of pass 2 are the hypotheses not in pass 1 with B(h) >= L, at most hn - PRUNE_M.  Each CTA
+// finds L and the candidates once, keeps their hypotheses in shared memory, streams the non-empty ones of its sub-cells
+// (stream_records) and adds, for every candidate, the bound over them to b2 (count_bound over a
+// finer partition of the same pixels: DESIGN.md 4.2); the last CTA of (b, k) to finish lists pass 2 = {candidates with
+// B2(h) >= L} in index order.  L = 0 excludes nothing and skips the sums.
 __global__ void __launch_bounds__(NEXT_THREADS)
 prune_next_kernel(VoteArgs a, PruneArgs q)
 {
-    const int k = blockIdx.y, b = blockIdx.z, tid = threadIdx.x;
+    const int x = blockIdx.x, k = blockIdx.y, b = blockIdx.z, tid = threadIdx.x;
     const size_t bk = (size_t)b * a.K + k;
     const size_t BK = (size_t)a.B * a.K;
     const int hn = a.hn;
-    __shared__ __align__(16) int s_rec[NEXT_SUBS * PRUNE_REC];
-    __shared__ int s_cand[PRUNE_MAX_HN];
-    __shared__ int s_b2[PRUNE_MAX_HN];
-    __shared__ int s_idx[NEXT_SUBS];
+    __shared__ __align__(16) int s_rec[2 * STAGE_RECS * PRUNE_REC];
+    __shared__ int s_idx[3 * NEXT_THREADS];
     __shared__ int s_warp[NEXT_THREADS / 32];
     __shared__ int s_last;
+    extern __shared__ __align__(16) unsigned char s_dyn[];
+    const int ncap = hn - PRUNE_M;
+    float2 *s_hyp = reinterpret_cast<float2 *>(s_dyn);
+    int *s_b2 = reinterpret_cast<int *>(s_hyp + ncap);
+    unsigned short *s_cand = reinterpret_cast<unsigned short *>(s_b2 + ncap);
     const int *key = q.key + bk * hn;
     const float2 *hyp = a.hyp + bk * hn;
     int *b2 = q.b2 + bk * hn;
     // L = the best exact count of pass 1 (0 when nothing was scored: then nothing is excluded)
-    auto pass1_best = [&]() {
+    int L = 0;
+    {
         const int *counts = a.counts + bk * hn;
         int best = 0;
         const int n1 = q.len[bk];
         for (int s = tid; s < n1; s += NEXT_THREADS) best = max(best, counts[q.list[bk * hn + s]]);
         best = __reduce_max_sync(0xffffffffu, best);
-        __syncthreads();                                  // s_warp is free
         if ((tid & 31) == 0) s_warp[tid >> 5] = best;
         __syncthreads();
-        int L = 0;
         for (int w = 0; w < NEXT_THREADS / 32; ++w) L = max(L, s_warp[w]);
-        return L;
-    };
-    // the slice's non-empty sub-cells, staged while L and the candidates are found; a slice without any (most of an
-    // image) has nothing to add
-    const int *sub = q.sub + bk * q.ncells * 4 * PRUNE_REC;
-    const int c = blockIdx.x * NEXT_SUBS + tid;
-    const bool fc = tid < NEXT_SUBS && c < 4 * q.ncells && cell_total(sub + (size_t)c * PRUNE_REC) > 0;
-    int m;
-    const int pc = cta_scan(fc, s_warp, &m);
-    if (fc) s_idx[pc] = c;
-    int L = -1;
-    if (m > 0) {
-        __syncthreads();
-        for (int i = tid; i < m * REC_V4; i += NEXT_THREADS) {
-            const int r = i / REC_V4, w = (i - r * REC_V4) * 4;
-            cp_async16(s_rec + r * PRUNE_REC + w, sub + (size_t)s_idx[r] * PRUNE_REC + w);
-        }
-        cp_async_commit();
-        L = pass1_best();
-        // the candidates that have a bound (the others stay in pass 2)
-        int nc = 0;
-        for (int h0 = 0; h0 < hn && L > 0; h0 += NEXT_THREADS) {
-            const int h = h0 + tid;
-            const bool f = h < hn && key[h] >= L && bounded(hyp[h]);
-            int n;
-            const int pos = nc + cta_scan(f, s_warp, &n);
-            if (f) { s_cand[pos] = h; s_b2[pos] = 0; }
-            nc += n;
-        }
-        cp_async_wait<0>();
-        __syncthreads();
-        if (nc > 0) {
-            // P threads per candidate, each over a contiguous part of the staged records
-            const int P = max(1, NEXT_THREADS / nc);
+    }
+    // the candidates that have a bound (the others stay in pass 2); pass 1's keys are -1 < L
+    int nc = 0;
+    for (int h0 = 0; h0 < hn && L > 0; h0 += NEXT_THREADS) {
+        const int h = h0 + tid;
+        const float2 hp = h < hn ? hyp[h] : make_float2(0.f, 0.f);
+        const bool f = h < hn && key[h] >= L && bounded(hp);
+        int n;
+        const int pos = nc + cta_scan(f, s_warp, &n);
+        if (f) { s_cand[pos] = (unsigned short)h; s_hyp[pos] = hp; s_b2[pos] = 0; }
+        nc += n;
+    }
+    if (nc > 0) {
+        __syncthreads();                                  // s_warp is free, the candidates are in place
+        // P threads per candidate, each over a contiguous part of every staged chunk
+        const int P = max(1, NEXT_THREADS / nc);
+        const int *sub = q.sub + (bk * q.ncells * 4 + x) * PRUNE_REC;
+        const int nsub = (4 * q.ncells - x + NEXT_CTAS - 1) / NEXT_CTAS;
+        stream_records<NEXT_THREADS>(sub, NEXT_CTAS * PRUNE_REC, nsub, s_rec, s_idx, s_warp, [&](const int *rec, int n) {
             for (int it = tid; it < nc * P; it += NEXT_THREADS) {
                 const int j = it % nc, p = it / nc;
-                const int r0 = p * m / P, r1 = (p + 1) * m / P;
+                const int r0 = p * n / P, r1 = (p + 1) * n / P;
                 if (r1 == r0) continue;
-                const float2 hp = hyp[s_cand[j]];
+                const float2 hp = s_hyp[j];
                 int bound = 0;
-                count_bound(q, s_rec + r0 * PRUNE_REC, r1 - r0, hp.x, hp.y, bound);
+                count_bound(q, rec + r0 * PRUNE_REC, r1 - r0, hp.x, hp.y, bound);
                 if (bound) atomicAdd(&s_b2[j], bound);
             }
-            __syncthreads();
-            for (int j = tid; j < nc; j += NEXT_THREADS)
-                if (s_b2[j]) atomicAdd(&b2[s_cand[j]], s_b2[j]);
-        }
+        });
+        for (int j = tid; j < nc; j += NEXT_THREADS)
+            if (s_b2[j]) atomicAdd(&b2[s_cand[j]], s_b2[j]);
     }
     // q.ticket[bk] is 0 here (the bound step leaves it so) and is left 0 for the refit
     __threadfence();
@@ -517,7 +530,6 @@ prune_next_kernel(VoteArgs a, PruneArgs q)
     __syncthreads();
     if (!s_last) return;
     __threadfence();
-    if (L < 0) L = pass1_best();
     int *list = q.list + (BK + bk) * hn;
     int base = 0;
     for (int h0 = 0; h0 < hn; h0 += NEXT_THREADS) {
@@ -559,7 +571,7 @@ cudaError_t launch_vote_pruned(const VoteArgs &a, const PruneArgs &q, cudaStream
     prune_bound_kernel<<<dim3((a.hn + BOUND_HYPS - 1) / BOUND_HYPS, a.K, a.B), BOUND_THREADS, 0, st>>>(a, q);
     cudaError_t e = launch_vote_list_slices(a, q.list, q.len, PRUNE_M, st);
     if (e != cudaSuccess) return e;
-    prune_next_kernel<<<dim3((4 * q.ncells + NEXT_SUBS - 1) / NEXT_SUBS, a.K, a.B), NEXT_THREADS, 0, st>>>(a, q);
+    prune_next_kernel<<<dim3(NEXT_CTAS, a.K, a.B), NEXT_THREADS, (a.hn - PRUNE_M) * NEXT_CAND_BYTES, st>>>(a, q);
     return launch_vote_list(a, q.list + BK * a.hn, q.len + BK, a.hn - PRUNE_M, st);
 }
 
