@@ -207,7 +207,9 @@ cudaError_t run_vote(const Plan &P, bool prune, cudaStream_t st)
 {
     PruneArgs q = P.prune;
     if (prune && prune_setup(P.v, q)) return launch_vote_pruned(P.v, q, st);
-    return launch_vote(P.v, false, st);
+    // the unpruned vote is launched plainly: chained after generate it measured slower where its grid is a single partial
+    // wave (H100, B = 1, K = 17, 720x540: 0.163 against 0.127 ms per call), and no faster at B = 1, K = 9 (DESIGN.md 4.3)
+    return launch_vote(P.v, false, false, st);
 }
 
 int run_select(const Plan &P, cudaStream_t st)
@@ -227,7 +229,7 @@ int run_front(const Plan &P, bool prune, cudaStream_t st, ProfCall *pc)
     if (rc) return rc;
     prof_end(pc, PVB_STAGE_SELECT, st);
     prof_start(pc, PVB_STAGE_GENERATE, st);
-    cudaError_t e = launch_generate(P.v, st);
+    cudaError_t e = launch_generate(P.v, true, st);     // chained after thin_gather, which exits as its trigger (common.cuh)
     if (e != cudaSuccess) return cuda_fail(e, "generate kernel");
     prof_end(pc, PVB_STAGE_GENERATE, st);
     prof_start(pc, PVB_STAGE_VOTE, st);
@@ -961,7 +963,7 @@ PVB_API int pvb_ransac_voting_v3_host(const pvb_desc *d, const void *mask_host, 
         if (e != cudaSuccess) return cuda_fail(e, "pipeline event");
         PeerPush none;
         memset(&none, 0, sizeof(none));
-        e = launch_generate(P.v, hp->cmp);
+        e = launch_generate(P.v, false, hp->cmp);     // its predecessor on cmp is the event wait, not thin_gather
         if (e == cudaSuccess) e = run_vote(P, true, hp->cmp);
         if (e == cudaSuccess) e = launch_refit(P.v, P.win, P.refit, reinterpret_cast<float *>(sb + S.out), none, hp->cmp);
         if (e != cudaSuccess) return cuda_fail(e, "compute kernels");
@@ -1102,7 +1104,7 @@ PVB_API int pvb_vote_count(const float *direct, const float *coords, const float
     v.B = 1; v.K = vn; v.hn = hn; v.cap = tn; v.W = 0; v.H = 0; v.thresh = inlier_thresh;
     v.tn = meta; v.state = meta + 1; v.xy = xy;
     v.dirs = dirs; v.idxs = nullptr; v.hyp = hyp_k; v.counts = counts_k;
-    e = launch_vote(v, true, st);
+    e = launch_vote(v, true, false, st);
     if (e != cudaSuccess) return cuda_fail(e, "vote kernel");
     e = launch_compat_unpack_counts(counts_k, counts, vn, hn, st);
     return e == cudaSuccess ? PVB_OK : cuda_fail(e, "unpack");

@@ -8,8 +8,45 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <utility>
 
 namespace pvb {
+
+// ---------------------------------------------------------------------------------
+// Programmatic dependent launch (PDL) of the v3 chain (DESIGN.md 4.3):
+//   thin_gather | generate -> [prune_hist -> prune_bound -> vote_kernel (pass 1) -> prune_next -> vote_list_kernel
+//   | vote_kernel] -> refit
+// thin_gather is launched plainly and never triggers early, so its exit is its trigger.  A chained kernel may start while
+// its immediate predecessor is still running.  The dependency rule every chained kernel keeps, so that this is no race:
+//   1. it executes grid_dep_wait() before it reads anything its immediate predecessor writes, before it writes anything
+//      that predecessor reads, and before it exits (every thread, on every path, early returns included);
+//   2. it executes grid_dep_launch_dependents() only after its own grid_dep_wait().
+// By induction, when a kernel starts, every kernel two or more launches back has completed and its writes are visible:
+// the predecessor has passed its wait (rule 2), which waited for the one before it (rule 1).  Only such data may be read
+// before the wait.  A kernel is launched chained only when its predecessor in the stream is a kernel of the chain that keeps
+// the rule; after a memset, an event or a foreign kernel it is launched plainly, and the wait returns at once.
+// ---------------------------------------------------------------------------------
+__device__ __forceinline__ void grid_dep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void grid_dep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
+// Launches kernel<<<grid, block, smem, st>>>(args...), allowed to overlap its predecessor in the stream (PDL) when
+// `chained`.  Returns the launch's error.
+template <typename... Params, typename... Args>
+cudaError_t launch_chained(bool chained, void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                           Args &&...args)
+{
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = chained ? 1 : 0;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+}
 
 // ---------------------------------------------------------------------------------
 // Philox4x32-10.  Counter layout of the built-in sampling mode (DESIGN.md "Sampling"):

@@ -44,10 +44,14 @@ struct VoteArgs {
     float2 *hyp;          // [B][K][hn]
     int *counts;          // [B][K][hn]
 };
+// The v3 chain's launches (select, generate, vote, refit) are programmatic dependent launches (common.cuh states the rule).
+// `chained`: the launch directly follows the chain kernel before it in the same stream (thin_gather for generate); pass
+// false after anything else (a memset, an event wait) or where chaining measured slower (DESIGN.md 4.3).
 // hypotheses for every (image, keypoint): explicit idxs or philox; also zeroes counts[b][k][h]
-cudaError_t launch_generate(const VoteArgs &a, cudaStream_t st);
+cudaError_t launch_generate(const VoteArgs &a, bool chained, cudaStream_t st);
 // counts[b][k][h] += #pixels voting for hyp[b][k][h]; launch_generate zeroes counts, other callers pass zero_counts = true
-cudaError_t launch_vote(const VoteArgs &a, bool zero_counts, cudaStream_t st);
+// (and chained = false: the memset precedes the kernel)
+cudaError_t launch_vote(const VoteArgs &a, bool zero_counts, bool chained, cudaStream_t st);
 
 // Pruned v3 vote (prune.cu, DESIGN.md 4.2): only hypotheses that can still be the first maximum are scored.  A bound
 // B(h) >= count(h) comes from per-cell direction histograms; pass 1 scores the PRUNE_M largest bounds, pass 2 every other

@@ -63,7 +63,8 @@ constexpr int HIST_SUBX = 2 * HIST_CELLS;      // their sub-cell columns; two su
 constexpr int HIST_SUBS = 2 * HIST_SUBX;       // 128 sub-cells x 64 words of two 16-bit bin counts: 32 KB
 static_assert(PRUNE_SUB * PRUNE_SUB < 65536, "a sub-cell's bin counts fit 16 bits");
 
-// One CTA per (band of PRUNE_CELL pixel rows, k, b).  The selected-pixel list is in raster (torch.nonzero) order, so the
+// One CTA per (band of PRUNE_CELL pixel rows, k, b), chained after generate but independent of it (it waits only at the end).
+// The selected-pixel list is in raster (torch.nonzero) order, so the
 // band's pixels are one contiguous segment of it.  The histogram and box are taken per sub-cell; every sub-cell and
 // every cell of the band gets a record, empty ones with total 0, and a cell's record is the union of its sub-cells'
 // (box: min / max of the same float bits; counts: sums), so it is what a histogram over the whole cell gives.
@@ -170,6 +171,10 @@ prune_hist_kernel(VoteArgs a, PruneArgs q)
         }
         __syncthreads();                                  // s_hist / s_box are reset for the next cells
     }
+    // the whole body reads only thin_gather's output and writes nothing generate reads, so it runs alongside generate;
+    // the wait keeps the chain's rule for the kernels after this one (common.cuh)
+    grid_dep_wait();
+    grid_dep_launch_dependents();
 }
 
 __device__ __forceinline__ int cell_total(const int *rec) { return (int)((unsigned)rec[PRUNE_REC - 1] >> 16); }
@@ -399,7 +404,9 @@ prune_bound_kernel(VoteArgs a, PruneArgs q)
     __shared__ int s_part[BOUND_SPLIT][BOUND_HYPS];
     __shared__ int s_w[2 * BOUND_WARPS];
     __shared__ int s_sel[2];
-    const float2 hp = (h < a.hn) ? a.hyp[bk * a.hn + h] : make_float2(0.f, 0.f);
+    const float2 hp = (h < a.hn) ? a.hyp[bk * a.hn + h] : make_float2(0.f, 0.f);   // generate's: before the wait
+    grid_dep_wait();                                      // the cell records are prune_hist's output
+    grid_dep_launch_dependents();
     int bound = 0;
     stream_records<BOUND_THREADS>(q.cells + bk * q.ncells * PRUNE_REC, PRUNE_REC, q.ncells, &s_rec[0][0], s_idx, s_w,
                                   [&](const int *rec, int n) {
@@ -477,13 +484,18 @@ prune_next_kernel(VoteArgs a, PruneArgs q)
     const int *key = q.key + bk * hn;
     const float2 *hyp = a.hyp + bk * hn;
     int *b2 = q.b2 + bk * hn;
-    // L = the best exact count of pass 1 (0 when nothing was scored: then nothing is excluded)
+    // L = the best exact count of pass 1 (0 when nothing was scored: then nothing is excluded).  Pass 1's list is the bound
+    // kernel's, two launches back, and is read before the wait; its counts are pass 1's, read after it
+    static_assert(PRUNE_M <= NEXT_THREADS, "one pass-1 entry per thread");
     int L = 0;
     {
         const int *counts = a.counts + bk * hn;
         int best = 0;
         const int n1 = q.len[bk];
-        for (int s = tid; s < n1; s += NEXT_THREADS) best = max(best, counts[q.list[bk * hn + s]]);
+        const int h1 = tid < n1 ? q.list[bk * hn + tid] : -1;
+        grid_dep_wait();
+        grid_dep_launch_dependents();
+        if (h1 >= 0) best = __ldcg(counts + h1);          // through L2: no L1 holds a line of the counts in a call
         best = __reduce_max_sync(0xffffffffu, best);
         if ((tid & 31) == 0) s_warp[tid >> 5] = best;
         __syncthreads();
@@ -567,11 +579,17 @@ cudaError_t launch_vote_pruned(const VoteArgs &a, const PruneArgs &q, cudaStream
 {
     const size_t BK = (size_t)a.B * a.K;
     const int nbands = (a.H + PRUNE_CELL - 1) / PRUNE_CELL;
-    prune_hist_kernel<<<dim3(nbands, a.K, a.B), HIST_THREADS, 0, st>>>(a, q);
-    prune_bound_kernel<<<dim3((a.hn + BOUND_HYPS - 1) / BOUND_HYPS, a.K, a.B), BOUND_THREADS, 0, st>>>(a, q);
-    cudaError_t e = launch_vote_list_slices(a, q.list, q.len, PRUNE_M, st);
+    // every launch is chained (common.cuh); prune_setup guarantees both passes launch (PRUNE_M > 0, hn > PRUNE_M), so
+    // each kernel's predecessor is the one before it in this list
+    cudaError_t e = launch_chained(true, prune_hist_kernel, dim3(nbands, a.K, a.B), HIST_THREADS, 0, st, a, q);
+    if (e == cudaSuccess)
+        e = launch_chained(true, prune_bound_kernel, dim3((a.hn + BOUND_HYPS - 1) / BOUND_HYPS, a.K, a.B), BOUND_THREADS, 0, st,
+                           a, q);
+    if (e == cudaSuccess) e = launch_vote_list_slices(a, q.list, q.len, PRUNE_M, st);
+    if (e == cudaSuccess)
+        e = launch_chained(true, prune_next_kernel, dim3(NEXT_CTAS, a.K, a.B), NEXT_THREADS,
+                           (size_t)(a.hn - PRUNE_M) * NEXT_CAND_BYTES, st, a, q);
     if (e != cudaSuccess) return e;
-    prune_next_kernel<<<dim3(NEXT_CTAS, a.K, a.B), NEXT_THREADS, (a.hn - PRUNE_M) * NEXT_CAND_BYTES, st>>>(a, q);
     return launch_vote_list(a, q.list + BK * a.hn, q.len + BK, a.hn - PRUNE_M, st);
 }
 

@@ -36,6 +36,10 @@ namespace pvb {
 __global__ void __launch_bounds__(256)
 generate_kernel(VoteArgs a)
 {
+    // tn, dirs and xy are thin_gather's output.  The trigger comes at once, so prune_hist, which needs none of what this
+    // kernel writes, runs alongside it (common.cuh, DESIGN.md 4)
+    grid_dep_wait();
+    grid_dep_launch_dependents();
     const int h = blockIdx.x * 256 + threadIdx.x;
     if (h >= a.hn) return;
     const int k = blockIdx.y, b = blockIdx.z;
@@ -64,11 +68,10 @@ generate_kernel(VoteArgs a)
     a.counts[((size_t)b * a.K + k) * a.hn + h] = 0;      // the vote kernel accumulates with atomics: saves a memset launch
 }
 
-cudaError_t launch_generate(const VoteArgs &a, cudaStream_t st)
+cudaError_t launch_generate(const VoteArgs &a, bool chained, cudaStream_t st)
 {
     dim3 g((a.hn + 255) / 256, a.K, a.B);
-    generate_kernel<<<g, 256, 0, st>>>(a);
-    return cudaGetLastError();
+    return launch_chained(chained, generate_kernel, g, 256, 0, st, a);
 }
 
 // ---------------------------------------------------------------------------------
@@ -187,11 +190,10 @@ vote_kernel(const VoteK p)
     const VoteArgs &a = p.a;
     const int b = blockIdx.z;
     const int k = blockIdx.y % a.K, slice = blockIdx.y / a.K;
-    const int tn = min(a.tn[b], a.cap);
+    const int tn = min(a.tn[b], a.cap);                 // thin_gather's: two or more launches back (common.cuh)
     const int t0 = blockIdx.x * VOTE_TILE;
     const size_t bk = (size_t)b * a.K + k;
-    const int nh = p.list ? __ldg(p.len + bk) : a.hn;      // hypothesis slots of this (image, keypoint)
-    if (t0 >= tn || slice * (TEAM * HPT) >= nh) return;
+    if (t0 >= tn) { grid_dep_wait(); return; }
     const int *lst = p.list ? p.list + bk * a.hn : nullptr;
     const int n = min(VOTE_TILE, tn - t0);
     const int npad = (n + VOTE_BLOCK - 1) / VOTE_BLOCK * VOTE_BLOCK;
@@ -203,7 +205,8 @@ vote_kernel(const VoteK p)
     const int team = tid / TEAM;
     const int hbase = slice * (TEAM * HPT) + (tid - team * TEAM);
 
-    // ---- stage 1: load this tile's pixels -> tile-local origin for the fast path
+    // ---- stage 1: load this tile's pixels -> tile-local origin for the fast path.  Stages 1 and 2 read only thin_gather's
+    // output, so in pass 1 they run while the bound kernel finishes
     float2 v[PPT], c[PPT];
     float ox, oy, cmax;
     load_tile<NT, PPT>(dk, xy, n, v, c, s_box, ox, oy, cmax);
@@ -220,13 +223,19 @@ vote_kernel(const VoteK p)
         }
     }
 
+    // the hypotheses and the list are the predecessors' output, and the counts are zeroed by generate
+    grid_dep_wait();
+    grid_dep_launch_dependents();
+    const int nh = p.list ? __ldcg(p.len + bk) : a.hn;     // hypothesis slots of this (image, keypoint)
+    if (slice * (TEAM * HPT) >= nh) return;
+
     // ---- hypotheses of this thread, relative to the tile origin
     float hxc[HPT], hyc[HPT], dl[HPT];
     int neg[HPT];   // tests whose margin is negative (sign bit) = non-inliers, padding included
 #pragma unroll
     for (int j = 0; j < HPT; ++j) {
         const int s = hbase + j * TEAM;
-        const float2 q = (s < nh) ? hyp[lst ? __ldg(lst + s) : s] : make_float2(0.f, 0.f);
+        const float2 q = (s < nh) ? hyp[lst ? __ldcg(lst + s) : s] : make_float2(0.f, 0.f);
         const float3 f = hyp_frame(q, ox, oy, cmax, p.cone);
         hxc[j] = f.x; hyc[j] = f.y; dl[j] = f.z;
         neg[j] = 0;
@@ -278,7 +287,7 @@ vote_kernel(const VoteK p)
                     const float hx_ = __shfl_sync(0xffffffffu, hxc[j], L), hy_ = __shfl_sync(0xffffffffu, hyc[j], L);
                     const float dl_ = __shfl_sync(0xffffffffu, dl[j], L);
                     const int s = hbase - lane + L + j * TEAM;
-                    const float2 q = (s < nh) ? __ldg(hyp + (lst ? __ldg(lst + s) : s)) : make_float2(0.f, 0.f);
+                    const float2 q = (s < nh) ? __ldg(hyp + (lst ? __ldcg(lst + s) : s)) : make_float2(0.f, 0.f);
                     int delta = 0;
                     if (lane < nb) {
                         const float m = cone_margin(ra, rb, hx_, hy_);
@@ -298,7 +307,7 @@ vote_kernel(const VoteK p)
     for (int j = 0; j < HPT; ++j) {
         const int s = hbase + j * TEAM;
         const int cnt = mine - neg[j];
-        if (s < nh && cnt) atomicAdd(counts + (lst ? __ldg(lst + s) : s), cnt);
+        if (s < nh && cnt) atomicAdd(counts + (lst ? __ldcg(lst + s) : s), cnt);
     }
 }
 
@@ -338,7 +347,7 @@ static std::atomic<int> g_vote_variant{0};
 
 void set_vote_tuning(int variant) { g_vote_variant.store(variant, std::memory_order_relaxed); }
 
-cudaError_t launch_vote(const VoteArgs &a, bool zero_counts, cudaStream_t st)
+cudaError_t launch_vote(const VoteArgs &a, bool zero_counts, bool chained, cudaStream_t st)
 {
     if (zero_counts) {     // callers that did not run generate_kernel (which zeroes the counts it creates hypotheses for)
         cudaError_t e = cudaMemsetAsync(a.counts, 0, sizeof(int) * (size_t)a.B * a.K * a.hn, st);
@@ -350,11 +359,12 @@ cudaError_t launch_vote(const VoteArgs &a, bool zero_counts, cudaStream_t st)
     p.list = nullptr;
     p.len = nullptr;
     const int variant = g_vote_variant.load(std::memory_order_relaxed);
+    cudaError_t e = cudaSuccess;
 #define PVB_VOTE(HPT, NT, MINB, TILE, WS)                                               \
     do {                                                                                \
         const int slices = (a.hn + (HPT) * (WS) * 32 - 1) / ((HPT) * (WS) * 32);        \
         dim3 g((a.cap + (TILE) - 1) / (TILE), a.K * slices, a.B);                       \
-        vote_kernel<HPT, NT, MINB, TILE, WS><<<g, NT, 0, st>>>(p);                      \
+        e = launch_chained(chained, vote_kernel<HPT, NT, MINB, TILE, WS>, g, NT, 0, st, p); \
     } while (0)
     if (a.hn <= 32) PVB_VOTE(1, 128, 8, 512, 1);
     else if (a.hn <= 64) PVB_VOTE(2, 128, 8, 512, 1);
@@ -364,7 +374,7 @@ cudaError_t launch_vote(const VoteArgs &a, bool zero_counts, cudaStream_t st)
     else if (variant == 3) PVB_VOTE(4, 128, 8, 512, 4);
     else PVB_VOTE(4, 128, 8, 1024, 4);    // H100 (400 W), cfg-2: 0.72 ms per launch vs 0.75 ms with 512-pixel tiles
 #undef PVB_VOTE
-    return cudaGetLastError();
+    return e;
 }
 
 // The pruned v3 vote's list kernel: vote_kernel turned inside out.  A CTA owns one (image, keypoint, 1024-pixel tile) and
@@ -412,10 +422,14 @@ vote_list_kernel(const VoteArgs a, const ConeParams cone, const int *__restrict_
     __shared__ float s_box[4][NW];
     const int b = blockIdx.z;
     const int k = blockIdx.y;
+    // The list is prune_next's output, and a CTA whose list is empty exits before it builds its records: building them
+    // before the wait cost more in the CTAs of empty lists than it hid (DESIGN.md 4.3), so the wait comes first
+    grid_dep_wait();
+    grid_dep_launch_dependents();
     const int tn = min(a.tn[b], a.cap);
     const int t0 = blockIdx.x * LIST_TILE;
     const size_t bk = (size_t)b * a.K + k;
-    const int nh = __ldg(len + bk);
+    const int nh = __ldcg(len + bk);
     if (t0 >= tn || nh <= 0) return;
     const int n = min(LIST_TILE, tn - t0);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -426,7 +440,7 @@ vote_list_kernel(const VoteArgs a, const ConeParams cone, const int *__restrict_
 
     int h = 0;                                          // this thread's first list entry, loaded while the pixels are
     float2 hq = make_float2(0.f, 0.f);
-    if (tid < nh) { h = __ldg(lst + tid); hq = hyp[h]; }
+    if (tid < nh) { h = __ldcg(lst + tid); hq = hyp[h]; }
     float4 ra[LIST_PPT];
     float2 rb[LIST_PPT];
     float ox, oy, cmax;
@@ -442,7 +456,7 @@ vote_list_kernel(const VoteArgs a, const ConeParams cone, const int *__restrict_
     unsigned *tally = s_tally[warp];
     for (int c0 = 0; c0 < nh; c0 += LIST_CHUNK) {
         const int ns = min(LIST_CHUNK, nh - c0);
-        if (c0 > 0 && tid < ns) { h = __ldg(lst + c0 + tid); hq = hyp[h]; }
+        if (c0 > 0 && tid < ns) { h = __ldcg(lst + c0 + tid); hq = hyp[h]; }
         if (tid < ns) {
             const float3 f = hyp_frame(hq, ox, oy, cmax, cone);
             s_h[tid] = make_float4(f.x, f.y, f.z, __int_as_float(h));
@@ -495,8 +509,7 @@ cudaError_t launch_vote_list(const VoteArgs &a, const int *list, const int *len,
 {
     if (max_len <= 0) return cudaSuccess;
     dim3 g((a.cap + LIST_TILE - 1) / LIST_TILE, a.K, a.B);
-    vote_list_kernel<<<g, LIST_NT, 0, st>>>(a, make_cone(a.thresh), list, len);
-    return cudaGetLastError();
+    return launch_chained(true, vote_list_kernel, g, LIST_NT, 0, st, a, make_cone(a.thresh), list, len);
 }
 
 // Pass 1: vote_kernel over a full list, in (HPT*32)-hypothesis slices (WS = 1) whose four warps split the 1024-pixel tile.
@@ -513,8 +526,7 @@ cudaError_t launch_vote_list_slices(const VoteArgs &a, const int *list, const in
     p.len = len;
     const int slices = (max_len + HPT * 32 - 1) / (HPT * 32);
     dim3 g((a.cap + TILE - 1) / TILE, a.K * slices, a.B);
-    vote_kernel<HPT, NT, 8, TILE, 1><<<g, NT, 0, st>>>(p);
-    return cudaGetLastError();
+    return launch_chained(true, vote_kernel<HPT, NT, 8, TILE, 1>, g, NT, 0, st, p);
 }
 
 // Multi-GPU exchange tail shared by the refit and the covariance kernel: one thread stores NV floats of unit `bk` into every
@@ -560,6 +572,8 @@ __device__ __forceinline__ bool vote_winner(float vx, float vy, float cx, float 
 __global__ void __launch_bounds__(RF_THREADS)
 refit_kernel(VoteArgs a, float2 *__restrict__ win, RefitScratch rs, float *__restrict__ out, ConeParams cone, PeerPush pp)
 {
+    // the counts are the last vote pass's output.  The last kernel of the chain: no dependent to trigger (common.cuh)
+    grid_dep_wait();
     const int split = blockIdx.x, k = blockIdx.y, b = blockIdx.z;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     constexpr int NW = RF_THREADS / 32;
@@ -661,8 +675,7 @@ cudaError_t launch_refit(const VoteArgs &a, float2 *win, const RefitScratch &rs,
                          cudaStream_t st)
 {
     dim3 g(rs.splits, a.K, a.B);
-    refit_kernel<<<g, RF_THREADS, 0, st>>>(a, win, rs, out_kpt, make_cone(a.thresh), pp);
-    return cudaGetLastError();
+    return launch_chained(true, refit_kernel, g, RF_THREADS, 0, st, a, win, rs, out_kpt, make_cone(a.thresh), pp);
 }
 
 // ---------------------------------------------------------------------------------
