@@ -1,4 +1,6 @@
 // api.cu -- the C ABI declared in include/pvnet_vote_b200.h.
+#include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -160,7 +162,7 @@ int make_plan(const pvb_desc *d, const void *mask, const float *vertex, const in
     for (int i = 0; i < 5; ++i) s.vs[i] = d->vertex_stride[i];
     s.selection = selection;
     s.B = d->B; s.H = d->H; s.W = d->W; s.K = d->K; s.nwords = L.nwords; s.nblocks = L.nblocks; s.cap = L.capacity;
-    s.min_num = d->min_num; s.max_num = d->max_num; s.img_base = d->img_base;
+    s.min_num = d->min_num; s.max_num = d->max_num; s.img_base = d->img_base; s.b0 = 0;
     s.seed = d->seed; s.tag_sel = d->rng_tag_sel ? (uint32_t)d->rng_tag_sel : tag_sel;
     s.rowwise_gather = 0;
     s.seg_classes = 0; s.seg_cs = 0; s.mask_out = nullptr;
@@ -192,6 +194,8 @@ int make_plan(const pvb_desc *d, const void *mask, const float *vertex, const in
     P->prune.list = reinterpret_cast<int *>(w + L.prune_list);
     P->prune.len = reinterpret_cast<int *>(w + L.prune_len);
     const size_t BK = (size_t)d->B * d->K;
+    P->prune.list2 = P->prune.list + BK * d->hn;
+    P->prune.len2 = P->prune.len + BK;
     const size_t prune_sub = align_up(L.prune_len + 2 * BK * sizeof(int));
     P->prune.sub = reinterpret_cast<int *>(w + prune_sub);
     P->prune.b2 = reinterpret_cast<int *>(w + align_up(prune_sub + BK * L.prune_ncells * 4 * PRUNE_REC * sizeof(int)));
@@ -280,6 +284,152 @@ size_t mask_elt_bytes(int dt)
     }
 }
 
+// ---- grouped launch of the pruned v3 call (DESIGN.md 4.4) ----------------------------------------------------------
+// Every stage from select to refit works on each image alone, so a call's batch runs as groups of consecutive images, each
+// group's whole chain on one of a few internal streams: one group's latency-bound kernels (hist, bound, next, pass 2,
+// refit, select) then run while another group's pass 1 keeps the FP32 pipes busy.
+constexpr int GROUPS_DEFAULT = 2;          // groups per call at most (cfg-2: 2 x 8 images); DESIGN.md 4.4 has the sweep
+constexpr int GROUP_STREAMS_DEFAULT = 2;   // internal streams the groups go to, round-robin
+constexpr int GROUP_MAX_STREAMS = 4;
+constexpr int MAX_DEVICES = 64;
+std::atomic<int> g_group_limit{0};         // pvb_set_group_tuning: 0 = GROUPS_DEFAULT
+std::atomic<int> g_group_streams{0};       // 0 = GROUP_STREAMS_DEFAULT
+
+// Groups of a call: the most, up to the limit, whose smallest group (floor(B / G) images) still passes the prune gate.
+// One group (today's single chain) when the call does not prune.
+int group_count(const Plan &P, bool prune)
+{
+    PruneArgs q = P.prune;
+    if (!prune || !prune_setup(P.v, q)) return 1;
+    const int lim = g_group_limit.load(std::memory_order_relaxed);
+    int G = std::min(lim > 0 ? lim : GROUPS_DEFAULT, P.v.B);
+    for (; G > 1; --G) {
+        VoteArgs v = P.v;
+        v.B = P.v.B / G;
+        if (prune_setup(v, q)) break;
+    }
+    return G;
+}
+
+// The plan of images [b0, b0 + nb) of a call: the call's own workspace layout and arguments, with every per-image pointer
+// advanced by b0 images (all of them are image-major), so a group's kernels read and write exactly the bytes the ungrouped
+// call's blocks b0 .. b0 + nb - 1 do.  Philox stays keyed by the global image index (img_base + b0 + b); the status word is
+// the call's, and reports image b0 + b.
+Plan group_view(const Plan &P, int b0, int nb)
+{
+    Plan G = P;
+    const size_t b = (size_t)b0, K = (size_t)P.v.K, hn = (size_t)P.v.hn, cap = (size_t)P.L.capacity;
+    const size_t HW = (size_t)P.s.H * P.s.W;
+    SelectArgs &s = G.s;
+    const size_t melt = s.seg_classes > 0 ? sizeof(float) : mask_elt_bytes(s.mask_dtype);
+    s.mask = static_cast<const char *>(P.s.mask) + (long long)b0 * P.s.msb * (long long)melt;
+    s.vertex = P.s.vertex + (long long)b0 * P.s.vs[0];
+    if (s.selection) s.selection += b * HW;
+    if (s.mask_out) s.mask_out += b * HW;
+    s.B = nb; s.img_base += b0; s.b0 = b0;
+    s.bits += b * P.L.nwords; s.blocktot += b * P.L.nblocks;
+    s.ticket += b; s.fgsum += b; s.nz += b; s.tn += b; s.state += b;
+    s.xy += b * cap; s.dirs += b * K * cap;
+    VoteArgs &v = G.v;
+    v.B = nb; v.img_base += b0;
+    v.tn = s.tn; v.state = s.state; v.xy = s.xy; v.dirs = s.dirs;
+    if (v.idxs) v.idxs += b * hn * K * 2;
+    v.hyp += b * K * hn; v.counts += b * K * hn;
+    G.win += b * K;
+    G.refit.partial += b * K * P.refit.splits * 5; G.refit.ticket += b * K;
+    PruneArgs &q = G.prune;
+    const size_t nc = (size_t)P.prune.ncells;
+    q.cells += b * K * nc * PRUNE_REC; q.sub += b * K * nc * 4 * PRUNE_REC;
+    q.key += b * K * hn; q.b2 += b * K * hn; q.list += b * K * hn; q.list2 += b * K * hn;
+    q.len += b * K; q.len2 += b * K;
+    q.ticket = G.refit.ticket;
+    return G;
+}
+
+// internal streams and events of the grouped launch: one set per (host thread, device, caller stream), for up to
+// GROUP_SETS caller streams (beyond that, sets are reused round-robin: that only orders calls), created on first use and
+// kept.  Thread-local, so two host threads never interleave their chains on one stream (the PDL rule of common.cuh); one
+// set per caller stream, so calls a caller overlaps on several streams do not queue behind each other's groups.
+constexpr int GROUP_SETS = 8;
+struct GroupPipe {
+    cudaStream_t caller = nullptr;
+    cudaStream_t st[GROUP_MAX_STREAMS] = {};
+    cudaEvent_t fork = nullptr, join[GROUP_MAX_STREAMS] = {};
+    bool ready = false;
+};
+
+int group_pipe(cudaStream_t caller, GroupPipe **out)
+{
+    static thread_local GroupPipe pipes[MAX_DEVICES][GROUP_SETS];
+    static thread_local unsigned next[MAX_DEVICES];
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaGetDevice");
+    if (dev < 0 || dev >= MAX_DEVICES) return fail(PVB_ERR_CUDA, "device index %d out of range", dev);
+    GroupPipe *hit = nullptr;
+    for (GroupPipe &q : pipes[dev])
+        if (q.ready && q.caller == caller) { hit = &q; break; }
+    if (!hit) {
+        hit = &pipes[dev][next[dev]++ % GROUP_SETS];
+        hit->caller = caller;
+    }
+    GroupPipe &p = *hit;
+    if (!p.ready) {
+        e = cudaEventCreateWithFlags(&p.fork, cudaEventDisableTiming);
+        for (int i = 0; i < GROUP_MAX_STREAMS && e == cudaSuccess; ++i) {
+            e = cudaStreamCreateWithFlags(&p.st[i], cudaStreamNonBlocking);
+            if (e == cudaSuccess) e = cudaEventCreateWithFlags(&p.join[i], cudaEventDisableTiming);
+        }
+        if (e != cudaSuccess) return cuda_fail(e, "group streams");
+        p.ready = true;
+    }
+    *out = &p;
+    return PVB_OK;
+}
+
+// The v3 chain of a call in G groups: the header memset on the caller's stream, a fork event, each group's whole chain
+// (mask_bits .. refit) on internal stream g % S, then the caller's stream waits for every internal stream.  The first
+// kernel of a group (mask_bits) is launched plainly, so a chain is never chained onto another stream's or group's kernel.
+int run_groups(const Plan &P, int G, float *out_kpt, const PeerPush &pp, cudaStream_t st, ProfCall *pc)
+{
+    GroupPipe *gp = nullptr;
+    int rc = group_pipe(st, &gp);
+    if (rc) return rc;
+    const int sl = g_group_streams.load(std::memory_order_relaxed);
+    const int S = std::min(G, sl > 0 ? sl : GROUP_STREAMS_DEFAULT);
+    // the stage events stay on the caller's stream (an event between two kernels drains the pipeline): `select` brackets
+    // the memset, `vote` the groups from fork to join; `generate` and `finish` read 0
+    prof_start(pc, PVB_STAGE_SELECT, st);
+    cudaError_t e = cudaMemsetAsync(P.s.status, 0, P.L.bits, st);
+    if (e != cudaSuccess) return cuda_fail(e, "memset(header)");
+    prof_end(pc, PVB_STAGE_SELECT, st);
+    prof_end(pc, PVB_STAGE_GENERATE, st);
+    e = cudaEventRecord(gp->fork, st);
+    for (int i = 0; i < S && e == cudaSuccess; ++i) e = cudaStreamWaitEvent(gp->st[i], gp->fork, 0);
+    if (e != cudaSuccess) return cuda_fail(e, "group fork");
+    const int B = P.v.B, K = P.v.K;
+    for (int g = 0; g < G; ++g) {
+        const int b0 = (int)((long long)g * B / G), b1 = (int)((long long)(g + 1) * B / G);
+        const Plan Q = group_view(P, b0, b1 - b0);
+        PeerPush qp = pp;
+        for (int r = 0; r < qp.world; ++r) qp.recv[r] += (size_t)b0 * K * 2;
+        cudaStream_t gs = gp->st[g % S];
+        e = launch_select(Q.s, gs);
+        if (e == cudaSuccess) e = launch_generate(Q.v, true, gs);      // chained after thin_gather, as in run_front
+        if (e == cudaSuccess) e = run_vote(Q, true, gs);
+        if (e == cudaSuccess) e = launch_refit(Q.v, Q.win, Q.refit, out_kpt + (size_t)b0 * K * 2, qp, gs);
+        if (e != cudaSuccess) return cuda_fail(e, "group kernels");
+    }
+    for (int i = 0; i < S && e == cudaSuccess; ++i) {
+        e = cudaEventRecord(gp->join[i], gp->st[i]);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(st, gp->join[i], 0);
+    }
+    if (e != cudaSuccess) return cuda_fail(e, "group join");
+    prof_end(pc, PVB_STAGE_VOTE, st);
+    prof_end(pc, PVB_STAGE_FINISH, st);
+    return PVB_OK;
+}
+
 } // namespace
 
 extern "C" {
@@ -321,6 +471,8 @@ static int run_v3(const pvb_desc *d, const void *mask, const float *vertex, cons
         P.s.mask_out = reinterpret_cast<long long *>(mask_out);
     }
     ProfCall *pc = prof_begin(true);
+    const int G = group_count(P, prune);
+    if (G > 1) return run_groups(P, G, out_kpt, pp, st, pc);
     rc = run_front(P, prune, st, pc);
     if (rc) return rc;
     prof_start(pc, PVB_STAGE_FINISH, st);
@@ -837,7 +989,6 @@ struct HostPipe {
     cudaEvent_t user = nullptr, end = nullptr, dma[HOST_SLOTS] = {}, sel[HOST_SLOTS] = {}, done[HOST_SLOTS] = {};
     bool ready = false;
 };
-constexpr int MAX_DEVICES = 64;
 
 int host_pipe(int dev, HostPipe **out)
 {
@@ -986,6 +1137,15 @@ PVB_API int pvb_set_tuning(int32_t gather_mode, int32_t vote_variant)
     if (gather_mode < 0 || gather_mode > 2) return fail(PVB_ERR_INVALID, "gather_mode must be 0..2");
     set_gather_tuning(gather_mode);
     set_vote_tuning(vote_variant);
+    return PVB_OK;
+}
+
+PVB_API int pvb_set_group_tuning(int32_t max_groups, int32_t streams)
+{
+    if (max_groups < 0 || max_groups > 65535) return fail(PVB_ERR_INVALID, "max_groups must be 0..65535");
+    if (streams < 0 || streams > GROUP_MAX_STREAMS) return fail(PVB_ERR_INVALID, "streams must be 0..%d", GROUP_MAX_STREAMS);
+    g_group_limit.store(max_groups, std::memory_order_relaxed);
+    g_group_streams.store(streams, std::memory_order_relaxed);
     return PVB_OK;
 }
 

@@ -15,6 +15,7 @@ struct SelectArgs {
     long long vs[5];              // vertex strides (elements)
     const float *selection;       // optional [B,H,W]
     int B, H, W, K, nwords, nblocks, cap, min_num, max_num, img_base;
+    int b0;                       // index of image 0 in the call (a group's args, api.cu): status[1] reports b0 + b
     int rowwise_gather;           // 1: vertex is read in place from pinned host memory: always whole pixel rows per warp
     int seg_classes;              // > 0: `mask` points to fp32 logits [B,C,H,W]; the mask is argmax over C
     long long seg_cs;             // class stride of the logits (elements)
@@ -74,6 +75,7 @@ struct PruneArgs {
                          // prune_next_kernel
     int *list;           // [2][B][K][hn]
     int *len;            // [2][B][K]
+    int *list2, *len2;   // pass 2's half of each: list + B*K*hn, len + B*K (of the whole call when a group's args)
     int *ticket;         // [B][K] arrival counter of the bound CTAs: 0 at the start of the call, and left 0
     int ncx, ncells;     // ceil(W / PRUNE_CELL), ceil(H / PRUNE_CELL) * ncx
     float cos_w, sin_w;  // rotation by the widened cone half-angle theta'

@@ -470,7 +470,6 @@ prune_next_kernel(VoteArgs a, PruneArgs q)
 {
     const int x = blockIdx.x, k = blockIdx.y, b = blockIdx.z, tid = threadIdx.x;
     const size_t bk = (size_t)b * a.K + k;
-    const size_t BK = (size_t)a.B * a.K;
     const int hn = a.hn;
     __shared__ __align__(16) int s_rec[2 * STAGE_RECS * PRUNE_REC];
     __shared__ int s_idx[3 * NEXT_THREADS];
@@ -542,7 +541,7 @@ prune_next_kernel(VoteArgs a, PruneArgs q)
     __syncthreads();
     if (!s_last) return;
     __threadfence();
-    int *list = q.list + (BK + bk) * hn;
+    int *list = q.list2 + bk * hn;
     int base = 0;
     for (int h0 = 0; h0 < hn; h0 += NEXT_THREADS) {
         const int h = h0 + tid;
@@ -552,7 +551,7 @@ prune_next_kernel(VoteArgs a, PruneArgs q)
         if (f) list[pos] = h;
         base += n;
     }
-    if (tid == 0) q.len[BK + bk] = base;
+    if (tid == 0) q.len2[bk] = base;
 }
 
 bool prune_setup(const VoteArgs &a, PruneArgs &q)
@@ -577,7 +576,6 @@ bool prune_setup(const VoteArgs &a, PruneArgs &q)
 
 cudaError_t launch_vote_pruned(const VoteArgs &a, const PruneArgs &q, cudaStream_t st)
 {
-    const size_t BK = (size_t)a.B * a.K;
     const int nbands = (a.H + PRUNE_CELL - 1) / PRUNE_CELL;
     // every launch is chained (common.cuh); prune_setup guarantees both passes launch (PRUNE_M > 0, hn > PRUNE_M), so
     // each kernel's predecessor is the one before it in this list
@@ -590,7 +588,7 @@ cudaError_t launch_vote_pruned(const VoteArgs &a, const PruneArgs &q, cudaStream
         e = launch_chained(true, prune_next_kernel, dim3(NEXT_CTAS, a.K, a.B), NEXT_THREADS,
                            (size_t)(a.hn - PRUNE_M) * NEXT_CAND_BYTES, st, a, q);
     if (e != cudaSuccess) return e;
-    return launch_vote_list(a, q.list + BK * a.hn, q.len + BK, a.hn - PRUNE_M, st);
+    return launch_vote_list(a, q.list2, q.len2, a.hn - PRUNE_M, st);
 }
 
 } // namespace pvb

@@ -232,7 +232,7 @@ thin_gather_kernel(uint32_t *__restrict__ bits, unsigned *__restrict__ blocktot,
                    int *__restrict__ status, const float *__restrict__ selection, const float *__restrict__ vertex,
                    long long sB, long long sH, long long sW, long long sK, long long sC,
                    float2 *__restrict__ xy, float2 *__restrict__ dirs, int nwords, int nblocks, int K, int cap, int W, int HW,
-                   int min_num, int max_num, uint2 key, uint32_t tag, int img_base, int rowwise)
+                   int min_num, int max_num, uint2 key, uint32_t tag, int img_base, int b0, int rowwise)
 {
     __shared__ unsigned short s_list[TS_THREADS * 32];   // pixel index inside the block (12 bits)
     __shared__ int s_base, s_blk;
@@ -331,7 +331,7 @@ thin_gather_kernel(uint32_t *__restrict__ bits, unsigned *__restrict__ blocktot,
     if (tid == 0 && base + total > cap) {
         // more pixels selected than the workspace holds: report; the walks below stop at cap and every consumer clamps tn
         atomicCAS(status, 0, PVB_ERR_CAPACITY);
-        status[1] = b;
+        status[1] = b0 + b;
     }
     const bool vec = (sC == 1 && (sK & 1) == 0 && (sW & 1) == 0 && (sH & 1) == 0 && (sB & 1) == 0 &&
                       (reinterpret_cast<uintptr_t>(vertex) & 7u) == 0);
@@ -444,7 +444,7 @@ cudaError_t launch_select(const SelectArgs &a, cudaStream_t st)
                                                   a.vertex, a.vs[0], a.vs[1], a.vs[2], a.vs[3], a.vs[4], a.xy, a.dirs, nwords,
                                                   a.nblocks, a.K, a.cap, a.W, a.H * a.W, a.min_num, a.max_num,
                                                   make_uint2((uint32_t)a.seed, (uint32_t)(a.seed >> 32)), a.tag_sel, a.img_base,
-                                                  (a.rowwise_gather || gmode == 2) ? 1 : 0);
+                                                  a.b0, (a.rowwise_gather || gmode == 2) ? 1 : 0);
     return cudaGetLastError();
 }
 

@@ -505,6 +505,12 @@ PVB_API int pvb_profile_enable(int32_t every);
  *   vote_variant pixel tile of the vote kernel above 256 hypotheses per keypoint: 0 = 1 = 1024 pixels (default),
  *                2 = 256, 3 = 512; up to 256 hypotheses the tile is always 512 */
 PVB_API int pvb_set_tuning(int32_t gather_mode, int32_t vote_variant);
+/* Grouped launch of the pruned v3 entries (pvb_ransac_voting_v3, _push, pvb_decode_v3; DESIGN.md 4.4): a call whose every
+ * group still prunes runs as up to max_groups groups of consecutive images on `streams` internal streams of the calling
+ * host thread, joined back into the caller's stream before the entry returns.  0 = the default (2 groups, 2 streams);
+ * max_groups = 1 runs every call as one chain on the caller's stream.  Same tooling kind as pvb_set_tuning: process-wide,
+ * atomic, and results do not depend on it. */
+PVB_API int pvb_set_group_tuning(int32_t max_groups, int32_t streams);
 PVB_API int pvb_profile_reset(void);
 PVB_API int pvb_profile_read(double *ms, int32_t n);
 
