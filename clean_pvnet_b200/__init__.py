@@ -17,6 +17,8 @@ Public surface (same names/signatures as the reference):
     install_vote_loss_as_reference
     render.render_depth_batch (the depth image the T-LESS evaluator's OpenGL DepthRender renders, n poses per launch),
     vsd_batch (T-LESS's VSD error for n pose pairs), install_depth_renderer_as_reference
+    crop.crop_inputs (T-LESS's PVNet crop, pvnet_transform, for n boxes), uncrop_keypoints (the evaluator's un-crop),
+    warp_affine_batch (cv2.warpAffine INTER_LINEAR for n rows), install_crop_as_reference (the cascade's crop)
 """
 from . import _lib  # noqa: F401
 from . import nn  # noqa: F401
@@ -34,6 +36,8 @@ from . import pose  # noqa: F401
 from .pose import pnp_batch  # noqa: F401
 from . import render  # noqa: F401
 from .render import render_depth_batch, vsd_batch, install_depth_renderer_as_reference  # noqa: F401
+from . import crop  # noqa: F401
+from .crop import crop_inputs, uncrop_keypoints, warp_affine_batch, install_crop_as_reference  # noqa: F401
 from .vote_loss import vote_loss, vote_target_batch, NetworkWrapper, install_vote_loss_as_reference  # noqa: F401
 from .ransac_voting_gpu import (  # noqa: F401
     estimate_voting_distribution_with_mean,
@@ -52,4 +56,5 @@ __all__ = [
     "metrics", "pose_metrics_batch", "mask_iou_batch", "linemod_scores",
     "vote_loss", "vote_target_batch", "NetworkWrapper", "install_vote_loss_as_reference",
     "render", "render_depth_batch", "vsd_batch", "install_depth_renderer_as_reference",
+    "crop", "crop_inputs", "uncrop_keypoints", "warp_affine_batch", "install_crop_as_reference",
 ]

@@ -14,6 +14,7 @@ PVB_HOST_STAGE_VERTEX, PVB_HOST_INPLACE_MASK = 2, 4
 PVB_IPC_HANDLE_BYTES = 64
 (PVB_MASK_U8, PVB_MASK_I8, PVB_MASK_I16, PVB_MASK_I32, PVB_MASK_I64, PVB_MASK_F32, PVB_MASK_F64) = range(7)
 PVB_SELECT_BYTE, PVB_SELECT_EQ1 = 0, 1
+PVB_CROP_MASK_TO_BOX, PVB_CROP_CENTER_F64 = 1, 2
 (PVB_PNP_OK, PVB_PNP_ITERATION_LIMIT, PVB_PNP_TOO_FEW_POINTS, PVB_PNP_PLANAR, PVB_PNP_DEGENERATE) = range(5)
 
 
@@ -79,6 +80,12 @@ SIGNATURES = {
     "pvb_vsd_workspace_bytes": (_sz, [_i32]),
     "pvb_vsd": (ctypes.c_int, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _vp, _i32, _vp, ctypes.c_int64, _i32, _i32,
                                ctypes.c_double, ctypes.c_double, _vp, _vp, _sz, _vp]),
+    "pvb_crop_inputs": (ctypes.c_int, [_vp, _i32, _i32, _i32, ctypes.POINTER(ctypes.c_int64), _vp, _vp, _i32, _i32, _i32,
+                                       ctypes.c_double, ctypes.c_double, _i32, ctypes.POINTER(ctypes.c_float),
+                                       ctypes.POINTER(ctypes.c_float), _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "pvb_uncrop_keypoints": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "pvb_warp_affine_linear": (ctypes.c_int, [_vp, _i32, _i32, _i32, _i32, ctypes.POINTER(ctypes.c_int64), _vp, _vp, _i32,
+                                              _i32, _i32, _vp, _vp]),
     "pvb_vote_target":(ctypes.c_int, [_vp, _i32, ctypes.POINTER(ctypes.c_int64), _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
     "pvb_vote_loss_workspace_bytes": (_sz, [_i32, _i32, _i32]),
     "pvb_vote_loss_forward": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int64), _vp, _i32, ctypes.POINTER(ctypes.c_int64),

@@ -828,6 +828,84 @@ PVB_API int pvb_vsd(const float *depth_test, int32_t B, const float *depth_est, 
 
 namespace {
 
+// the image and output arguments the crop and the warp share; fills the image and size fields of `a`
+int warp_common(WarpArgs &a, const uint8_t *img, int32_t B, int32_t H, int32_t W, int32_t C, const int64_t *img_stride,
+                int32_t n, int32_t out_w, int32_t out_h)
+{
+    if (n < 0 || B < 0) return fail(PVB_ERR_INVALID, "negative size (n=%d B=%d)", n, B);
+    if (H < 1 || W < 1 || H > 32767 || W > 32767) return fail(PVB_ERR_INVALID, "image must be 1..32767 pixels a side (got %dx%d)", W, H);
+    if (C < 1 || C > 4) return fail(PVB_ERR_INVALID, "C must be in [1,4] (got %d)", C);
+    if (out_w < 1 || out_h < 1) return fail(PVB_ERR_INVALID, "output size must be >= 1 (got %dx%d)", out_w, out_h);
+    if ((long long)n * out_h > 0x7fffffffll) return fail(PVB_ERR_INVALID, "n * out_h too large (>= 2^31)");
+    if (!img_stride) return fail(PVB_ERR_INVALID, "NULL stride array");
+    for (int i = 0; i < 4; ++i)
+        if (img_stride[i] < 0) return fail(PVB_ERR_INVALID, "negative stride");
+    if (n > 0 && B > 0 && !img) return fail(PVB_ERR_INVALID, "NULL tensor");
+    a.img = img; a.sb = img_stride[0]; a.sh = img_stride[1]; a.sw = img_stride[2]; a.sc = img_stride[3];
+    a.B = B; a.H = H; a.W = W; a.C = C; a.n = n; a.out_w = out_w; a.out_h = out_h;
+    return PVB_OK;
+}
+
+} // namespace
+
+PVB_API int pvb_crop_inputs(const uint8_t *img, int32_t B, int32_t H, int32_t W, const int64_t *img_stride,
+                            const double *boxes, const int32_t *image_index, int32_t n, int32_t out_w, int32_t out_h,
+                            double scale_ratio, double box_ratio, int32_t flags, const float *mean, const float *std,
+                            float *inp, uint8_t *crop_u8, double *center, double *scale, double *matrix,
+                            double *matrix_inv, pvb_stream_t stream)
+{
+    WarpArgs w = {};
+    if (int rc = warp_common(w, img, B, H, W, 3, img_stride, n, out_w, out_h)) return rc;
+    if (!std::isfinite(scale_ratio) || !std::isfinite(box_ratio))
+        return fail(PVB_ERR_INVALID, "scale_ratio and box_ratio must be finite (got %g, %g)", scale_ratio, box_ratio);
+    if (box_ratio < 0) return fail(PVB_ERR_INVALID, "box_ratio must be >= 0 (got %g)", box_ratio);
+    if (flags & ~(PVB_CROP_MASK_TO_BOX | PVB_CROP_CENTER_F64)) return fail(PVB_ERR_INVALID, "unknown flags 0x%x", flags);
+    if (!mean || !std) return fail(PVB_ERR_INVALID, "NULL mean / std");
+    for (int c = 0; c < 3; ++c)
+        if (!(std[c] != 0.0f) || !std::isfinite(mean[c])) return fail(PVB_ERR_INVALID, "std must be non-zero and mean finite");
+    if (!img || !boxes || !inp || !center || !scale || !matrix) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (n == 0) return PVB_OK;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CropArgs c;
+    c.boxes = boxes; c.n = n; c.out_w = out_w; c.out_h = out_h; c.center_f64 = (flags & PVB_CROP_CENTER_F64) != 0;
+    c.scale_ratio = scale_ratio; c.center = center; c.scale = scale; c.M = matrix; c.Minv = matrix_inv;
+    cudaError_t e = launch_crop_setup(c, st);
+    if (e != cudaSuccess) return cuda_fail(e, "crop setup kernel");
+    w.M = matrix; w.image_index = image_index; w.boxes = boxes; w.mask = (flags & PVB_CROP_MASK_TO_BOX) != 0;
+    w.box_ratio = box_ratio; w.inp = inp; w.out_u8 = crop_u8;
+    for (int k = 0; k < 3; ++k) { w.mean[k] = mean[k]; w.stdv[k] = std[k]; }
+    e = launch_warp(w, true, st);
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "crop warp kernel");
+}
+
+PVB_API int pvb_uncrop_keypoints(const float *kpt_2d, const double *center, const double *scale, int32_t n, int32_t K,
+                                 int32_t in_w, int32_t in_h, double *out, pvb_stream_t stream)
+{
+    if (n < 0 || K < 0) return fail(PVB_ERR_INVALID, "negative size (n=%d K=%d)", n, K);
+    if (in_w < 1 || in_h < 1) return fail(PVB_ERR_INVALID, "input size must be >= 1 (got %dx%d)", in_w, in_h);
+    if (n == 0 || K == 0) return PVB_OK;
+    if (!kpt_2d || !center || !scale || !out) return fail(PVB_ERR_INVALID, "NULL tensor");
+    UncropArgs a;
+    a.kpt = kpt_2d; a.center = center; a.scale = scale; a.n = n; a.K = K; a.in_w = in_w; a.in_h = in_h; a.out = out;
+    cudaError_t e = launch_uncrop(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "uncrop kernel");
+}
+
+PVB_API int pvb_warp_affine_linear(const uint8_t *img, int32_t B, int32_t H, int32_t W, int32_t C, const int64_t *img_stride,
+                                   const double *M, const int32_t *image_index, int32_t n, int32_t out_w, int32_t out_h,
+                                   uint8_t *out, pvb_stream_t stream)
+{
+    WarpArgs w = {};
+    if (int rc = warp_common(w, img, B, H, W, C, img_stride, n, out_w, out_h)) return rc;
+    if (n == 0) return PVB_OK;
+    if (!img || !M || !out) return fail(PVB_ERR_INVALID, "NULL tensor");
+    w.M = M; w.image_index = image_index; w.out_u8 = out;
+    cudaError_t e = launch_warp(w, false, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "warp kernel");
+}
+
+namespace {
+
 constexpr int VOTE_LOSS_MAX_K = 1024;      // the image's keypoints live in 16 KB of shared memory
 
 // the arguments every vote-loss entry shares; fills the mask, keypoint and size fields of `a`

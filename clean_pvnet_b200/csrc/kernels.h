@@ -193,6 +193,39 @@ struct VsdArgs {
 size_t vsd_workspace_bytes(int n);
 cudaError_t launch_vsd(const VsdArgs &a, void *workspace, cudaStream_t st);
 
+// T-LESS's PVNet crop (crop.cu, DESIGN.md 8g).  Setup: one thread per box -> centre, scale, forward (and inverse) crop
+// matrix.  Warp: one CTA per (box, output row) over [n][out_h]; the crop variant masks, normalises and writes NCHW fp32.
+struct CropArgs {
+    const double *boxes;          // [n][4] xyxy, image coordinates
+    int n, out_w, out_h, center_f64;  // center_f64: the cascade's fp64 centre, else pvnet_transform's fp32 one
+    double scale_ratio;
+    double *center, *scale;       // [n][2], [n]: as the reference computes them (fp64)
+    double *M, *Minv;             // [n][6] forward crop matrix; inverse (inv=1) or NULL
+};
+cudaError_t launch_crop_setup(const CropArgs &a, cudaStream_t st);
+struct WarpArgs {
+    const unsigned char *img;     // [B][H][W][C] at element strides sb, sh, sw, sc
+    long long sb, sh, sw, sc;
+    int B, H, W, C;
+    const double *M;              // [n][6] forward matrices (warpAffine inverts them)
+    const int *image_index;       // [n] or NULL (every row reads image 0)
+    int n, out_w, out_h;
+    const double *boxes;          // crop: [n][4], for the box mask
+    int mask;                     // crop: zero what lies outside the magnified box
+    double box_ratio;
+    float mean[3], stdv[3];       // crop: normalisation
+    float *inp;                   // crop: [n][3][out_h][out_w]
+    unsigned char *out_u8;        // [n][out_h][out_w][C]: the warp's output; optional for the crop
+};
+cudaError_t launch_warp(const WarpArgs &a, bool crop, cudaStream_t st);
+struct UncropArgs {
+    const float *kpt;             // [n][K][2], crop frame
+    const double *center, *scale; // [n][2], [n]
+    int n, K, in_w, in_h;
+    double *out;                  // [n][K][2], image frame
+};
+cudaError_t launch_uncrop(const UncropArgs &a, cudaStream_t st);
+
 // PVNet's vote loss (loss.cu, DESIGN.md 8e): the target field of compute_vertex, the trainer's smooth-l1 vote loss and its
 // gradient, from the mask and the keypoints.  One thread per pixel over a (ceil(H*W / 256), B) grid; the image's keypoints
 // are staged in shared memory.

@@ -36,6 +36,10 @@
  *   utils/renderer/opengl_utils.py:405-490  DepthRender.render     pvb_render_depth (n poses per call, no OpenGL)
  *   utils/vsd/vsd_utils.py:5-48  vsd (cost 'step'), as
  *   evaluators/tless_test/pvnet.py:66-105  vsd_metric calls it     pvb_vsd (n pose pairs per call)
+ *   utils/tless/tless_test_utils.py:57-77  pvnet_transform,
+ *   networks/ct_pvnet/res.py:14-31  _crop                           pvb_crop_inputs (n boxes per call)
+ *   evaluators/tless_test/pvnet.py:229-239  keypoint un-crop        pvb_uncrop_keypoints (n boxes per call)
+ *   cv2.warpAffine(..., INTER_LINEAR)                              pvb_warp_affine_linear (n rows per call)
  *
  *   and the training side of the vote field:
  *   utils/pvnet/pvnet_data_utils.py:30-44  compute_vertex          pvb_vote_target (B images per call)
@@ -382,6 +386,47 @@ PVB_API int pvb_vsd(const float *depth_test, int32_t B, const float *depth_est, 
                     const float *depth_gt, int32_t n_gt, int32_t gt_base, const int32_t *pairs, int32_t n, const double *K,
                     int64_t k_stride, int32_t H, int32_t W, double delta, double tau, double *e, void *workspace,
                     size_t workspace_bytes, pvb_stream_t stream);
+
+/* ---- T-LESS's PVNet crop and un-crop (DESIGN.md section 8g) ---------------------------------------------------------
+ * Shared: img device uint8 [B,H,W,C] at element strides img_stride (HOST int64[4], for B, H, W, C), H, W <= 32767;
+ * image_index device int32 [n] or NULL (every row reads image 0; an index outside [0, B) reads as an all-border image).
+ * Pixels follow cv2.warpAffine(INTER_LINEAR) with the zero border exactly: the forward matrix inverted as warpAffine
+ * inverts it, 10-bit offsets rounded half to even, 5-bit sub-pixel positions, 15-bit integer bilinear weights.
+ * n * out_h < 2^31.  Bad arguments return PVB_ERR_INVALID before any CUDA call; n == 0 is a no-op. */
+#define PVB_CROP_MASK_TO_BOX 1     /* zero what lies outside the magnified box (pvnet_transform; the cascade does not) */
+#define PVB_CROP_CENTER_F64  2     /* the cascade's fp64 centre (res.py _crop), else pvnet_transform's fp32 centre */
+
+/* Replaces tless_test_utils.pvnet_transform (lib/utils/tless/tless_test_utils.py:57-77) and, with flags =
+ * PVB_CROP_CENTER_F64, the cascade's _crop (lib/networks/ct_pvnet/res.py:14-31), for n boxes (device fp64 [n,4] xyxy):
+ *   center = ((x0 + x2) / 2, (y0 + y2) / 2) (rounded to fp32 unless PVB_CROP_CENTER_F64), scale = max(x2 - x0, y2 - y0) *
+ *   scale_ratio; matrix = get_affine_transform(center, scale, 0, [out_w, out_h]) bit for bit with cv2.getAffineTransform
+ *   (all zeros for a singular system, as cv2 returns), matrix_inv the same with inv=1 (optional);
+ *   crop = cv2.warpAffine(img, matrix, (out_w, out_h)), zeroed outside magnify_box(box corners through matrix,
+ *   box_ratio) under PVB_CROP_MASK_TO_BOX; inp = (crop / 255 - mean) / std in fp32 (mean, std HOST float[3], std != 0).
+ * Outputs (device): inp fp32 [n,3,out_h,out_w] (NCHW), crop_u8 uint8 [n,out_h,out_w,3] or NULL (the dataset's orig_img),
+ * center fp64 [n,2], scale fp64 [n] (the unrounded product; get_affine_transform uses it rounded to fp32), matrix fp64
+ * [n,2,3], matrix_inv fp64 [n,2,3] or NULL.  C must be 3.  The output is bit-identical run to run and a box's output
+ * does not depend on the other boxes. */
+PVB_API int pvb_crop_inputs(const uint8_t *img, int32_t B, int32_t H, int32_t W, const int64_t *img_stride,
+                            const double *boxes, const int32_t *image_index, int32_t n, int32_t out_w, int32_t out_h,
+                            double scale_ratio, double box_ratio, int32_t flags, const float *mean, const float *std,
+                            float *inp, uint8_t *crop_u8, double *center, double *scale, double *matrix,
+                            double *matrix_inv, pvb_stream_t stream);
+
+/* Replaces the evaluator's affine_transform(kpt_2d, get_affine_transform(center, scale, 0, [in_w, in_h], inv=1))
+ * (lib/evaluators/tless_test/pvnet.py:229-239) for n boxes: kpt_2d device fp32 [n,K,2] in the crop frame, center device
+ * fp64 [n,2], scale device fp64 [n] (rounded to fp32, as get_affine_transform does) -> out device fp64 [n,K,2] in the
+ * image.  The matrix is bit for bit cv2's; the product follows np.dot's rounding on x86-64 OpenBLAS (y * m1 fused into
+ * the rounded x * m0), pinned to <= 1e-12 px. */
+PVB_API int pvb_uncrop_keypoints(const float *kpt_2d, const double *center, const double *scale, int32_t n, int32_t K,
+                                 int32_t in_w, int32_t in_h, double *out, pvb_stream_t stream);
+
+/* cv2.warpAffine(img[image_index[i]], M[i], (out_w, out_h), flags=INTER_LINEAR) (zero border) for n rows: M device fp64
+ * [n,2,3] forward matrices, C in 1..4, out device uint8 [n,out_h,out_w,C].  Also the detector's full-image resize
+ * (tless_test_utils.augment, lib/utils/tless/tless_test_utils.py:14-31). */
+PVB_API int pvb_warp_affine_linear(const uint8_t *img, int32_t B, int32_t H, int32_t W, int32_t C, const int64_t *img_stride,
+                                   const double *M, const int32_t *image_index, int32_t n, int32_t out_w, int32_t out_h,
+                                   uint8_t *out, pvb_stream_t stream);
 
 /* ---- training: PVNet's vote loss from the mask and the keypoints (DESIGN.md section 8e) ----------------------------
  * The trainer supervises the unit-vector field with a dense target that every dataset builds on the host
