@@ -19,6 +19,8 @@ Public surface (same names/signatures as the reference):
     vsd_batch (T-LESS's VSD error for n pose pairs), install_depth_renderer_as_reference
     crop.crop_inputs (T-LESS's PVNet crop, pvnet_transform, for n boxes), uncrop_keypoints (the evaluator's un-crop),
     warp_affine_batch (cv2.warpAffine INTER_LINEAR for n rows), install_crop_as_reference (the cascade's crop)
+    dcn.dcn_v2_conv / DCNv2 / DCN (twins of lib/networks/dcn_v2.py, the detector's deformable convolution, forward and
+    backward), install_dcn_as_reference_module (call it before anything imports lib.networks.ct*)
 """
 from . import _lib  # noqa: F401
 from . import nn  # noqa: F401
@@ -38,6 +40,8 @@ from . import render  # noqa: F401
 from .render import render_depth_batch, vsd_batch, install_depth_renderer_as_reference  # noqa: F401
 from . import crop  # noqa: F401
 from .crop import crop_inputs, uncrop_keypoints, warp_affine_batch, install_crop_as_reference  # noqa: F401
+from . import dcn  # noqa: F401
+from .dcn import dcn_v2_conv, DCNv2, DCN, install_dcn_as_reference_module  # noqa: F401
 from .vote_loss import vote_loss, vote_target_batch, NetworkWrapper, install_vote_loss_as_reference  # noqa: F401
 from .ransac_voting_gpu import (  # noqa: F401
     estimate_voting_distribution_with_mean,
@@ -57,4 +61,5 @@ __all__ = [
     "vote_loss", "vote_target_batch", "NetworkWrapper", "install_vote_loss_as_reference",
     "render", "render_depth_batch", "vsd_batch", "install_depth_renderer_as_reference",
     "crop", "crop_inputs", "uncrop_keypoints", "warp_affine_batch", "install_crop_as_reference",
+    "dcn", "dcn_v2_conv", "DCNv2", "DCN", "install_dcn_as_reference_module",
 ]

@@ -48,6 +48,12 @@ class PvbPnpOptions(ctypes.Structure):
                 ("parameter_tolerance", ctypes.c_double)]
 
 
+class PvbDcnDesc(ctypes.Structure):
+    """== struct pvb_dcn_desc (include/pvnet_vote_b200.h)"""
+    _fields_ = [(n, ctypes.c_int32) for n in ("B", "C", "H", "W", "C_out", "kh", "kw", "stride_h", "stride_w", "pad_h",
+                                             "pad_w", "dilation_h", "dilation_w", "deformable_groups")]
+
+
 # every symbol include/pvnet_vote_b200.h declares: name -> (restype, argtypes)
 _vp, _i32, _sz, _f = ctypes.c_void_p, ctypes.c_int32, ctypes.c_size_t, ctypes.c_float
 _dp, _lp = ctypes.POINTER(PvbDesc), ctypes.POINTER(PvbLayout)
@@ -92,6 +98,10 @@ SIGNATURES = {
                                              _vp, _vp, _i32, _i32, _i32, _i32, _vp, _sz, _vp]),
     "pvb_vote_loss_backward": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int64), _vp, _i32, ctypes.POINTER(ctypes.c_int64),
                                               _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _sz, _vp]),
+    "pvb_dcn_forward": (ctypes.c_int, [ctypes.POINTER(PvbDcnDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "pvb_dcn_backward_workspace_bytes": (_sz, [ctypes.POINTER(PvbDcnDesc), _i32]),
+    "pvb_dcn_backward": (ctypes.c_int, [ctypes.POINTER(PvbDcnDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                        _i32, _vp, _sz, _vp]),
     "pvb_read_status": (ctypes.c_int, [_dp, _vp, _vp]),
     "pvb_host_scratch_bytes": (_sz, [_dp, _i32]),
     "pvb_ransac_voting_v3_host": (ctypes.c_int, [_dp, _vp, _vp, _vp, _i32, ctypes.c_uint32, _vp, _sz, _vp]),

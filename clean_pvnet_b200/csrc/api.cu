@@ -705,6 +705,81 @@ PVB_API int pvb_nearest_point_idx(const float *ref, const float *que, int32_t *i
     return e == cudaSuccess ? PVB_OK : cuda_fail(e, "nearest point kernels");
 }
 
+namespace {
+
+// checks a DCN descriptor and fills the kernels' argument block; PVB_OK or PVB_ERR_INVALID (no CUDA call)
+int dcn_args(const pvb_dcn_desc *d, DcnArgs &a)
+{
+    if (!d) return fail(PVB_ERR_INVALID, "descriptor is NULL");
+    if (d->B < 0 || d->C < 1 || d->H < 1 || d->W < 1 || d->C_out < 1 || d->kh < 1 || d->kw < 1)
+        return fail(PVB_ERR_INVALID, "bad shape B=%d C=%d H=%d W=%d C_out=%d kh=%d kw=%d", d->B, d->C, d->H, d->W,
+                    d->C_out, d->kh, d->kw);
+    if (d->stride_h < 1 || d->stride_w < 1 || d->pad_h < 0 || d->pad_w < 0 || d->dilation_h < 1 || d->dilation_w < 1)
+        return fail(PVB_ERR_INVALID, "bad stride/pad/dilation (%d,%d)/(%d,%d)/(%d,%d)", d->stride_h, d->stride_w,
+                    d->pad_h, d->pad_w, d->dilation_h, d->dilation_w);
+    if (d->deformable_groups < 1 || d->C % d->deformable_groups)
+        return fail(PVB_ERR_INVALID, "deformable_groups=%d must be >= 1 and divide C=%d", d->deformable_groups, d->C);
+    const long long ext_h = (long long)d->dilation_h * (d->kh - 1) + 1, ext_w = (long long)d->dilation_w * (d->kw - 1) + 1;
+    const long long span_h = d->H + 2ll * d->pad_h, span_w = d->W + 2ll * d->pad_w;
+    if (span_h > (1ll << 30) || span_w > (1ll << 30) || ext_h > (1ll << 30) || ext_w > (1ll << 30))
+        return fail(PVB_ERR_INVALID, "padded input or dilated kernel extent >= 2^30");
+    if (span_h < ext_h || span_w < ext_w) return fail(PVB_ERR_INVALID, "the dilated kernel does not fit the padded input");
+    const long long Ho = (span_h - ext_h) / d->stride_h + 1, Wo = (span_w - ext_w) / d->stride_w + 1;
+    const long long K = (long long)d->C * d->kh * d->kw, T = (long long)d->kh * d->kw;
+    if (d->B > 65535) return fail(PVB_ERR_INVALID, "B=%d > 65535", d->B);
+    if ((long long)d->H * d->W >= (1ll << 31) || Ho * Wo >= (1ll << 31)) return fail(PVB_ERR_INVALID, "H*W or Ho*Wo >= 2^31");
+    if (K > 65535ll * 64 || d->C_out > 65535 * 64) return fail(PVB_ERR_INVALID, "C*kh*kw or C_out > 4194240");
+    if (T * d->deformable_groups > 65535) return fail(PVB_ERR_INVALID, "deformable_groups*kh*kw > 65535");
+    a = DcnArgs{};
+    a.B = d->B; a.C = d->C; a.H = d->H; a.W = d->W; a.Co = d->C_out; a.kh = d->kh; a.kw = d->kw;
+    a.sh = d->stride_h; a.sw = d->stride_w; a.ph = d->pad_h; a.pw = d->pad_w; a.dh = d->dilation_h; a.dw = d->dilation_w;
+    a.dg = d->deformable_groups; a.Ho = (int)Ho; a.Wo = (int)Wo;
+    return PVB_OK;
+}
+
+size_t dcn_workspace_bytes(const DcnPlan &p) { return p.cols_bytes + p.part_bytes; }
+
+} // namespace
+
+PVB_API int pvb_dcn_forward(const pvb_dcn_desc *d, const float *input, const float *offset, const float *mask,
+                            const float *weight, const float *bias, float *output, pvb_stream_t stream)
+{
+    DcnArgs a;
+    if (int rc = dcn_args(d, a)) return rc;
+    if (a.B == 0) return PVB_OK;
+    if (!input || !offset || !mask || !weight || !bias || !output) return fail(PVB_ERR_INVALID, "NULL tensor");
+    a.input = input; a.offset = offset; a.mask = mask; a.weight = weight; a.bias = bias; a.out = output;
+    cudaError_t e = launch_dcn_forward(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "dcn forward kernel");
+}
+
+PVB_API size_t pvb_dcn_backward_workspace_bytes(const pvb_dcn_desc *d, int32_t chunk)
+{
+    DcnArgs a;
+    if (!d || d->B < 1 || dcn_args(d, a) != PVB_OK) return 0;
+    return dcn_workspace_bytes(dcn_plan(a, chunk));
+}
+
+PVB_API int pvb_dcn_backward(const pvb_dcn_desc *d, const float *input, const float *offset, const float *mask,
+                             const float *weight, const float *grad_output, float *grad_input, float *grad_offset,
+                             float *grad_mask, float *grad_weight, float *grad_bias, int32_t chunk, void *workspace,
+                             size_t workspace_bytes, pvb_stream_t stream)
+{
+    DcnArgs a;
+    if (int rc = dcn_args(d, a)) return rc;
+    if (a.B == 0) return PVB_OK;
+    if (!input || !offset || !mask || !weight || !grad_output || !grad_input || !grad_offset || !grad_mask ||
+        !grad_weight || !grad_bias)
+        return fail(PVB_ERR_INVALID, "NULL tensor");
+    const DcnPlan plan = dcn_plan(a, chunk);
+    if (int rc = nn_check_workspace(dcn_workspace_bytes(plan), workspace, workspace_bytes)) return rc;
+    a.input = input; a.offset = offset; a.mask = mask; a.weight = weight; a.grad_out = grad_output;
+    a.grad_input = grad_input; a.grad_offset = grad_offset; a.grad_mask = grad_mask; a.grad_weight = grad_weight;
+    a.grad_bias = grad_bias;
+    cudaError_t e = launch_dcn_backward(a, plan, workspace, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "dcn backward kernels");
+}
+
 PVB_API size_t pvb_add_metric_workspace_bytes(int32_t n, int32_t pn, int32_t syn)
 {
     if (n <= 0 || pn < 0 || (syn != 0 && syn != 1)) return 0;

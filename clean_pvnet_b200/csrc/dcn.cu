@@ -1,0 +1,442 @@
+// Modulated deformable convolution (DCNv2), fp32 NCHW, forward and backward: the device twin of clean-pvnet's
+// lib/csrc/dcn_v2 extension (dcn_v2_cuda.cu + dcn_v2_im2col_cuda.cu), which the DLA-34 CenterNet detector runs.
+//
+// The reference writes the whole column matrix cols[b][c*kh*kw + i*kw + j][ho*Wo + wo] (im2col) and multiplies it by
+// the weight with batched SGEMM; its backward loops over the images.  Here the forward is one implicit-GEMM kernel
+// whose B-operand tiles are sampled straight into shared memory, so the columns are never stored, and the backward runs
+// the whole batch: grad_cols = W^T grad_out in image chunks (the only stored column matrix), one kernel for
+// grad_offset + grad_mask, one for grad_input (float atomics, as the reference), grad_weight re-sampling the columns in
+// split-K partials reduced in a fixed order, and a fixed-order grad_bias.  Everything but grad_input is bitwise
+// reproducible.  All arithmetic is FP32 FFMA (no TF32, no tensor cores).
+//
+// A sample point of (pixel, tap, deformable group) has four corner offsets and four bilinear weights that do not depend
+// on the channel: they are computed once per tile and reused over the group's channels.  The sampled value is the
+// reference kernel's bit for bit: nvcc contracts its `w1*v1 + w2*v2 + w3*v3 + w4*v4` (dcn_v2_im2col_cuda.cu:52) into
+// fma(w4,v4, fma(w3,v3, fma(w1,v1, w2*v2))) at sm_90a (read off the reference build's SASS), written out below with
+// explicit intrinsics; the mask multiplies after the bilinear sum.
+#include "kernels.h"
+
+namespace pvb {
+namespace {
+
+constexpr int BM = 64, BN = 128, BK = 16, NT = 256;   // CTA tile (rows x columns x depth), threads
+constexpr int GW_TARGET_CTAS = 528;                    // grad_weight: split the reduction until ~4 CTAs per H100 SM
+
+// The sample point (h, w) of the reference (dcn_v2_im2col_cuda.cu:177-187): used only when h > -1, w > -1, h < H,
+// w < W (so NaN gives 0); a corner counts only inside the image.  off = -1 marks a corner that reads as 0.
+struct Corners { int off[4]; float wt[4]; };
+
+__device__ __forceinline__ Corners sample_point(float h, float w, int H, int W)
+{
+    Corners s;
+    if (h > -1.f && w > -1.f && h < (float)H && w < (float)W) {
+        const int hl = (int)floorf(h), wl = (int)floorf(w);
+        const float lh = __fsub_rn(h, (float)hl), lw = __fsub_rn(w, (float)wl);
+        const float hh = __fsub_rn(1.f, lh), hw = __fsub_rn(1.f, lw);
+        s.wt[0] = __fmul_rn(hh, hw); s.wt[1] = __fmul_rn(hh, lw); s.wt[2] = __fmul_rn(lh, hw); s.wt[3] = __fmul_rn(lh, lw);
+        s.off[0] = (hl >= 0 && wl >= 0) ? hl * W + wl : -1;
+        s.off[1] = (hl >= 0 && wl + 1 <= W - 1) ? hl * W + wl + 1 : -1;
+        s.off[2] = (hl + 1 <= H - 1 && wl >= 0) ? (hl + 1) * W + wl : -1;
+        s.off[3] = (hl + 1 <= H - 1 && wl + 1 <= W - 1) ? (hl + 1) * W + wl + 1 : -1;
+    } else {
+        for (int q = 0; q < 4; ++q) { s.off[q] = -1; s.wt[q] = 0.f; }
+    }
+    return s;
+}
+
+__device__ __forceinline__ float bilinear(const float *plane, const int off[4], const float wt[4])
+{
+    const float v1 = off[0] >= 0 ? __ldg(plane + off[0]) : 0.f;
+    const float v2 = off[1] >= 0 ? __ldg(plane + off[1]) : 0.f;
+    const float v3 = off[2] >= 0 ? __ldg(plane + off[2]) : 0.f;
+    const float v4 = off[3] >= 0 ? __ldg(plane + off[3]) : 0.f;
+    return __fmaf_rn(wt[3], v4, __fmaf_rn(wt[2], v3, __fmaf_rn(wt[0], v1, __fmul_rn(wt[1], v2))));
+}
+
+// the sample coordinate of output pixel p at tap (i, j): float(ho*s - p + i*d) + offset, rounded once
+__device__ __forceinline__ void sample_coord(const DcnArgs &a, long long ob, int tap, int p, float &h, float &w)
+{
+    const int ho = p / a.Wo, wo = p - (p / a.Wo) * a.Wo;
+    const int i = tap / a.kw, j = tap - (tap / a.kw) * a.kw;
+    const long long P = (long long)a.Ho * a.Wo;
+    const float dy = __ldg(a.offset + ob + (2ll * tap) * P + p);
+    const float dx = __ldg(a.offset + ob + (2ll * tap + 1) * P + p);
+    h = __fadd_rn((float)(ho * a.sh - a.ph + i * a.dh), dy);
+    w = __fadd_rn((float)(wo * a.sw - a.pw + j * a.dw), dx);
+}
+
+// shared-memory sample table of one tile: corners, weights and mask of up to BN sample points
+struct SampleTable { int off[4][BN]; float wt[4][BN]; float m[BN]; };
+
+__device__ __forceinline__ void store_sample(SampleTable &t, int n, const Corners &s, float m)
+{
+    for (int q = 0; q < 4; ++q) { t.off[q][n] = s.off[q]; t.wt[q][n] = s.wt[q]; }
+    t.m[n] = m;
+}
+
+__device__ __forceinline__ float sample_col(const SampleTable &t, int n, const float *plane)
+{
+    const int off[4] = {t.off[0][n], t.off[1][n], t.off[2][n], t.off[3][n]};
+    const float wt[4] = {t.wt[0][n], t.wt[1][n], t.wt[2][n], t.wt[3][n]};
+    return __fmul_rn(t.m[n], bilinear(plane, off, wt));
+}
+
+// acc[4][8] += As[.][tm*4 + 0..3] x Bs[.][tn*4 + 0..3, 64 + tn*4 + 0..3] over the BK-deep tile, in k order
+__device__ __forceinline__ void mma_tile(const float (&As)[BK][BM], const float (&Bs)[BK][BN], float (&acc)[4][8],
+                                         int tm, int tn)
+{
+#pragma unroll
+    for (int k = 0; k < BK; ++k) {
+        const float4 av = *reinterpret_cast<const float4 *>(&As[k][tm * 4]);
+        const float4 b0 = *reinterpret_cast<const float4 *>(&Bs[k][tn * 4]);
+        const float4 b1 = *reinterpret_cast<const float4 *>(&Bs[k][64 + tn * 4]);
+        const float ar[4] = {av.x, av.y, av.z, av.w};
+        const float br[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+            for (int c = 0; c < 8; ++c) acc[r][c] = __fmaf_rn(ar[r], br[c], acc[r][c]);
+    }
+}
+
+__device__ __forceinline__ int col_of(int tn, int c) { return c < 4 ? tn * 4 + c : 64 + tn * 4 + (c - 4); }
+
+// out[b][o][p] = bias[o] + sum over (g, tap, c in group g) of W[o][c*T + tap] * cols[b][c*T + tap][p]
+// grid (ceil(P / BN), ceil(Co / BM), B)
+__global__ void __launch_bounds__(NT) dcn_forward_kernel(DcnArgs a)
+{
+    __shared__ __align__(16) float As[BK][BM];
+    __shared__ __align__(16) float Bs[BK][BN];
+    __shared__ SampleTable st;
+    const int tid = threadIdx.x, tm = tid / 16, tn = tid % 16;
+    const int P = a.Ho * a.Wo, p0 = blockIdx.x * BN, o0 = blockIdx.y * BM, b = blockIdx.z;
+    const int T = a.kh * a.kw, Cg = a.C / a.dg;
+    const long long K = (long long)a.C * T, HW = (long long)a.H * a.W;
+
+    float acc[4][8];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+        const int o = o0 + tm * 4 + r;
+        const float bv = o < a.Co ? __ldg(a.bias + o) : 0.f;
+#pragma unroll
+        for (int c = 0; c < 8; ++c) acc[r][c] = bv;
+    }
+
+    for (int g = 0; g < a.dg; ++g) {
+        const long long ob = ((long long)b * a.dg + g) * 2 * T * P;
+        const long long mb = ((long long)b * a.dg + g) * T * P;
+        for (int tap = 0; tap < T; ++tap) {
+            __syncthreads();                                     // the previous tap's tiles are consumed
+            if (tid < BN) {
+                const int p = p0 + tid;
+                if (p < P) {
+                    float h, w;
+                    sample_coord(a, ob, tap, p, h, w);
+                    store_sample(st, tid, sample_point(h, w, a.H, a.W), __ldg(a.mask + mb + (long long)tap * P + p));
+                } else {
+                    Corners z;
+                    for (int q = 0; q < 4; ++q) { z.off[q] = -1; z.wt[q] = 0.f; }
+                    store_sample(st, tid, z, 0.f);
+                }
+            }
+            for (int c0 = 0; c0 < Cg; c0 += BK) {
+                __syncthreads();                                 // sample table ready; previous tile consumed
+#pragma unroll
+                for (int r = 0; r < BK * BM / NT; ++r) {
+                    const int e = tid + r * NT, k = e / BM, m = e % BM;
+                    const int o = o0 + m, c = g * Cg + c0 + k;
+                    As[k][m] = (o < a.Co && c0 + k < Cg) ? __ldg(a.weight + (long long)o * K + (long long)c * T + tap) : 0.f;
+                }
+#pragma unroll
+                for (int r = 0; r < BK * BN / NT; ++r) {
+                    const int e = tid + r * NT, k = e / BN, n = e % BN;
+                    const int c = g * Cg + c0 + k;
+                    Bs[k][n] = (c0 + k < Cg && p0 + n < P) ? sample_col(st, n, a.input + ((long long)b * a.C + c) * HW) : 0.f;
+                }
+                __syncthreads();
+                mma_tile(As, Bs, acc, tm, tn);
+            }
+        }
+    }
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+        const int o = o0 + tm * 4 + r;
+        if (o >= a.Co) continue;
+        float *dst = a.out + ((long long)b * a.Co + o) * P;
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+            const int p = p0 + col_of(tn, c);
+            if (p < P) dst[p] = acc[r][c];
+        }
+    }
+}
+
+// grad_cols[bl][k][p] = sum over o (in order) of W[o][k] * grad_out[b0 + bl][o][p]
+// grid (ceil(P / BN), ceil(K / BM), nb)
+__global__ void __launch_bounds__(NT) dcn_grad_cols_kernel(DcnArgs a, int b0)
+{
+    __shared__ __align__(16) float As[BK][BM];
+    __shared__ __align__(16) float Bs[BK][BN];
+    const int tid = threadIdx.x, tm = tid / 16, tn = tid % 16;
+    const int P = a.Ho * a.Wo, p0 = blockIdx.x * BN, k0 = blockIdx.y * BM, bl = blockIdx.z;
+    const long long K = (long long)a.C * a.kh * a.kw;
+    const float *go = a.grad_out + (long long)(b0 + bl) * a.Co * P;
+    float acc[4][8] = {};
+    for (int o0 = 0; o0 < a.Co; o0 += BK) {
+        __syncthreads();
+#pragma unroll
+        for (int r = 0; r < BK * BM / NT; ++r) {
+            const int e = tid + r * NT, kk = e / BM, m = e % BM;
+            As[kk][m] = (o0 + kk < a.Co && k0 + m < K) ? __ldg(a.weight + (long long)(o0 + kk) * K + k0 + m) : 0.f;
+        }
+#pragma unroll
+        for (int r = 0; r < BK * BN / NT; ++r) {
+            const int e = tid + r * NT, kk = e / BN, n = e % BN;
+            Bs[kk][n] = (o0 + kk < a.Co && p0 + n < P) ? __ldg(go + (long long)(o0 + kk) * P + p0 + n) : 0.f;
+        }
+        __syncthreads();
+        mma_tile(As, Bs, acc, tm, tn);
+    }
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+        const long long k = k0 + tm * 4 + r;
+        if (k >= K) continue;
+        float *dst = a.cols + ((long long)bl * K + k) * P;
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+            const int p = p0 + col_of(tn, c);
+            if (p < P) dst[p] = acc[r][c];
+        }
+    }
+}
+
+// grad_offset and grad_mask of one (image, group, tap, pixel), summed over the group's channels in order
+// (the reference's col2im_coord, dcn_v2_im2col_cuda.cu:256-327).  grid (ceil(P / 256), dg * T, nb)
+__global__ void __launch_bounds__(256) dcn_grad_coord_kernel(DcnArgs a, int b0)
+{
+    const int P = a.Ho * a.Wo, p = blockIdx.x * 256 + threadIdx.x;
+    if (p >= P) return;
+    const int T = a.kh * a.kw, g = blockIdx.y / T, tap = blockIdx.y % T, bl = blockIdx.z, b = b0 + bl;
+    const int Cg = a.C / a.dg;
+    const long long HW = (long long)a.H * a.W, K = (long long)a.C * T;
+    const long long ob = ((long long)b * a.dg + g) * 2 * T * P, mb = ((long long)b * a.dg + g) * T * P;
+    float h, w;
+    sample_coord(a, ob, tap, p, h, w);
+    const float m = __ldg(a.mask + mb + (long long)tap * P + p);
+    float gy = 0.f, gx = 0.f, gm = 0.f;
+    // a point with h <= -1, w <= -1, h >= H or w >= W contributes nothing (the reference's predicate: NaN passes it)
+    if (!(h <= -1.f || w <= -1.f || h >= (float)a.H || w >= (float)a.W)) {
+        const Corners s = sample_point(h, w, a.H, a.W);
+        const int hl = (int)floorf(h), wl = (int)floorf(w);
+        // d(bilinear)/dh and /dw per corner; at integer h the derivative is that of the cell [floor h, floor h + 1]
+        const float ah = __fsub_rn((float)(hl + 1), h), bh = __fsub_rn(h, (float)hl);
+        const float aw = __fsub_rn((float)(wl + 1), w), bw = __fsub_rn(w, (float)wl);
+        const float *cp = a.cols + ((long long)bl * K + (long long)(g * Cg) * T + tap) * P + p;
+        const float *ip = a.input + ((long long)b * a.C + (long long)g * Cg) * HW;
+        for (int c = 0; c < Cg; ++c, cp += (long long)T * P, ip += HW) {
+            const float col = __ldg(cp);
+            const float v1 = s.off[0] >= 0 ? __ldg(ip + s.off[0]) : 0.f;
+            const float v2 = s.off[1] >= 0 ? __ldg(ip + s.off[1]) : 0.f;
+            const float v3 = s.off[2] >= 0 ? __ldg(ip + s.off[2]) : 0.f;
+            const float v4 = s.off[3] >= 0 ? __ldg(ip + s.off[3]) : 0.f;
+            const float val = __fmaf_rn(s.wt[3], v4, __fmaf_rn(s.wt[2], v3, __fmaf_rn(s.wt[0], v1, __fmul_rn(s.wt[1], v2))));
+            const float wy = -aw * v1 - bw * v2 + aw * v3 + bw * v4;
+            const float wx = -ah * v1 + ah * v2 - bh * v3 + bh * v4;
+            const float cm = col * m;
+            gm = __fmaf_rn(col, val, gm);
+            gy = __fmaf_rn(wy, cm, gy);
+            gx = __fmaf_rn(wx, cm, gx);
+        }
+    }
+    a.grad_offset[ob + (2ll * tap) * P + p] = gy;
+    a.grad_offset[ob + (2ll * tap + 1) * P + p] = gx;
+    a.grad_mask[mb + (long long)tap * P + p] = gm;
+}
+
+// grad_input += the bilinear weights x grad_cols x mask, scattered with float atomics (the reference's col2im,
+// dcn_v2_im2col_cuda.cu:197-254).  grid (ceil(P / 256), dg * T, nb)
+__global__ void __launch_bounds__(256) dcn_grad_input_kernel(DcnArgs a, int b0)
+{
+    const int P = a.Ho * a.Wo, p = blockIdx.x * 256 + threadIdx.x;
+    if (p >= P) return;
+    const int T = a.kh * a.kw, g = blockIdx.y / T, tap = blockIdx.y % T, bl = blockIdx.z, b = b0 + bl;
+    const int Cg = a.C / a.dg;
+    const long long HW = (long long)a.H * a.W, K = (long long)a.C * T;
+    const long long ob = ((long long)b * a.dg + g) * 2 * T * P, mb = ((long long)b * a.dg + g) * T * P;
+    float h, w;
+    sample_coord(a, ob, tap, p, h, w);
+    if (!(h > -1.f && w > -1.f && h < (float)a.H && w < (float)a.W)) return;
+    const float m = __ldg(a.mask + mb + (long long)tap * P + p);
+    const int hl = (int)floorf(h), wl = (int)floorf(w);
+    // corner (y, x) gets (1 - |h - y|)(1 - |w - x|) when |h - y| < 1 and |w - x| < 1 and it lies in the image
+    const bool hi_h = h > (float)hl, hi_w = w > (float)wl;
+    const float ly = __fsub_rn((float)(hl + 1), h), uy = __fsub_rn(__fadd_rn(h, 1.f), (float)(hl + 1));
+    const float lx = __fsub_rn((float)(wl + 1), w), ux = __fsub_rn(__fadd_rn(w, 1.f), (float)(wl + 1));
+    int off[4]; float wt[4];
+    off[0] = (hl >= 0 && wl >= 0) ? hl * a.W + wl : -1;                                     wt[0] = __fmul_rn(ly, lx);
+    off[1] = (hl >= 0 && hi_w && wl + 1 < a.W) ? hl * a.W + wl + 1 : -1;                    wt[1] = __fmul_rn(ly, ux);
+    off[2] = (hi_h && hl + 1 < a.H && wl >= 0) ? (hl + 1) * a.W + wl : -1;                  wt[2] = __fmul_rn(uy, lx);
+    off[3] = (hi_h && hi_w && hl + 1 < a.H && wl + 1 < a.W) ? (hl + 1) * a.W + wl + 1 : -1; wt[3] = __fmul_rn(uy, ux);
+    const float *cp = a.cols + ((long long)bl * K + (long long)(g * Cg) * T + tap) * P + p;
+    float *gp = a.grad_input + ((long long)b * a.C + (long long)g * Cg) * HW;
+    for (int c = 0; c < Cg; ++c, cp += (long long)T * P, gp += HW) {
+        const float top = __fmul_rn(__ldg(cp), m);
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+            if (off[q] >= 0) atomicAdd(gp + off[q], __fmul_rn(wt[q], top));
+    }
+}
+
+// split s of grad_weight: part[s][o][c*T + tap] = sum over the split's (image, pixel) range, in order, of
+// grad_out[b][o][p] * cols[b][c*T + tap][p], with the columns re-sampled like the forward.
+// grid (ntile_n, ceil(Co / BM), S); tile n covers channels cb .. cb + BN - 1 of group g at tap
+__global__ void __launch_bounds__(NT) dcn_grad_weight_kernel(DcnArgs a, long long span, float *part)
+{
+    __shared__ __align__(16) float As[BK][BM];
+    __shared__ __align__(16) float Bs[BK][BN];
+    __shared__ int sb[BK], sp[BK];
+    __shared__ struct { int off[4][BK]; float wt[4][BK]; float m[BK]; } st;
+    const int tid = threadIdx.x, tm = tid / 16, tn = tid % 16;
+    const int T = a.kh * a.kw, Cg = a.C / a.dg, nct = (Cg + BN - 1) / BN;
+    const int g = blockIdx.x / (T * nct), tap = (blockIdx.x / nct) % T, cb = (blockIdx.x % nct) * BN;
+    const int o0 = blockIdx.y * BM, P = a.Ho * a.Wo;
+    const long long K = (long long)a.C * T, HW = (long long)a.H * a.W, Q = (long long)a.B * P;
+    const long long q0 = (long long)blockIdx.z * span, q1 = min(Q, q0 + span);
+    float acc[4][8] = {};
+    for (long long qs = q0; qs < q1; qs += BK) {
+        __syncthreads();
+        if (tid < BK) {
+            const long long q = qs + tid;
+            Corners s;
+            float m = 0.f;
+            int b = 0, p = 0;
+            if (q < q1) {
+                b = (int)(q / P); p = (int)(q - (long long)b * P);
+                float h, w;
+                sample_coord(a, ((long long)b * a.dg + g) * 2 * T * P, tap, p, h, w);
+                s = sample_point(h, w, a.H, a.W);
+                m = __ldg(a.mask + ((long long)b * a.dg + g) * T * P + (long long)tap * P + p);
+            } else {
+                for (int k = 0; k < 4; ++k) { s.off[k] = -1; s.wt[k] = 0.f; }
+            }
+            for (int k = 0; k < 4; ++k) { st.off[k][tid] = s.off[k]; st.wt[k][tid] = s.wt[k]; }
+            st.m[tid] = m; sb[tid] = b; sp[tid] = p;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int r = 0; r < BK * BM / NT; ++r) {       // pixel-fastest: 16 lanes read 16 consecutive pixels
+            const int e = tid + r * NT, kk = e % BK, m = e / BK, o = o0 + m;
+            As[kk][m] = (qs + kk < q1 && o < a.Co) ? __ldg(a.grad_out + ((long long)sb[kk] * a.Co + o) * P + sp[kk]) : 0.f;
+        }
+#pragma unroll
+        for (int r = 0; r < BK * BN / NT; ++r) {
+            const int e = tid + r * NT, kk = e % BK, n = e / BK, c = cb + n;
+            float v = 0.f;
+            if (qs + kk < q1 && c < Cg) {
+                const int off[4] = {st.off[0][kk], st.off[1][kk], st.off[2][kk], st.off[3][kk]};
+                const float wt[4] = {st.wt[0][kk], st.wt[1][kk], st.wt[2][kk], st.wt[3][kk]};
+                v = __fmul_rn(st.m[kk], bilinear(a.input + ((long long)sb[kk] * a.C + g * Cg + c) * HW, off, wt));
+            }
+            Bs[kk][n] = v;
+        }
+        __syncthreads();
+        mma_tile(As, Bs, acc, tm, tn);
+    }
+    float *dst = part + (long long)blockIdx.z * a.Co * K;
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+        const int o = o0 + tm * 4 + r;
+        if (o >= a.Co) continue;
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+            const int ch = cb + col_of(tn, c);
+            if (ch < Cg) dst[(long long)o * K + (long long)(g * Cg + ch) * T + tap] = acc[r][c];
+        }
+    }
+}
+
+// grad_weight[i] = sum over s = 0 .. S-1 (in order) of part[s][i]
+__global__ void __launch_bounds__(256) dcn_reduce_splits_kernel(const float *part, float *out, long long n, int S)
+{
+    const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+    if (i >= n) return;
+    float s = part[i];
+    for (int k = 1; k < S; ++k) s = __fadd_rn(s, part[(long long)k * n + i]);
+    out[i] = s;
+}
+
+// grad_bias[o] = sum over (b, p) of grad_out[b][o][p]: per-thread strided sums, then a fixed reduction tree
+__global__ void __launch_bounds__(256) dcn_grad_bias_kernel(DcnArgs a)
+{
+    __shared__ float red[8];
+    const int o = blockIdx.x, P = a.Ho * a.Wo;
+    float s = 0.f;
+    for (int b = 0; b < a.B; ++b) {
+        const float *go = a.grad_out + ((long long)b * a.Co + o) * P;
+        for (int p = threadIdx.x; p < P; p += 256) s = __fadd_rn(s, __ldg(go + p));
+    }
+    for (int d = 16; d > 0; d >>= 1) s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, d));
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float t = red[0];
+        for (int w = 1; w < 8; ++w) t = __fadd_rn(t, red[w]);
+        a.grad_bias[o] = t;
+    }
+}
+
+size_t align256(size_t n) { return (n + 255) & ~size_t(255); }
+
+} // namespace
+
+DcnPlan dcn_plan(const DcnArgs &a, int chunk)
+{
+    DcnPlan pl;
+    const int T = a.kh * a.kw, Cg = a.C / a.dg;
+    const long long K = (long long)a.C * T, P = (long long)a.Ho * a.Wo, Q = (long long)a.B * P;
+    pl.chunk = chunk < 1 ? 1 : (chunk > a.B ? a.B : chunk);
+    pl.ntile_n = (long long)a.dg * T * ((Cg + BN - 1) / BN);
+    const long long tiles = pl.ntile_n * ((a.Co + BM - 1) / BM);
+    long long S = (GW_TARGET_CTAS + tiles - 1) / tiles;
+    const long long maxS = (Q + 4 * BK - 1) / (4 * BK);       // at least 4 BK-steps per split
+    S = S < 1 ? 1 : (S > maxS ? maxS : S);
+    if (S > 65535) S = 65535;
+    pl.span = ((Q + S - 1) / S + BK - 1) / BK * BK;
+    pl.splits = (int)((Q + pl.span - 1) / pl.span);
+    pl.cols_bytes = align256((size_t)pl.chunk * K * P * sizeof(float));
+    pl.part_bytes = pl.splits > 1 ? align256((size_t)pl.splits * a.Co * K * sizeof(float)) : 0;
+    return pl;
+}
+
+cudaError_t launch_dcn_forward(const DcnArgs &a, cudaStream_t st)
+{
+    const int P = a.Ho * a.Wo;
+    dim3 grid((P + BN - 1) / BN, (a.Co + BM - 1) / BM, a.B);
+    dcn_forward_kernel<<<grid, NT, 0, st>>>(a);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_dcn_backward(DcnArgs a, const DcnPlan &pl, void *workspace, cudaStream_t st)
+{
+    const int P = a.Ho * a.Wo, T = a.kh * a.kw;
+    const long long K = (long long)a.C * T;
+    a.cols = static_cast<float *>(workspace);
+    float *part = pl.splits > 1 ? reinterpret_cast<float *>(static_cast<char *>(workspace) + pl.cols_bytes) : a.grad_weight;
+    cudaError_t e = cudaMemsetAsync(a.grad_input, 0, (size_t)a.B * a.C * a.H * a.W * sizeof(float), st);
+    if (e != cudaSuccess) return e;
+    for (int b0 = 0; b0 < a.B; b0 += pl.chunk) {
+        const int nb = a.B - b0 < pl.chunk ? a.B - b0 : pl.chunk;
+        dcn_grad_cols_kernel<<<dim3((P + BN - 1) / BN, (unsigned)((K + BM - 1) / BM), nb), NT, 0, st>>>(a, b0);
+        dcn_grad_coord_kernel<<<dim3((P + 255) / 256, a.dg * T, nb), 256, 0, st>>>(a, b0);
+        dcn_grad_input_kernel<<<dim3((P + 255) / 256, a.dg * T, nb), 256, 0, st>>>(a, b0);
+    }
+    dcn_grad_weight_kernel<<<dim3((unsigned)pl.ntile_n, (a.Co + BM - 1) / BM, pl.splits), NT, 0, st>>>(a, pl.span, part);
+    if (pl.splits > 1) {
+        const long long n = (long long)a.Co * K;
+        dcn_reduce_splits_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(part, a.grad_weight, n, pl.splits);
+    }
+    dcn_grad_bias_kernel<<<a.Co, 256, 0, st>>>(a);
+    return cudaGetLastError();
+}
+
+} // namespace pvb

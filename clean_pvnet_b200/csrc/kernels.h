@@ -250,6 +250,27 @@ cudaError_t launch_vote_target(const VoteLossArgs &a, cudaStream_t st);
 cudaError_t launch_vote_loss_forward(const VoteLossArgs &a, cudaStream_t st);
 cudaError_t launch_vote_loss_backward(const VoteLossArgs &a, cudaStream_t st);
 
+// modulated deformable convolution, DCNv2 (dcn.cu).  Contiguous fp32 NCHW; shapes validated by the C ABI.
+struct DcnArgs {
+    const float *input;       // [B][C][H][W]
+    const float *offset;      // [B][dg*2*kh*kw][Ho][Wo]
+    const float *mask;        // [B][dg*kh*kw][Ho][Wo]
+    const float *weight;      // [Co][C][kh][kw]
+    const float *bias;        // [Co]
+    float *out;               // [B][Co][Ho][Wo] (forward)
+    const float *grad_out;    // [B][Co][Ho][Wo] (backward)
+    float *grad_input, *grad_offset, *grad_mask, *grad_weight, *grad_bias;   // shaped like their inputs (backward)
+    float *cols;              // grad_cols [chunk][C*kh*kw][Ho*Wo] (backward workspace)
+    int B, C, H, W, Co, kh, kw, sh, sw, ph, pw, dh, dw, dg, Ho, Wo;
+};
+// backward plan: images per grad_cols chunk, and grad_weight's split of the (image, pixel) reduction into `splits`
+// ranges of `span` pixels over `ntile_n` column tiles.  Workspace: cols_bytes of grad_cols, then part_bytes of
+// grad_weight partials (0 when splits == 1), each 256-byte aligned.  A function of the shapes only.
+struct DcnPlan { int chunk, splits; long long span, ntile_n; size_t cols_bytes, part_bytes; };
+DcnPlan dcn_plan(const DcnArgs &a, int chunk);
+cudaError_t launch_dcn_forward(const DcnArgs &a, cudaStream_t st);
+cudaError_t launch_dcn_backward(DcnArgs a, const DcnPlan &plan, void *workspace, cudaStream_t st);
+
 // twins of the reference extension on its own layouts
 cudaError_t launch_compat_generate(const float *direct, const float *coords, const int32_t *idxs, float *hyp,
                                    int tn, int vn, int hn, bool vanishing, cudaStream_t st);

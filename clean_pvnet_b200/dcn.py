@@ -1,0 +1,208 @@
+"""Twin of clean-pvnet's `lib/networks/dcn_v2.py:16-128` (the modulated deformable convolution, DCNv2, of the DLA-34
+CenterNet detector, lib/networks/ct/dla_dcn.py) on the device kernels of csrc/dcn.cu.
+
+    dcn_v2_conv(input, offset, mask, weight, bias, stride, padding, dilation, deformable_groups)
+                                      the autograd Function, same positional signature as the reference's
+    DCNv2(in, out, kernel_size, stride, padding, dilation=1, deformable_groups=1)
+    DCN(...)                          the same module, with its own conv_offset_mask (what dla_dcn.py builds)
+    install_dcn_as_reference_module() `from lib.networks.dcn_v2 import DCN` binds this module
+
+The reference's extension, lib/csrc/dcn_v2, is written against THC and does not build on current torch, so
+`import lib.networks.ct.dla_dcn` fails there; with install_dcn_as_reference_module() called first it imports and runs
+on these kernels, and net_utils.load_network loads a trained detector unchanged (same parameter names).  fp32 CUDA
+tensors only; there is no CPU implementation behind them.
+"""
+import ctypes
+import math
+import sys
+
+import torch
+from torch import nn
+from torch.autograd import Function
+from torch.autograd.function import once_differentiable
+from torch.nn.modules.utils import _pair
+
+from . import _lib
+
+# grad_cols, the backward's only stored column matrix ([chunk, C*kh*kw, Ho*Wo] fp32), is planned in image chunks of at
+# most this many bytes (one image always fits); the other outputs do not depend on the chunking.
+MAX_COLUMN_BYTES = 1 << 28
+
+
+def _desc(input, weight, stride, padding, dilation, deformable_groups):
+    d = _lib.PvbDcnDesc()
+    d.B, d.C, d.H, d.W = (int(s) for s in input.shape)
+    d.C_out, _, d.kh, d.kw = (int(s) for s in weight.shape)
+    d.stride_h, d.stride_w = _pair(stride)
+    d.pad_h, d.pad_w = _pair(padding)
+    d.dilation_h, d.dilation_w = _pair(dilation)
+    d.deformable_groups = int(deformable_groups)
+    return d
+
+
+def _out_hw(d):
+    ho = (d.H + 2 * d.pad_h - (d.dilation_h * (d.kh - 1) + 1)) // d.stride_h + 1
+    wo = (d.W + 2 * d.pad_w - (d.dilation_w * (d.kw - 1) + 1)) // d.stride_w + 1
+    return ho, wo
+
+
+def _check(input, offset, mask, weight, bias, d):
+    ts = dict(input=input, offset=offset, mask=mask, weight=weight, bias=bias)
+    for name, t in ts.items():
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise RuntimeError(f"dcn_v2_conv: {name} must be a CUDA tensor")
+        if t.dtype != torch.float32:
+            raise RuntimeError(f"dcn_v2_conv: {name} must be float32, got {t.dtype} (the kernels are fp32 only)")
+        if t.device != input.device:
+            raise RuntimeError(f"dcn_v2_conv: {name} is on {t.device}, input on {input.device}")
+    if input.dim() != 4 or weight.dim() != 4 or weight.shape[1] != input.shape[1]:
+        raise RuntimeError(f"dcn_v2_conv: input [B,C,H,W] and weight [C_out,C,kh,kw] do not match: "
+                           f"{list(input.shape)} and {list(weight.shape)}")
+    ho, wo = _out_hw(d)
+    t, dg = d.kh * d.kw, d.deformable_groups
+    want = dict(offset=[d.B, dg * 2 * t, ho, wo], mask=[d.B, dg * t, ho, wo], bias=[d.C_out])
+    for name, shape in want.items():
+        if list(ts[name].shape) != shape:
+            raise RuntimeError(f"dcn_v2_conv: {name} must be {shape}, got {list(ts[name].shape)}")
+
+
+def _call(entry, dev, *args):
+    args = [ctypes.c_void_p(a.data_ptr()) if isinstance(a, torch.Tensor) else a for a in args]
+    with torch.cuda.device(dev):
+        _lib.check(getattr(_lib.load(), entry)(*args, ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+
+
+def dcn_forward(input, offset, mask, weight, bias, stride, padding, dilation, deformable_groups):
+    """The forward of dcn_v2_conv without autograd: output [B,C_out,Ho,Wo] on input's device; no host sync."""
+    d = _desc(input, weight, stride, padding, dilation, deformable_groups)
+    _check(input, offset, mask, weight, bias, d)
+    ho, wo = _out_hw(d)
+    out = torch.empty((d.B, d.C_out, ho, wo), dtype=torch.float32, device=input.device)
+    if d.B:
+        c = [t.contiguous() for t in (input, offset, mask, weight, bias)]
+        _call("pvb_dcn_forward", input.device, ctypes.byref(d), *c, out)
+    return out
+
+
+def dcn_backward(input, offset, mask, weight, bias, grad_output, stride, padding, dilation, deformable_groups,
+                 max_column_bytes=None):
+    """(grad_input, grad_offset, grad_mask, grad_weight, grad_bias) of dcn_v2_conv for grad_output; no host sync.
+    grad_cols goes through a workspace of at most max_column_bytes (default MAX_COLUMN_BYTES) per image chunk."""
+    d = _desc(input, weight, stride, padding, dilation, deformable_groups)
+    _check(input, offset, mask, weight, bias, d)
+    ho, wo = _out_hw(d)
+    if list(grad_output.shape) != [d.B, d.C_out, ho, wo] or grad_output.dtype != torch.float32 or not grad_output.is_cuda:
+        raise RuntimeError(f"dcn_v2_conv: grad_output must be fp32 CUDA [{d.B},{d.C_out},{ho},{wo}], got "
+                           f"{grad_output.dtype} {list(grad_output.shape)}")
+    c = [t.contiguous() for t in (input, offset, mask, weight, grad_output)]
+    grads = [torch.empty_like(t) for t in (c[0], c[1], c[2], c[3])] + [torch.empty_like(bias)]
+    if d.B == 0:
+        for g in grads[3:]:
+            g.zero_()
+        return tuple(grads)
+    budget = MAX_COLUMN_BYTES if max_column_bytes is None else int(max_column_bytes)
+    per_image = d.C * d.kh * d.kw * ho * wo * 4
+    chunk = max(1, min(d.B, budget // max(per_image, 1)))
+    lib = _lib.load()
+    nbytes = lib.pvb_dcn_backward_workspace_bytes(ctypes.byref(d), chunk)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=input.device)
+    _call("pvb_dcn_backward", input.device, ctypes.byref(d), *c, *grads, chunk, ws, nbytes)
+    return tuple(grads)
+
+
+class _DCNv2(Function):
+    @staticmethod
+    def forward(ctx, input, offset, mask, weight, bias, stride, padding, dilation, deformable_groups):
+        ctx.stride = _pair(stride)
+        ctx.padding = _pair(padding)
+        ctx.dilation = _pair(dilation)
+        ctx.kernel_size = _pair(weight.shape[2:4])
+        ctx.deformable_groups = deformable_groups
+        output = dcn_forward(input, offset, mask, weight, bias, ctx.stride, ctx.padding, ctx.dilation,
+                             deformable_groups)
+        ctx.save_for_backward(input, offset, mask, weight, bias)
+        return output
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_output):
+        input, offset, mask, weight, bias = ctx.saved_tensors
+        grad_input, grad_offset, grad_mask, grad_weight, grad_bias = dcn_backward(
+            input, offset, mask, weight, bias, grad_output.contiguous(), ctx.stride, ctx.padding, ctx.dilation,
+            ctx.deformable_groups)
+        return grad_input, grad_offset, grad_mask, grad_weight, grad_bias, None, None, None, None
+
+
+dcn_v2_conv = _DCNv2.apply
+
+
+class DCNv2(nn.Module):
+    """lib/networks/dcn_v2.py:57-94: weight [out, in, kh, kw] ~ U(-1/sqrt(in*kh*kw), +), bias zero."""
+
+    def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation=1, deformable_groups=1):
+        super(DCNv2, self).__init__()
+        self.in_channels = in_channels
+        self.out_channels = out_channels
+        self.kernel_size = _pair(kernel_size)
+        self.stride = _pair(stride)
+        self.padding = _pair(padding)
+        self.dilation = _pair(dilation)
+        self.deformable_groups = deformable_groups
+
+        self.weight = nn.Parameter(torch.Tensor(out_channels, in_channels, *self.kernel_size))
+        self.bias = nn.Parameter(torch.Tensor(out_channels))
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        n = self.in_channels
+        for k in self.kernel_size:
+            n *= k
+        stdv = 1. / math.sqrt(n)
+        self.weight.data.uniform_(-stdv, stdv)
+        self.bias.data.zero_()
+
+    def forward(self, input, offset, mask):
+        assert 2 * self.deformable_groups * self.kernel_size[0] * self.kernel_size[1] == offset.shape[1]
+        assert self.deformable_groups * self.kernel_size[0] * self.kernel_size[1] == mask.shape[1]
+        return dcn_v2_conv(input, offset, mask, self.weight, self.bias, self.stride, self.padding, self.dilation,
+                           self.deformable_groups)
+
+
+class DCN(DCNv2):
+    """lib/networks/dcn_v2.py:97-128: DCNv2 whose offsets and mask come from its own conv_offset_mask (zero-initialised),
+    split as (o1, o2, mask) thirds, offset = cat(o1, o2), mask = sigmoid(mask)."""
+
+    def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation=1, deformable_groups=1):
+        super(DCN, self).__init__(in_channels, out_channels, kernel_size, stride, padding, dilation, deformable_groups)
+
+        channels_ = self.deformable_groups * 3 * self.kernel_size[0] * self.kernel_size[1]
+        self.conv_offset_mask = nn.Conv2d(self.in_channels, channels_, kernel_size=self.kernel_size,
+                                          stride=self.stride, padding=self.padding, bias=True)
+        self.init_offset()
+
+    def init_offset(self):
+        self.conv_offset_mask.weight.data.zero_()
+        self.conv_offset_mask.bias.data.zero_()
+
+    def forward(self, input):
+        out = self.conv_offset_mask(input)
+        o1, o2, mask = torch.chunk(out, 3, dim=1)
+        offset = torch.cat((o1, o2), dim=1)
+        mask = torch.sigmoid(mask)
+        return dcn_v2_conv(input, offset, mask, self.weight, self.bias, self.stride, self.padding, self.dilation,
+                           self.deformable_groups)
+
+
+def install_dcn_as_reference_module():
+    """Makes `from lib.networks.dcn_v2 import DCN` (lib/networks/ct/dla_dcn.py:16) bind this module, so the detector
+    imports and runs without the THC extension `lib.csrc.dcn_v2._ext` ever being built or imported.  Only the leaf
+    `lib.networks.dcn_v2` is replaced; `lib` and `lib.networks` stay the real packages whenever they import.
+
+    Call it BEFORE anything imports `lib.networks.ct*` (for the cascade: before install_crop_as_reference()).  Unlike
+    the other drop-ins it cannot be installed afterwards: without it that import fails on the extension.  Idempotent."""
+    from ._dropin import reference_package
+    this = sys.modules[__name__]
+    parent = reference_package("lib.networks")
+    sys.modules["lib.networks.dcn_v2"] = this
+    parent.dcn_v2 = this
+    return this

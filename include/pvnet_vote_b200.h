@@ -467,6 +467,44 @@ PVB_API int pvb_vote_loss_backward(const float *pred, const int64_t *pred_stride
                                    float *grad_pred, int32_t B, int32_t H, int32_t W, int32_t K, const void *workspace,
                                    size_t workspace_bytes, pvb_stream_t stream);
 
+/* ---- the detector: modulated deformable convolution, DCNv2 (DESIGN.md section 8h) -----------------------------------
+ * The DLA-34 CenterNet (lib/networks/ct/dla_dcn.py) runs its DCN layers through lib/csrc/dcn_v2, an extension written
+ * against THC that does not build on current torch.  Shapes: input [B,C,H,W], offset [B,dg*2*kh*kw,Ho,Wo] ((dy, dx) of
+ * tap (i, j) of group g at channels g*2*kh*kw + 2*(i*kw + j) and + 1), mask [B,dg*kh*kw,Ho,Wo], weight [C_out,C,kh,kw],
+ * bias [C_out], output [B,C_out,Ho,Wo], Ho = (H + 2*pad_h - (dilation_h*(kh - 1) + 1)) / stride_h + 1 (Wo alike); all
+ * device fp32, contiguous.  Channel c belongs to group c / (C / dg).  The sample point of output (ho, wo) at tap (i, j)
+ * is h = float(ho*stride_h - pad_h + i*dilation_h) + dy (w alike), used only when h > -1, w > -1, h < H, w < W; its
+ * bilinear value over the in-image corners times the mask is the column entry cols[c*kh*kw + i*kw + j][ho*Wo + wo].
+ * Requirements: B >= 0 (0 is a no-op), every other size >= 1 (pads >= 0), C % dg == 0, Ho, Wo >= 1, B <= 65535,
+ * H*W and Ho*Wo < 2^31, C*kh*kw <= 4194240, C_out <= 4194240, dg*kh*kw <= 65535.  No entry synchronises with the host
+ * or allocates.  A malformed descriptor or a NULL tensor returns PVB_ERR_INVALID, a missing, short or misaligned
+ * workspace PVB_ERR_WORKSPACE, both before any CUDA call. */
+typedef struct pvb_dcn_desc {
+    int32_t B, C, H, W, C_out, kh, kw;
+    int32_t stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w, deformable_groups;
+} pvb_dcn_desc;
+
+/* Replaces dcn_v2_cuda_forward (lib/csrc/dcn_v2/src/cuda/dcn_v2_cuda.cu:43): output = bias + weight . cols per image in
+ * one fused kernel that samples the columns into its operand tiles and never stores them.  The columns are the
+ * reference im2col kernel's bit for bit; the product is an fp32 FFMA sum starting from the bias.  The result is
+ * bit-identical run to run, and an image's output does not depend on the other images. */
+PVB_API int pvb_dcn_forward(const pvb_dcn_desc *d, const float *input, const float *offset, const float *mask,
+                            const float *weight, const float *bias, float *output, pvb_stream_t stream);
+
+/* Replaces dcn_v2_cuda_backward (dcn_v2_cuda.cu:206) for the whole batch: grad_cols = weight^T . grad_output goes to the
+ * workspace `chunk` images at a time (the only column matrix stored); grad_offset / grad_mask (the reference's
+ * col2im_coord: grad_mask = sum grad_col * value, grad_offset = sum d(value)/d(h, w) * grad_col * mask, 0 for a point
+ * with h <= -1, w <= -1, h >= H or w >= W, the cell [floor h, floor h + 1] at integer h) and grad_input (col2im, float
+ * atomics) per chunk; grad_weight = sum over the images of grad_output . cols^T with the columns re-sampled, in split
+ * partials added in a fixed order; grad_bias in a fixed order.  All five outputs are fully written (grad_input is
+ * zeroed by the call); every one but grad_input is bit-identical run to run.  workspace:
+ * pvb_dcn_backward_workspace_bytes(d, chunk) bytes of 256-byte aligned device memory; chunk is clamped to [1, B]. */
+PVB_API size_t pvb_dcn_backward_workspace_bytes(const pvb_dcn_desc *d, int32_t chunk);
+PVB_API int pvb_dcn_backward(const pvb_dcn_desc *d, const float *input, const float *offset, const float *mask,
+                             const float *weight, const float *grad_output, float *grad_input, float *grad_offset,
+                             float *grad_mask, float *grad_weight, float *grad_bias, int32_t chunk, void *workspace,
+                             size_t workspace_bytes, pvb_stream_t stream);
+
 /* Reads the sticky status word of a workspace (synchronises `stream`). */
 PVB_API int pvb_read_status(const pvb_desc *d, const void *workspace, pvb_stream_t stream);
 
