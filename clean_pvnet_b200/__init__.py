@@ -21,6 +21,9 @@ Public surface (same names/signatures as the reference):
     warp_affine_batch (cv2.warpAffine INTER_LINEAR for n rows), install_crop_as_reference (the cascade's crop)
     dcn.dcn_v2_conv / DCNv2 / DCN (twins of lib/networks/dcn_v2.py, the detector's deformable convolution, forward and
     backward), install_dcn_as_reference_module (call it before anything imports lib.networks.ct*)
+    ct_loss.ct_focal_loss (the CenterNet trainer's heatmap focal loss and its gradient from the boxes), ct_target_batch
+    (twin of the datasets' draw_umich_gaussian heatmap), ct_radius, CtNetworkWrapper (twin of lib/train/trainers/ct.py),
+    install_ct_loss_as_reference
 """
 from . import _lib  # noqa: F401
 from . import nn  # noqa: F401
@@ -43,6 +46,9 @@ from .crop import crop_inputs, uncrop_keypoints, warp_affine_batch, install_crop
 from . import dcn  # noqa: F401
 from .dcn import dcn_v2_conv, DCNv2, DCN, install_dcn_as_reference_module  # noqa: F401
 from .vote_loss import vote_loss, vote_target_batch, NetworkWrapper, install_vote_loss_as_reference  # noqa: F401
+from . import ct_loss  # noqa: F401
+from .ct_loss import (ct_focal_loss, ct_target_batch, ct_radius, CtNetworkWrapper,  # noqa: F401
+                      install_ct_loss_as_reference)
 from .ransac_voting_gpu import (  # noqa: F401
     estimate_voting_distribution_with_mean,
     ransac_voting_layer,
@@ -62,4 +68,5 @@ __all__ = [
     "render", "render_depth_batch", "vsd_batch", "install_depth_renderer_as_reference",
     "crop", "crop_inputs", "uncrop_keypoints", "warp_affine_batch", "install_crop_as_reference",
     "dcn", "dcn_v2_conv", "DCNv2", "DCN", "install_dcn_as_reference_module",
+    "ct_loss", "ct_focal_loss", "ct_target_batch", "ct_radius", "CtNetworkWrapper", "install_ct_loss_as_reference",
 ]

@@ -32,3 +32,28 @@ def reference_package(name):
             setattr(parent, parts[i - 1], mod)
         parent = mod
     return parent
+
+
+def chain_wrapper_factory(task, wrapper, marker):
+    """Patches lib.train.trainers.make_trainer._wrapper_factory to return wrapper(network) for cfg.task == task and to
+    call the factory it replaces for every other task.  make_trainer loads the trainer file by path (make_trainer.py:6-10),
+    so replacing a sys.modules entry would not reach it.  Each drop-in's factory carries its `marker` attribute and the
+    markers of the factories it chains to, so installing a drop-in again is a no-op whatever was installed in between."""
+    trainer = reference_package("lib.train.trainers.make_trainer")
+    original = getattr(trainer, "_wrapper_factory", None)
+    if getattr(original, marker, False):
+        return
+    if original is None:
+        def original(cfg, network):
+            raise RuntimeError(f"no trainer for task {cfg.task!r}: lib.train.trainers.make_trainer is not importable")
+
+    def _wrapper_factory(cfg, network):
+        if cfg.task == task:
+            return wrapper(network)
+        return original(cfg, network)
+
+    for name, value in vars(original).items():
+        if name.startswith("__pvb_"):
+            setattr(_wrapper_factory, name, value)
+    setattr(_wrapper_factory, marker, True)
+    trainer._wrapper_factory = _wrapper_factory

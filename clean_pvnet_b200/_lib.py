@@ -98,6 +98,12 @@ SIGNATURES = {
                                              _vp, _vp, _i32, _i32, _i32, _i32, _vp, _sz, _vp]),
     "pvb_vote_loss_backward": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int64), _vp, _i32, ctypes.POINTER(ctypes.c_int64),
                                               _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _sz, _vp]),
+    "pvb_ct_target": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "pvb_ct_loss_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32]),
+    "pvb_ct_loss_forward": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int64), _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32,
+                                           _i32, _i32, _vp, _sz, _vp]),
+    "pvb_ct_loss_backward": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int64), _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32,
+                                            _i32, _i32, _i32, _vp, _sz, _vp]),
     "pvb_dcn_forward": (ctypes.c_int, [ctypes.POINTER(PvbDcnDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "pvb_dcn_backward_workspace_bytes": (_sz, [ctypes.POINTER(PvbDcnDesc), _i32]),
     "pvb_dcn_backward": (ctypes.c_int, [ctypes.POINTER(PvbDcnDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,

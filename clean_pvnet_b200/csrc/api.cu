@@ -1085,6 +1085,112 @@ PVB_API int pvb_vote_loss_backward(const float *pred, const int64_t *pred_stride
     return e == cudaSuccess ? PVB_OK : cuda_fail(e, "vote loss backward kernel");
 }
 
+namespace {
+
+constexpr int CT_MAX_M = 1024;      // the tile's staged objects take at most 24 KB of shared memory
+
+// the arguments every CenterNet-loss entry shares; fills the object and size fields of `a`
+int ct_common(CtArgs &a, const int64_t *ct_ind, const int32_t *ct_radius, const int64_t *ct_cls, const float *ct_01,
+              int32_t B, int32_t M, int32_t C, int32_t H, int32_t W)
+{
+    if (B < 0 || M < 0 || C < 0 || H < 0 || W < 0)
+        return fail(PVB_ERR_INVALID, "negative size (B=%d M=%d C=%d H=%d W=%d)", B, M, C, H, W);
+    if (M > CT_MAX_M) return fail(PVB_ERR_INVALID, "M must be at most %d objects per image, got %d", CT_MAX_M, M);
+    if (B > 65535) return fail(PVB_ERR_INVALID, "B must be at most 65535, got %d", B);
+    if (C > 65535) return fail(PVB_ERR_INVALID, "C must be at most 65535, got %d", C);
+    if ((long long)H * W > 0x7fffffffll) return fail(PVB_ERR_INVALID, "image too large (H*W >= 2^31)");
+    if ((long long)B * M > 0 && (!ct_ind || !ct_radius || !ct_cls || !ct_01)) return fail(PVB_ERR_INVALID, "NULL tensor");
+    a = CtArgs{};
+    a.ct_ind = reinterpret_cast<const long long *>(ct_ind);
+    a.ct_radius = ct_radius;
+    a.ct_cls = reinterpret_cast<const long long *>(ct_cls);
+    a.ct_01 = ct_01;
+    a.B = B; a.M = M; a.C = C; a.H = H; a.W = W;
+    return PVB_OK;
+}
+
+int ct_logits(CtArgs &a, const float *logits, const int64_t *logit_stride)
+{
+    if (!logit_stride) return fail(PVB_ERR_INVALID, "NULL stride array");
+    for (int i = 0; i < 4; ++i) {
+        if (logit_stride[i] < 0) return fail(PVB_ERR_INVALID, "negative stride");
+        a.ls[i] = logit_stride[i];
+    }
+    if ((long long)a.B * a.C * a.H * a.W > 0 && !logits) return fail(PVB_ERR_INVALID, "NULL tensor");
+    a.logits = logits;
+    return PVB_OK;
+}
+
+// fills the workspace fields of `a` from a checked workspace
+int ct_workspace(CtArgs &a, const void *workspace, size_t workspace_bytes)
+{
+    size_t po = 0, no = 0, co = 0;
+    const size_t need = ct_loss_workspace_bytes(a.B, a.C, a.H, a.W, &po, &no, &co);
+    if (!workspace || workspace_bytes < need)
+        return fail(PVB_ERR_WORKSPACE, "workspace too small: need %zu bytes, got %zu", need, workspace ? workspace_bytes : 0);
+    if (reinterpret_cast<uintptr_t>(workspace) & 255u) return fail(PVB_ERR_WORKSPACE, "workspace must be 256-byte aligned");
+    char *ws = static_cast<char *>(const_cast<void *>(workspace));
+    a.num_pos = reinterpret_cast<long long *>(ws);
+    a.pos_part = reinterpret_cast<double *>(ws + po);
+    a.neg_part = reinterpret_cast<double *>(ws + no);
+    a.cnt_part = reinterpret_cast<int *>(ws + co);
+    return PVB_OK;
+}
+
+} // namespace
+
+// lib/datasets/tless*/ct.py ct_hm: data_utils.draw_umich_gaussian per object
+PVB_API int pvb_ct_target(const int64_t *ct_ind, const int32_t *ct_radius, const int64_t *ct_cls, const float *ct_01,
+                          float *ct_hm, int32_t B, int32_t M, int32_t C, int32_t H, int32_t W, pvb_stream_t stream)
+{
+    CtArgs a;
+    if (int rc = ct_common(a, ct_ind, ct_radius, ct_cls, ct_01, B, M, C, H, W)) return rc;
+    if ((long long)B * C * H * W > 0 && !ct_hm) return fail(PVB_ERR_INVALID, "NULL tensor");
+    a.out = ct_hm;
+    cudaError_t e = launch_ct_target(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "ct target kernel");
+}
+
+PVB_API size_t pvb_ct_loss_workspace_bytes(int32_t B, int32_t C, int32_t H, int32_t W)
+{
+    if (B < 0 || C < 0 || H < 0 || W < 0) return 0;
+    return ct_loss_workspace_bytes(B, C, H, W, nullptr, nullptr, nullptr);
+}
+
+// lib/train/trainers/ct.py:20-21, the forward pass
+PVB_API int pvb_ct_loss_forward(const float *logits, const int64_t *logit_stride, const int64_t *ct_ind,
+                                const int32_t *ct_radius, const int64_t *ct_cls, const float *ct_01, float *loss,
+                                int32_t B, int32_t M, int32_t C, int32_t H, int32_t W, void *workspace,
+                                size_t workspace_bytes, pvb_stream_t stream)
+{
+    CtArgs a;
+    if (int rc = ct_common(a, ct_ind, ct_radius, ct_cls, ct_01, B, M, C, H, W)) return rc;
+    if (int rc = ct_logits(a, logits, logit_stride)) return rc;
+    if (!loss) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (int rc = ct_workspace(a, workspace, workspace_bytes)) return rc;
+    a.loss = loss;
+    cudaError_t e = launch_ct_loss_forward(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "ct loss forward kernels");
+}
+
+// lib/train/trainers/ct.py:20-21, autograd's backward pass of it
+PVB_API int pvb_ct_loss_backward(const float *logits, const int64_t *logit_stride, const int64_t *ct_ind,
+                                 const int32_t *ct_radius, const int64_t *ct_cls, const float *ct_01,
+                                 const float *grad_loss, float *grad_logits, int32_t B, int32_t M, int32_t C, int32_t H,
+                                 int32_t W, const void *workspace, size_t workspace_bytes, pvb_stream_t stream)
+{
+    CtArgs a;
+    if (int rc = ct_common(a, ct_ind, ct_radius, ct_cls, ct_01, B, M, C, H, W)) return rc;
+    if (int rc = ct_logits(a, logits, logit_stride)) return rc;
+    if ((long long)B * C * H * W == 0) return PVB_OK;
+    if (!grad_loss || !grad_logits) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (int rc = ct_workspace(a, workspace, workspace_bytes)) return rc;
+    a.grad_loss = grad_loss;
+    a.out = grad_logits;
+    cudaError_t e = launch_ct_loss_backward(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "ct loss backward kernel");
+}
+
 PVB_API int pvb_read_status(const pvb_desc *d, const void *workspace, pvb_stream_t stream)
 {
     pvb_layout L;

@@ -250,6 +250,29 @@ cudaError_t launch_vote_target(const VoteLossArgs &a, cudaStream_t st);
 cudaError_t launch_vote_loss_forward(const VoteLossArgs &a, cudaStream_t st);
 cudaError_t launch_vote_loss_backward(const VoteLossArgs &a, cudaStream_t st);
 
+// The CenterNet heatmap target and focal loss (ct_loss.cu, DESIGN.md 8i), from the boxes.  One CTA per (32x16 pixel
+// tile, class, image); the image's objects of that class whose window meets the tile are staged in shared memory.
+struct CtArgs {
+    const float *logits;      // [B][C][H][W] at element strides ls (forward, backward)
+    long long ls[4];
+    const long long *ct_ind;  // [B][M] cy * W + cx
+    const int *ct_radius;     // [B][M]
+    const long long *ct_cls;  // [B][M]
+    const float *ct_01;       // [B][M] an object counts where ct_01 == 1
+    int B, M, C, H, W;
+    float *out;               // contiguous [B][C][H][W]: the target (target) or grad_logits (backward)
+    double *pos_part, *neg_part;   // [nparts] per-CTA fp64 sums of the pos and neg terms (forward)
+    int *cnt_part;            // [nparts] per-CTA counts of target == 1 (forward)
+    long long *num_pos;       // exact count of target == 1: written by the forward pass, read by the backward pass
+    float *loss;              // the scalar loss (forward)
+    const float *grad_loss;   // the scalar upstream gradient (backward)
+};
+// workspace: num_pos at offset 0, then the three partial arrays, each 256-byte aligned
+size_t ct_loss_workspace_bytes(int B, int C, int H, int W, size_t *pos_offset, size_t *neg_offset, size_t *cnt_offset);
+cudaError_t launch_ct_target(const CtArgs &a, cudaStream_t st);
+cudaError_t launch_ct_loss_forward(const CtArgs &a, cudaStream_t st);
+cudaError_t launch_ct_loss_backward(const CtArgs &a, cudaStream_t st);
+
 // modulated deformable convolution, DCNv2 (dcn.cu).  Contiguous fp32 NCHW; shapes validated by the C ABI.
 struct DcnArgs {
     const float *input;       // [B][C][H][W]

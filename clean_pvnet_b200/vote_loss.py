@@ -185,22 +185,9 @@ def install_vote_loss_as_reference():
       - lib.train.trainers.make_trainer._wrapper_factory: make_trainer loads the trainer file by path (make_trainer.py:6-10),
         so replacing a sys.modules entry would not reach it; the patched factory returns NetworkWrapper for
         cfg.task == 'pvnet' and calls the original for every other task.
-    Packages resolve through _dropin.reference_package, as for the other drop-ins.  Idempotent."""
-    from ._dropin import reference_package
+    Packages resolve through _dropin.reference_package, as for the other drop-ins.  Idempotent, and it coexists with
+    install_ct_loss_as_reference() in either order."""
+    from ._dropin import chain_wrapper_factory, reference_package
     data_utils = reference_package("lib.utils.pvnet.pvnet_data_utils")
     data_utils.compute_vertex = compact_vertex
-    trainer = reference_package("lib.train.trainers.make_trainer")
-    original = getattr(trainer, "_wrapper_factory", None)
-    if getattr(original, "__pvb_vote_loss__", False):
-        return
-    if original is None:
-        def original(cfg, network):
-            raise RuntimeError(f"no trainer for task {cfg.task!r}: lib.train.trainers.make_trainer is not importable")
-
-    def _wrapper_factory(cfg, network):
-        if cfg.task == 'pvnet':
-            return NetworkWrapper(network)
-        return original(cfg, network)
-
-    _wrapper_factory.__pvb_vote_loss__ = True
-    trainer._wrapper_factory = _wrapper_factory
+    chain_wrapper_factory('pvnet', NetworkWrapper, "__pvb_vote_loss__")

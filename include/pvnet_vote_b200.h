@@ -45,6 +45,12 @@
  *   utils/pvnet/pvnet_data_utils.py:30-44  compute_vertex          pvb_vote_target (B images per call)
  *   train/trainers/pvnet.py:25-27  vote loss                       pvb_vote_loss_forward / pvb_vote_loss_backward
  *
+ *   and the training side of the detector's heatmap:
+ *   datasets/tless{,_ag,_test}/ct.py ct_hm: utils/data_utils.py:36-64
+ *     gaussian2D + draw_umich_gaussian                             pvb_ct_target (B images per call)
+ *   train/trainers/ct.py:20-21 + utils/net_utils.py:9-39
+ *     FocalLoss(sigmoid(output['ct_hm']), ct_hm)                   pvb_ct_loss_forward / pvb_ct_loss_backward
+ *
  * Conventions
  *   - plain C: device pointers, sizes, strides (in ELEMENTS), a CUDA stream
  *     handle.  No torch types.  All work is enqueued on `stream`; no entry
@@ -466,6 +472,47 @@ PVB_API int pvb_vote_loss_backward(const float *pred, const int64_t *pred_stride
                                    const int64_t *mask_stride, const double *kpt_2d, const float *grad_loss,
                                    float *grad_pred, int32_t B, int32_t H, int32_t W, int32_t K, const void *workspace,
                                    size_t workspace_bytes, pvb_stream_t stream);
+
+/* ---- training the detector: CenterNet's heatmap target and focal loss from the boxes (DESIGN.md section 8i) -----------
+ * The CenterNet datasets (lib/datasets/{tless,tless_ag,tless_test}/ct.py) draw a dense [C,H,W] heatmap per sample with
+ * data_utils.draw_umich_gaussian; the trainer (lib/train/trainers/ct.py:20-21) takes net_utils.FocalLoss of
+ * net_utils.sigmoid(logits) against it.  These entries compute that target, and the loss and gradient that consume it,
+ * on the device from the objects.  Shared arguments, each device [B,M] contiguous:
+ *   ct_ind     int64, cy * W + cx of the object's centre
+ *   ct_radius  int32, r = max(0, int(gaussian_radius((ceil(h), ceil(w))))) from the sample's own float64 box size
+ *   ct_cls     int64, the object's class
+ *   ct_01      fp32, 1 for an object, anything else for padding
+ * An object counts where ct_01 == 1, 0 <= ct_cls < C, 0 <= ct_ind < H*W and r >= 0; any other values match nothing.
+ * The target at (b, c, y, x) is the maximum over the counting objects of class c with |x - cx| <= r and |y - cy| <= r of
+ * float32(gaussian2D's fp64 value at (x - cx, y - cy)), 0 where none qualifies: draw_umich_gaussian's ct_hm bit for bit.
+ * Requirements: B <= 65535, C <= 65535, 0 <= M <= 1024, H*W < 2^31.  Bad arguments (negative sizes, those limits, NULL
+ * pointers or stride arrays, negative strides) return PVB_ERR_INVALID, a missing, short or misaligned workspace
+ * PVB_ERR_WORKSPACE, both before any CUDA call.  No entry synchronises with the host. */
+
+/* data_utils.draw_umich_gaussian over a batch's objects: ct_hm device fp32 [B,C,H,W] contiguous, fully written.
+ * B, C, H or W == 0 is a no-op. */
+PVB_API int pvb_ct_target(const int64_t *ct_ind, const int32_t *ct_radius, const int64_t *ct_cls, const float *ct_01,
+                          float *ct_hm, int32_t B, int32_t M, int32_t C, int32_t H, int32_t W, pvb_stream_t stream);
+
+/* The focal loss of lib/train/trainers/ct.py:20-21 with batch['ct_hm'] = that target, never built:
+ *   pred = clamp(sigmoid(logits), 1e-4, 1 - 1e-4);  pos = sum log(pred) (1 - pred)^2 [t == 1];
+ *   neg = sum log(1 - pred) pred^2 (1 - t)^4 [t < 1];  loss = -neg if num_pos == 0 else -(pos + neg) / num_pos
+ * logits device fp32 [B,C,H,W] at element strides logit_stride (HOST int64[4]).  Each term is CUDA torch's fp32 value;
+ * the two sums are fp64, added in a fixed order and rounded once, so the loss is reproducible bit for bit; num_pos is
+ * exact.  loss: device fp32 scalar.  workspace: pvb_ct_loss_workspace_bytes(B, C, H, W) bytes of 256-byte aligned device
+ * memory; it keeps num_pos for pvb_ct_loss_backward, so pass the same workspace to both. */
+PVB_API size_t pvb_ct_loss_workspace_bytes(int32_t B, int32_t C, int32_t H, int32_t W);
+PVB_API int pvb_ct_loss_forward(const float *logits, const int64_t *logit_stride, const int64_t *ct_ind,
+                                const int32_t *ct_radius, const int64_t *ct_cls, const float *ct_01, float *loss,
+                                int32_t B, int32_t M, int32_t C, int32_t H, int32_t W, void *workspace,
+                                size_t workspace_bytes, pvb_stream_t stream);
+/* autograd's gradient of that loss with respect to the logits, bit for bit: grad_loss is the device fp32 upstream
+ * gradient (read on the device, never by the host), grad_logits device fp32 [B,C,H,W] contiguous, fully written.  The
+ * workspace is the forward call's, after it.  B, C, H or W == 0 is a no-op. */
+PVB_API int pvb_ct_loss_backward(const float *logits, const int64_t *logit_stride, const int64_t *ct_ind,
+                                 const int32_t *ct_radius, const int64_t *ct_cls, const float *ct_01,
+                                 const float *grad_loss, float *grad_logits, int32_t B, int32_t M, int32_t C, int32_t H,
+                                 int32_t W, const void *workspace, size_t workspace_bytes, pvb_stream_t stream);
 
 /* ---- the detector: modulated deformable convolution, DCNv2 (DESIGN.md section 8h) -----------------------------------
  * The DLA-34 CenterNet (lib/networks/ct/dla_dcn.py) runs its DCN layers through lib/csrc/dcn_v2, an extension written
