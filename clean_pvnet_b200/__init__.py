@@ -24,6 +24,8 @@ Public surface (same names/signatures as the reference):
     ct_loss.ct_focal_loss (the CenterNet trainer's heatmap focal loss and its gradient from the boxes), ct_target_batch
     (twin of the datasets' draw_umich_gaussian heatmap), ct_radius, CtNetworkWrapper (twin of lib/train/trainers/ct.py),
     install_ct_loss_as_reference
+    ct_decode.decode_detections (twin of lib/networks/ct/dla.py's Network.decode_detection for B images),
+    detection_boxes (the consumers' un-crop of the boxes to the image), install_ct_decode_as_reference
 """
 from . import _lib  # noqa: F401
 from . import nn  # noqa: F401
@@ -49,6 +51,8 @@ from .vote_loss import vote_loss, vote_target_batch, NetworkWrapper, install_vot
 from . import ct_loss  # noqa: F401
 from .ct_loss import (ct_focal_loss, ct_target_batch, ct_radius, CtNetworkWrapper,  # noqa: F401
                       install_ct_loss_as_reference)
+from . import ct_decode  # noqa: F401
+from .ct_decode import decode_detections, detection_boxes, install_ct_decode_as_reference  # noqa: F401
 from .ransac_voting_gpu import (  # noqa: F401
     estimate_voting_distribution_with_mean,
     ransac_voting_layer,
@@ -69,4 +73,5 @@ __all__ = [
     "crop", "crop_inputs", "uncrop_keypoints", "warp_affine_batch", "install_crop_as_reference",
     "dcn", "dcn_v2_conv", "DCNv2", "DCN", "install_dcn_as_reference_module",
     "ct_loss", "ct_focal_loss", "ct_target_batch", "ct_radius", "CtNetworkWrapper", "install_ct_loss_as_reference",
+    "ct_decode", "decode_detections", "detection_boxes", "install_ct_decode_as_reference",
 ]

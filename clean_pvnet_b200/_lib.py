@@ -104,6 +104,9 @@ SIGNATURES = {
                                            _i32, _i32, _vp, _sz, _vp]),
     "pvb_ct_loss_backward": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int64), _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32,
                                             _i32, _i32, _i32, _vp, _sz, _vp]),
+    "pvb_ct_decode_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32, _i32]),
+    "pvb_ct_decode": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int64), _vp, ctypes.POINTER(ctypes.c_int64), _i32, _i32,
+                                     _i32, _i32, _i32, _i32, _vp, _vp, _vp, _sz, _vp]),
     "pvb_dcn_forward": (ctypes.c_int, [ctypes.POINTER(PvbDcnDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "pvb_dcn_backward_workspace_bytes": (_sz, [ctypes.POINTER(PvbDcnDesc), _i32]),
     "pvb_dcn_backward": (ctypes.c_int, [ctypes.POINTER(PvbDcnDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,

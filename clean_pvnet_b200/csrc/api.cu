@@ -1191,6 +1191,60 @@ PVB_API int pvb_ct_loss_backward(const float *logits, const int64_t *logit_strid
     return e == cudaSuccess ? PVB_OK : cuda_fail(e, "ct loss backward kernel");
 }
 
+namespace {
+
+// the sizes pvb_ct_decode accepts (the limits keep every index exact in fp32 and every key unique)
+int ct_decode_sizes(int32_t B, int32_t C, int32_t H, int32_t W, int32_t K)
+{
+    if (B < 0 || B > 65535) return fail(PVB_ERR_INVALID, "B must be in [0, 65535], got %d", B);
+    if (C < 1 || C > 65535 || H < 1 || W < 1)
+        return fail(PVB_ERR_INVALID, "C, H and W must be >= 1 and C <= 65535 (got C=%d H=%d W=%d)", C, H, W);
+    const long long HW = (long long)H * W;
+    if (HW >= (1ll << 24)) return fail(PVB_ERR_INVALID, "H*W must be < 2^24, got %lld", HW);
+    if (K < 1 || K > HW) return fail(PVB_ERR_INVALID, "K must be in [1, H*W = %lld], got %d", HW, K);
+    if ((long long)C * K >= (1ll << 24)) return fail(PVB_ERR_INVALID, "C*K must be < 2^24, got %lld", (long long)C * K);
+    if ((long long)C * HW >= (1ll << 31)) return fail(PVB_ERR_INVALID, "C*H*W must be < 2^31, got %lld", (long long)C * HW);
+    return PVB_OK;
+}
+
+} // namespace
+
+PVB_API size_t pvb_ct_decode_workspace_bytes(int32_t B, int32_t C, int32_t H, int32_t W, int32_t K)
+{
+    if (B < 0 || C < 0 || H < 0 || W < 0 || K < 0) return 0;
+    return ct_decode_workspace_bytes(B, C, H, W, K, nullptr);
+}
+
+// lib/networks/ct/dla.py:20-26 Network.decode_detection: sigmoid, ct_decode.decode_ct_hm, data_utils.clip_to_image
+PVB_API int pvb_ct_decode(const float *ct_hm, const int64_t *hm_stride, const float *wh, const int64_t *wh_stride,
+                          int32_t B, int32_t C, int32_t H, int32_t W, int32_t K, int32_t clip, float *ct,
+                          float *detection, void *workspace, size_t workspace_bytes, pvb_stream_t stream)
+{
+    if (int rc = ct_decode_sizes(B, C, H, W, K)) return rc;
+    if (clip != 0 && clip != 1) return fail(PVB_ERR_INVALID, "clip must be 0 or 1 (got %d)", clip);
+    if (!hm_stride || !wh_stride) return fail(PVB_ERR_INVALID, "NULL stride array");
+    CtDecodeArgs a = {};
+    for (int i = 0; i < 4; ++i) {
+        if (hm_stride[i] < 0 || wh_stride[i] < 0) return fail(PVB_ERR_INVALID, "negative stride");
+        a.hs[i] = hm_stride[i];
+        a.ws[i] = wh_stride[i];
+    }
+    if (B == 0) return PVB_OK;
+    if (!ct_hm || !wh || !ct || !detection) return fail(PVB_ERR_INVALID, "NULL tensor");
+    size_t so = 0;
+    const size_t need = ct_decode_workspace_bytes(B, C, H, W, K, &so);
+    if (!workspace || workspace_bytes < need)
+        return fail(PVB_ERR_WORKSPACE, "workspace too small: need %zu bytes, got %zu", need, workspace ? workspace_bytes : 0);
+    if (reinterpret_cast<uintptr_t>(workspace) & 255u) return fail(PVB_ERR_WORKSPACE, "workspace must be 256-byte aligned");
+    char *ws = static_cast<char *>(workspace);
+    a.hm = ct_hm; a.wh = wh; a.B = B; a.C = C; a.H = H; a.W = W; a.K = K; a.clip = clip;
+    a.lists = reinterpret_cast<unsigned long long *>(ws);
+    a.sel = reinterpret_cast<unsigned long long *>(ws + so);
+    a.ct = ct; a.det = detection;
+    cudaError_t e = launch_ct_decode(a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "ct decode kernels");
+}
+
 PVB_API int pvb_read_status(const pvb_desc *d, const void *workspace, pvb_stream_t stream)
 {
     pvb_layout L;

@@ -110,6 +110,10 @@ __device__ __forceinline__ bool vote_exact(float vx, float vy, float cx, float c
 // (float(1e-6) = 0x358637BD = 9.99999997e-07 < 1e-6 < next float).
 __device__ __forceinline__ float below_1e6() { return __int_as_float(0x358637BD); }
 
+// CUDA torch's fp32 sigmoid, 1 / (1 + exp(-x)), bit for bit (pinned against autograd in DESIGN.md 8i); the CenterNet
+// loss (ct_loss.cu) and decode (ct_decode.cu) both use it.  NaN stays NaN, -inf gives +0, +inf gives 1.
+__device__ __forceinline__ float ct_sigmoid(float x) { return __fdiv_rn(1.f, __fadd_rn(1.f, expf(-x))); }
+
 __device__ __forceinline__ float warp_sum(float v)
 {
 #pragma unroll

@@ -75,8 +75,7 @@ __device__ __forceinline__ float ct_target(const CtObj *s_obj, int n, int x, int
     return t;
 }
 
-// net_utils.sigmoid: torch's sigmoid (1 / (1 + exp(-x)) in fp32) clamped to [1e-4, 1 - 1e-4], NaN propagated
-__device__ __forceinline__ float ct_sigmoid(float x) { return __fdiv_rn(1.f, __fadd_rn(1.f, expf(-x))); }
+// net_utils.sigmoid: torch's sigmoid (ct_sigmoid, common.cuh) clamped to [1e-4, 1 - 1e-4], NaN propagated
 __device__ __forceinline__ float ct_clamp(float s) { return isnan(s) ? s : fminf(fmaxf(s, CT_LO), CT_HI); }
 
 struct CtTerms { float pos, neg; };

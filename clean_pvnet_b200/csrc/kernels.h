@@ -273,6 +273,24 @@ cudaError_t launch_ct_target(const CtArgs &a, cudaStream_t st);
 cudaError_t launch_ct_loss_forward(const CtArgs &a, cudaStream_t st);
 cudaError_t launch_ct_loss_backward(const CtArgs &a, cudaStream_t st);
 
+// The CenterNet decode (ct_decode.cu, DESIGN.md 8j): sigmoid, 3x3 peak test and top-K per image, then the boxes.
+struct CtDecodeArgs {
+    const float *hm;          // [B][C][H][W] logits at element strides hs
+    long long hs[4];
+    const float *wh;          // [B][2][H][W] at element strides ws
+    long long ws[4];
+    int B, C, H, W, K, clip;
+    int T, Lk;                // tiles per class and entries per list (set by launch_ct_decode)
+    long long L;              // lists per image, C * T
+    unsigned long long *lists;   // workspace [B][L][Lk]: each tile's largest keys, descending
+    unsigned long long *sel;     // workspace [B][K]: the image's K selected keys, unordered
+    float *ct;                // [B][K][2] (xs, ys)
+    float *det;               // [B][K][6] (x0, y0, x1, y1, score, class)
+};
+// workspace: the lists at offset 0, then sel, 256-byte aligned
+size_t ct_decode_workspace_bytes(int B, int C, int H, int W, int K, size_t *sel_offset);
+cudaError_t launch_ct_decode(CtDecodeArgs a, cudaStream_t st);
+
 // modulated deformable convolution, DCNv2 (dcn.cu).  Contiguous fp32 NCHW; shapes validated by the C ABI.
 struct DcnArgs {
     const float *input;       // [B][C][H][W]

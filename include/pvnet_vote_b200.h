@@ -51,6 +51,10 @@
  *   train/trainers/ct.py:20-21 + utils/net_utils.py:9-39
  *     FocalLoss(sigmoid(output['ct_hm']), ct_hm)                   pvb_ct_loss_forward / pvb_ct_loss_backward
  *
+ *   and the detector's decode at inference:
+ *   networks/ct/dla.py:20-26  decode_detection: sigmoid +
+ *     utils/ct/ct_decode.py:6-75 decode_ct_hm + clip_to_image     pvb_ct_decode (B images per call)
+ *
  * Conventions
  *   - plain C: device pointers, sizes, strides (in ELEMENTS), a CUDA stream
  *     handle.  No torch types.  All work is enqueued on `stream`; no entry
@@ -513,6 +517,26 @@ PVB_API int pvb_ct_loss_backward(const float *logits, const int64_t *logit_strid
                                  const int32_t *ct_radius, const int64_t *ct_cls, const float *ct_01,
                                  const float *grad_loss, float *grad_logits, int32_t B, int32_t M, int32_t C, int32_t H,
                                  int32_t W, const void *workspace, size_t workspace_bytes, pvb_stream_t stream);
+
+/* ---- the detector's decode: from the output maps to the boxes (DESIGN.md section 8j) --------------------------------
+ * Replaces Network.decode_detection (lib/networks/ct/dla.py:20-26): torch.sigmoid, ct_decode.decode_ct_hm
+ * (lib/utils/ct/ct_decode.py:6-75) and, with clip = 1, data_utils.clip_to_image (lib/utils/data_utils.py:373-377), for
+ * B images.  ct_hm: device fp32 logits [B,C,H,W] at element strides hm_stride (HOST int64[4]); wh: device fp32 [B,2,H,W]
+ * at wh_stride.  Per image: heat = sigmoid(logit) in CUDA torch's fp32; a pixel keeps heat where the 3x3 max_pool2d of
+ * heat (padding never wins, a NaN in the window wins) equals it and becomes heat * 0 elsewhere; the K largest of the
+ * C*H*W values under (value descending, NaN above +inf, class ascending, pixel index ascending) are, in that order,
+ *   ct[b][k] = (xs, ys) = (i mod W, i div W);  detection[b][k] = (xs - w/2, ys - h/2, xs + w/2, ys + h/2, value, class)
+ * with (w, h) = wh[b, :, ys, xs] and each operation rounded once in fp32; clip = 1 clamps x0, y0 to >= 0, x1 to <= W-1
+ * and y1 to <= H-1 (NaN passes).  ct device fp32 [B,K,2] and detection device fp32 [B,K,6], contiguous, fully written.
+ * Requirements: 0 <= B <= 65535, 1 <= C <= 65535, H*W < 2^24, 1 <= K <= H*W, C*K < 2^24, C*H*W < 2^31.  workspace:
+ * pvb_ct_decode_workspace_bytes(B, C, H, W, K) bytes of 256-byte aligned device memory.  Bad arguments return
+ * PVB_ERR_INVALID, a missing, short or misaligned workspace PVB_ERR_WORKSPACE, both before any CUDA call.  The result is
+ * bit-identical run to run, an image's result does not depend on the other images, and nothing synchronises with the
+ * host.  B == 0 is a no-op. */
+PVB_API size_t pvb_ct_decode_workspace_bytes(int32_t B, int32_t C, int32_t H, int32_t W, int32_t K);
+PVB_API int pvb_ct_decode(const float *ct_hm, const int64_t *hm_stride, const float *wh, const int64_t *wh_stride,
+                          int32_t B, int32_t C, int32_t H, int32_t W, int32_t K, int32_t clip, float *ct,
+                          float *detection, void *workspace, size_t workspace_bytes, pvb_stream_t stream);
 
 /* ---- the detector: modulated deformable convolution, DCNv2 (DESIGN.md section 8h) -----------------------------------
  * The DLA-34 CenterNet (lib/networks/ct/dla_dcn.py) runs its DCN layers through lib/csrc/dcn_v2, an extension written
