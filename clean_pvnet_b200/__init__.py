@@ -16,7 +16,9 @@ Public surface (same names/signatures as the reference):
     of lib/utils/pvnet/pvnet_data_utils.py's compute_vertex), NetworkWrapper (twin of lib/train/trainers/pvnet.py),
     install_vote_loss_as_reference
     render.render_depth_batch (the depth image the T-LESS evaluator's OpenGL DepthRender renders, n poses per launch),
-    vsd_batch (T-LESS's VSD error for n pose pairs), install_depth_renderer_as_reference
+    vsd_batch (T-LESS's VSD error for n pose pairs), install_depth_renderer_as_reference, instance_masks_batch /
+    instance_masks_from_depth (T-LESS's instance label maps, pixel counts and boxes for B images),
+    install_tless_renderer_as_reference
     crop.crop_inputs (T-LESS's PVNet crop, pvnet_transform, for n boxes), uncrop_keypoints (the evaluator's un-crop),
     warp_affine_batch (cv2.warpAffine INTER_LINEAR for n rows), install_crop_as_reference (the cascade's crop)
     dcn.dcn_v2_conv / DCNv2 / DCN (twins of lib/networks/dcn_v2.py, the detector's deformable convolution, forward and
@@ -43,6 +45,7 @@ from . import pose  # noqa: F401
 from .pose import pnp_batch  # noqa: F401
 from . import render  # noqa: F401
 from .render import render_depth_batch, vsd_batch, install_depth_renderer_as_reference  # noqa: F401
+from .render import instance_masks_batch, instance_masks_from_depth, install_tless_renderer_as_reference  # noqa: F401
 from . import crop  # noqa: F401
 from .crop import crop_inputs, uncrop_keypoints, warp_affine_batch, install_crop_as_reference  # noqa: F401
 from . import dcn  # noqa: F401
@@ -70,6 +73,7 @@ __all__ = [
     "metrics", "pose_metrics_batch", "mask_iou_batch", "linemod_scores",
     "vote_loss", "vote_target_batch", "NetworkWrapper", "install_vote_loss_as_reference",
     "render", "render_depth_batch", "vsd_batch", "install_depth_renderer_as_reference",
+    "instance_masks_batch", "instance_masks_from_depth", "install_tless_renderer_as_reference",
     "crop", "crop_inputs", "uncrop_keypoints", "warp_affine_batch", "install_crop_as_reference",
     "dcn", "dcn_v2_conv", "DCNv2", "DCN", "install_dcn_as_reference_module",
     "ct_loss", "ct_focal_loss", "ct_target_batch", "ct_radius", "CtNetworkWrapper", "install_ct_loss_as_reference",

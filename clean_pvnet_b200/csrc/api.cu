@@ -901,6 +901,57 @@ PVB_API int pvb_vsd(const float *depth_test, int32_t B, const float *depth_est, 
     return err == cudaSuccess ? PVB_OK : cuda_fail(err, "vsd kernels");
 }
 
+PVB_API size_t pvb_instance_masks_workspace_bytes(int32_t B, int32_t m)
+{
+    if (B <= 0 || m <= 0) return 0;
+    return instance_masks_workspace_bytes(B, m);
+}
+
+PVB_API int pvb_instance_masks(const float *depth, int32_t n_depth, const int32_t *slot, const int32_t *obj_id, int32_t n,
+                               const int32_t *image_first, int32_t B, int32_t H, int32_t W, int16_t *label,
+                               int64_t *a_pixel_num, int64_t *pixel_num, int32_t *bbox, void *workspace,
+                               size_t workspace_bytes, pvb_stream_t stream)
+{
+    if (n_depth < 0 || n < 0 || B < 0 || H < 0 || W < 0)
+        return fail(PVB_ERR_INVALID, "negative size (n_depth=%d n=%d B=%d H=%d W=%d)", n_depth, n, B, H, W);
+    if ((long long)H * W > 0x7fffffffll) return fail(PVB_ERR_INVALID, "image too large (H*W >= 2^31)");
+    if (B > 65535) return fail(PVB_ERR_INVALID, "B must be <= 65535 (got %d)", B);
+    if (B == 0) return PVB_OK;
+    if (!image_first || !slot || !obj_id) return fail(PVB_ERR_INVALID, "NULL host table");
+    const bool px = (long long)H * W > 0;
+    if (!a_pixel_num || !pixel_num || !bbox || (px && (!depth || !label))) return fail(PVB_ERR_INVALID, "NULL tensor");
+    const int32_t i0 = image_first[0];
+    if (i0 < 0) return fail(PVB_ERR_INVALID, "image 0's instances start at %d", i0);
+    int max_m = 0;
+    for (int32_t b = 0; b < B; ++b) {
+        const int32_t lo = image_first[b], hi = image_first[b + 1];
+        if (hi <= lo || hi > n)
+            return fail(PVB_ERR_INVALID, "image %d's instance range [%d, %d) is empty or outside [0, %d)", b, lo, hi, n);
+        if (hi - lo > MASK_MAX_INSTANCES)
+            return fail(PVB_ERR_INVALID, "image %d has %d instances (at most %d)", b, hi - lo, MASK_MAX_INSTANCES);
+        max_m = std::max(max_m, hi - lo);
+    }
+    const int32_t m = image_first[B] - i0;
+    std::vector<int32_t> table((size_t)B + 1 + 2 * (size_t)m);
+    for (int32_t b = 0; b <= B; ++b) table[b] = image_first[b] - i0;
+    for (int32_t b = 0; b < B; ++b)
+        for (int32_t i = image_first[b]; i < image_first[b + 1]; ++i) {
+            if (slot[i] < 0 || slot[i] >= n_depth)
+                return fail(PVB_ERR_INVALID, "instance %d reads depth slot %d (outside [0, %d))", i, slot[i], n_depth);
+            const long long lab = (long long)obj_id[i] * 1000 + (i - image_first[b]);
+            if (lab < -32768 || lab > 32767)
+                return fail(PVB_ERR_INVALID, "instance %d's label %lld (obj_id * 1000 + instance_id) does not fit int16", i, lab);
+            table[B + 1 + (i - i0)] = slot[i];
+            table[B + 1 + m + (i - i0)] = (int32_t)lab;
+        }
+    if (int rc = nn_check_workspace(instance_masks_workspace_bytes(B, m), workspace, workspace_bytes)) return rc;
+    cudaError_t e = launch_instance_masks(depth, table.data(), B, m, max_m, H, W, reinterpret_cast<short *>(label),
+                                          reinterpret_cast<long long *>(a_pixel_num) + i0,
+                                          reinterpret_cast<long long *>(pixel_num) + i0, bbox + 4ll * i0, workspace,
+                                          static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "instance mask kernels");
+}
+
 namespace {
 
 // the image and output arguments the crop and the warp share; fills the image and size fields of `a`

@@ -192,6 +192,15 @@ struct VsdArgs {
 // workspace: the integer counts of the n rows
 size_t vsd_workspace_bytes(int n);
 cudaError_t launch_vsd(const VsdArgs &a, void *workspace, cudaStream_t st);
+// T-LESS's instance masks (render.cu, DESIGN.md 8k).  table: HOST int32 [B + 1 + 2m], image b's instances are
+// [table[b], table[b+1]) (table[0] == 0), then the depth slot of each of the m instances, then its label.  Writes
+// label [B][H][W] int16 and a_out / p_out [m] int64, box_out [m][4] int32 (x, y, w, h).  max_m: the most instances
+// of one image (<= MASK_MAX_INSTANCES).  Workspace: the table, then the integer sums of the m instances.
+constexpr int MASK_MAX_INSTANCES = 2048;
+size_t instance_masks_workspace_bytes(int B, int m);
+cudaError_t launch_instance_masks(const float *depth, const int *table, int B, int m, int max_m, int H, int W,
+                                  short *label, long long *a_out, long long *p_out, int *box_out, void *workspace,
+                                  cudaStream_t st);
 
 // T-LESS's PVNet crop (crop.cu, DESIGN.md 8g).  Setup: one thread per box -> centre, scale, forward (and inverse) crop
 // matrix.  Warp: one CTA per (box, output row) over [n][out_h]; the crop variant masks, normalises and writes NCHW fp32.

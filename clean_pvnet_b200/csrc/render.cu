@@ -317,6 +317,114 @@ __global__ void vsd_final_kernel(VsdArgs a, const VsdCounts *__restrict__ counts
     a.e[i] = c.uni ? __ddiv_rn((double)(c.cost + (c.uni - c.inter)), (double)c.uni) : 1.0;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// T-LESS's instance masks (DESIGN.md 8k): handle_test_data.update_mask over an image's instances, in order, on the
+// depth opengl_renderer.render returns (the mm depth / 1000 in fp32):
+//   key = fp32(d / 1000);  the instance takes the pixel when key != 0 and key < depth_map (which starts at 10.0f), so
+//   ties go to the earlier instance and a key of 10 or more (or NaN) never takes it
+//   label = obj_id * 1000 + instance_id (int16, 0 where no instance took the pixel)
+//   a_pixel_num = #(key != 0), pixel_num = #(label pixels of the instance), box = cv2.boundingRect of those pixels
+// One CTA per (MASK_PIXELS pixels, image) keeps its pixels' running key and winner in registers over the image's
+// instances; the counts and box extremes go through warp reductions and shared atomics, then one global atomic per
+// instance and CTA.  Every sum is an integer, so the result is exact and independent of the order of the atomics.
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int MASK_THREADS = 256;
+constexpr int MASK_PPT = 8;                            // pixels per thread
+constexpr int MASK_PIXELS = MASK_THREADS * MASK_PPT;
+
+// per-instance sums; the box is kept as maxima of W - x, x + 1, H - y, y + 1, which are all 0 for an empty mask, so the
+// sums start from a zero fill
+struct MaskAcc { unsigned a, p, x0, x1, y0, y1; };
+
+__global__ void __launch_bounds__(MASK_THREADS)
+mask_compose_kernel(const float *__restrict__ depth, const int *__restrict__ table, int B, int m, int H, int W,
+                    short *__restrict__ label, MaskAcc *__restrict__ acc)
+{
+    extern __shared__ unsigned s_acc[];                // [instances of this image][6], a MaskAcc each
+    const int b = blockIdx.y;
+    const int i0 = __ldg(table + b), mi = __ldg(table + b + 1) - i0;
+    const int *slot = table + B + 1 + i0, *lab = table + B + 1 + m + i0;
+    const int HW = H * W;
+    for (int k = threadIdx.x; k < 6 * mi; k += MASK_THREADS) s_acc[k] = 0u;
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    const int p0 = blockIdx.x * MASK_PIXELS + threadIdx.x;
+    float key[MASK_PPT];
+    int win[MASK_PPT];
+#pragma unroll
+    for (int q = 0; q < MASK_PPT; ++q) { key[q] = 10.0f; win[q] = -1; }
+    for (int j = 0; j < mi; ++j) {
+        const float *d = depth + (long long)__ldg(slot + j) * HW;
+        unsigned nz = 0;
+#pragma unroll
+        for (int q = 0; q < MASK_PPT; ++q) {
+            const int p = p0 + q * MASK_THREADS;
+            if (p < HW) {
+                const float k = __fdiv_rn(__ldg(d + p), 1000.0f);
+                if (k != 0.0f) {
+                    ++nz;
+                    if (k < key[q]) { key[q] = k; win[q] = j; }
+                }
+            }
+        }
+        nz = __reduce_add_sync(0xffffffffu, nz);
+        if (lane == 0 && nz) atomicAdd(&s_acc[6 * j], nz);
+    }
+    short *out = label + (long long)b * HW;
+    int px[MASK_PPT], py[MASK_PPT];
+#pragma unroll
+    for (int q = 0; q < MASK_PPT; ++q) {
+        const int p = p0 + q * MASK_THREADS;
+        py[q] = p / W;
+        px[q] = p - py[q] * W;
+        if (p < HW) out[p] = (short)(win[q] >= 0 ? __ldg(lab + win[q]) : 0);
+    }
+    for (int j = 0; j < mi; ++j) {
+        unsigned c = 0, x0 = 0, x1 = 0, y0 = 0, y1 = 0;
+#pragma unroll
+        for (int q = 0; q < MASK_PPT; ++q)
+            if (win[q] == j) {                         // win is -1 past the end of the image
+                ++c;
+                x0 = max(x0, (unsigned)(W - px[q])); x1 = max(x1, (unsigned)(px[q] + 1));
+                y0 = max(y0, (unsigned)(H - py[q])); y1 = max(y1, (unsigned)(py[q] + 1));
+            }
+        if (!__any_sync(0xffffffffu, c != 0)) continue;
+        c = __reduce_add_sync(0xffffffffu, c);
+        x0 = __reduce_max_sync(0xffffffffu, x0); x1 = __reduce_max_sync(0xffffffffu, x1);
+        y0 = __reduce_max_sync(0xffffffffu, y0); y1 = __reduce_max_sync(0xffffffffu, y1);
+        if (lane == 0) {
+            unsigned *s = s_acc + 6 * j;
+            atomicAdd(s + 1, c);
+            atomicMax(s + 2, x0); atomicMax(s + 3, x1); atomicMax(s + 4, y0); atomicMax(s + 5, y1);
+        }
+    }
+    __syncthreads();
+    for (int j = threadIdx.x; j < mi; j += MASK_THREADS) {
+        const unsigned *s = s_acc + 6 * j;
+        MaskAcc *g = acc + i0 + j;
+        if (s[0]) atomicAdd(&g->a, s[0]);
+        if (s[1]) {
+            atomicAdd(&g->p, s[1]);
+            atomicMax(&g->x0, s[2]); atomicMax(&g->x1, s[3]); atomicMax(&g->y0, s[4]); atomicMax(&g->y1, s[5]);
+        }
+    }
+}
+
+__global__ void mask_finish_kernel(const MaskAcc *__restrict__ acc, int m, int H, int W, long long *__restrict__ a_out,
+                                   long long *__restrict__ p_out, int *__restrict__ box_out)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    const MaskAcc s = acc[i];
+    a_out[i] = s.a;
+    p_out[i] = s.p;
+    const int x = s.p ? W - (int)s.x0 : 0, y = s.p ? H - (int)s.y0 : 0;
+    box_out[4 * i + 0] = x;
+    box_out[4 * i + 1] = y;
+    box_out[4 * i + 2] = s.p ? (int)s.x1 - x : 0;
+    box_out[4 * i + 3] = s.p ? (int)s.y1 - y : 0;
+}
+
 } // namespace
 
 size_t render_workspace_bytes(int n, int F)
@@ -360,6 +468,37 @@ cudaError_t launch_vsd(const VsdArgs &a, void *workspace, cudaStream_t st)
     if (chunks > 0)
         vsd_count_kernel<<<dim3((unsigned)chunks, (unsigned)(a.n < 65535 ? a.n : 65535)), VSD_THREADS, 0, st>>>(a, counts);
     vsd_final_kernel<<<(unsigned)((a.n + 255) / 256), 256, 0, st>>>(a, counts);
+    return cudaGetLastError();
+}
+
+namespace {
+size_t mask_table_bytes(int B, int m)
+{
+    return (((size_t)B + 1 + 2 * (size_t)m) * sizeof(int) + 255) / 256 * 256;
+}
+} // namespace
+
+size_t instance_masks_workspace_bytes(int B, int m)
+{
+    return mask_table_bytes(B, m) + ((size_t)m * sizeof(MaskAcc) + 255) / 256 * 256;
+}
+
+cudaError_t launch_instance_masks(const float *depth, const int *table, int B, int m, int max_m, int H, int W,
+                                  short *label, long long *a_out, long long *p_out, int *box_out, void *workspace,
+                                  cudaStream_t st)
+{
+    int *d_table = static_cast<int *>(workspace);
+    MaskAcc *acc = reinterpret_cast<MaskAcc *>(static_cast<char *>(workspace) + mask_table_bytes(B, m));
+    // the table is pageable host memory: the copy stages it before returning, so the caller may free it at once
+    cudaError_t e = cudaMemcpyAsync(d_table, table, ((size_t)B + 1 + 2 * (size_t)m) * sizeof(int), cudaMemcpyHostToDevice, st);
+    if (e != cudaSuccess) return e;
+    e = cudaMemsetAsync(acc, 0, (size_t)m * sizeof(MaskAcc), st);
+    if (e != cudaSuccess) return e;
+    const int chunks = (H * W + MASK_PIXELS - 1) / MASK_PIXELS;
+    if (chunks > 0)
+        mask_compose_kernel<<<dim3((unsigned)chunks, (unsigned)B), MASK_THREADS, (size_t)max_m * sizeof(MaskAcc), st>>>(
+            depth, d_table, B, m, H, W, label, acc);
+    mask_finish_kernel<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(acc, m, H, W, a_out, p_out, box_out);
     return cudaGetLastError();
 }
 

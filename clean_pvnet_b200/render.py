@@ -8,9 +8,19 @@
     install_depth_renderer_as_reference()                  `lib.utils.renderer.opengl_utils` and `lib.utils.vsd.renderer`
                                                            bind this module: DepthRender / render(mode='depth') without glumpy
 
+and T-LESS's instance masks (DESIGN.md section 8k), what lib/datasets/tless/handle_test_data.py:get_mask builds with OpenGL:
+
+    instance_masks_batch(meshes, mesh_index, obj_ids, image_index, poses, K, size)
+                                                           label map, unoccluded and visible pixel counts and bounding box
+                                                           of every instance of B images -> CUDA tensors
+    instance_masks_from_depth(depth, slot, obj_ids, image_index)
+                                                           the same from given depth images (the compose step alone)
+    install_tless_renderer_as_reference()                  `lib.datasets.tless.opengl_backend` binds this module
+
 Poses are [R|t] in the units of the mesh: the evaluator renders its model in millimetres with t * 1000.  Nothing is
 copied to the host and nothing waits for the device; every chunk is planned from the shapes.
 """
+import ctypes
 import sys
 
 import numpy as np
@@ -158,6 +168,178 @@ def vsd_batch(pts, faces, pose_est, pose_gt, K, depth_test, pairs, delta=VSD_DEL
     return e
 
 
+# ---- T-LESS's instance masks (DESIGN.md section 8k) ------------------------------------------------------------------
+
+def _host_ints(x, name):
+    """A host table (from gt.yml) as a 1-D int64 numpy array; a CUDA tensor is refused rather than copied back."""
+    if isinstance(x, torch.Tensor) and x.is_cuda:
+        raise RuntimeError(f"{name} must be host data (a list, numpy array or CPU tensor), got a CUDA tensor")
+    a = np.asarray(x.numpy() if isinstance(x, torch.Tensor) else x)
+    if a.ndim != 1 or not (a.size == 0 or np.issubdtype(a.dtype, np.integer)):
+        raise RuntimeError(f"{name} must be a 1-D integer table, got {a.dtype} {list(a.shape)}")
+    return a.astype(np.int64)
+
+
+def _upload(a, dev):
+    """A host index table on the device without waiting for it: pinned staging and a non-blocking copy."""
+    return torch.from_numpy(np.ascontiguousarray(a)).pin_memory().to(dev, non_blocking=True)
+
+
+def _instance_plan(obj_ids, image_index, B):
+    """Checks the tables and returns image_first [B+1] (image b's instances are [first[b], first[b+1]))."""
+    n = len(image_index)
+    if len(obj_ids) != n:
+        raise RuntimeError(f"obj_ids and image_index must have one entry per instance, got {len(obj_ids)} and {n}")
+    if n and (np.any(np.diff(image_index) < 0) or image_index[0] < 0 or image_index[-1] >= B):
+        raise RuntimeError(f"image_index must be non-decreasing (each image's instances together, in gt order) and in "
+                           f"[0, {B})")
+    first = np.searchsorted(image_index, np.arange(B + 1), side="left")
+    rank = np.arange(n) - first[image_index] if n else np.zeros(0, np.int64)
+    label = obj_ids * 1000 + rank
+    if n and (label.min() < -32768 or label.max() > 32767):
+        raise RuntimeError("obj_id * 1000 + instance_id must fit int16 (the label map's type)")
+    return first
+
+
+def _compose(depth, n_depth, slot, obj, first, b0, b1, H, W, label, a_num, p_num, bbox, dev):
+    """pvb_instance_masks over images [b0, b1), split where an image has no instance (its label map stays 0)."""
+    slot32, obj32 = np.ascontiguousarray(slot, np.int32), np.ascontiguousarray(obj, np.int32)
+    b = b0
+    while b < b1:
+        if first[b] == first[b + 1]:
+            b += 1
+            continue
+        e = b
+        while e < b1 and e - b < 65535 and first[e] != first[e + 1]:
+            e += 1
+        f32 = np.ascontiguousarray(first[b:e + 1], np.int32)
+        nbytes = _lib.load().pvb_instance_masks_workspace_bytes(e - b, int(f32[-1] - f32[0]))
+        _call("pvb_instance_masks", dev, depth, n_depth, slot32.ctypes.data_as(ctypes.c_void_p),
+              obj32.ctypes.data_as(ctypes.c_void_p), len(obj32), f32.ctypes.data_as(ctypes.c_void_p), e - b, H, W,
+              label[b], a_num, p_num, bbox, _workspace(nbytes, dev), nbytes)
+        b = e
+
+
+def _mask_outputs(B, n, H, W, first, dev):
+    empty = bool(np.any(first[1:] == first[:-1]))
+    label = (torch.zeros if empty else torch.empty)((B, H, W), dtype=torch.int16, device=dev)
+    return (label, torch.empty(n, dtype=torch.int64, device=dev), torch.empty(n, dtype=torch.int64, device=dev),
+            torch.empty((n, 4), dtype=torch.int32, device=dev))
+
+
+def instance_masks_from_depth(depth, slot, obj_ids, image_index):
+    """handle_test_data.get_mask's compose step (lib/datasets/tless/handle_test_data.py:81-134) on given depth images:
+        depth        [S,H,W] depth slots in mm, as pvb_render_depth writes them (rounded to float32)
+        slot         host [n]: instance i reads depth[slot[i]]
+        obj_ids      host [n]: each instance's obj_id
+        image_index  host [n], non-decreasing: each instance's image; instance_id is its rank within the image
+    Each image b in [0, max(image_index)] composes its instances in order, as update_mask does on
+    opengl_renderer.render's depth / 1000.  Returns (label int16 [B,H,W], a_pixel_num int64 [n], pixel_num int64 [n],
+    bbox int32 [n,4]) on the device of depth: the mask/*.png label map (obj_id * 1000 + instance_id), pixel_num.pkl's
+    count of each instance's rendered pixels, the count of its labelled pixels, and cv2.boundingRect (x, y, w, h) of those
+    ((0, 0, 0, 0) when it has none).  Exact integers, bit-identical run to run; an image's outputs depend on nothing else."""
+    d = torch.as_tensor(depth)
+    if d.dim() != 3:
+        raise RuntimeError(f"depth must be [S,H,W], got {list(d.shape)}")
+    S, H, W = (int(s) for s in d.shape)
+    sl, obj, img = _host_ints(slot, "slot"), _host_ints(obj_ids, "obj_ids"), _host_ints(image_index, "image_index")
+    if len(sl) != len(img):
+        raise RuntimeError(f"slot and image_index must have one entry per instance, got {len(sl)} and {len(img)}")
+    if len(sl) and (sl.min() < 0 or sl.max() >= S):
+        raise RuntimeError(f"slot must index depth's {S} images")
+    n = len(img)
+    B = int(img[-1]) + 1 if n else 0
+    first = _instance_plan(obj, img, B)
+    dev = _device(d)
+    d = _to(d, dev, torch.float32)
+    out = _mask_outputs(B, n, H, W, first, dev)
+    _compose(d, S, sl, obj, first, 0, B, H, W, *out, dev)
+    return out
+
+
+def instance_masks_batch(meshes, mesh_index, obj_ids, image_index, poses, K, size, near=10, far=10000,
+                         max_render_bytes=1 << 30):
+    """handle_test_data.get_mask (lib/datasets/tless/handle_test_data.py:93-134) for B images at once, without OpenGL:
+        meshes       list of (pts [V,3], faces [F,3]) in mm (the CAD models as load_ply returns them)
+        mesh_index   host [n]: the mesh of each instance; obj_ids host [n]: its obj_id (gt.yml's obj_id)
+        image_index  host [n], non-decreasing: its image (instance_id is its rank within the image, gt_'s order)
+        poses        [n,3,4] [R|t] with t in mm (cam_t_m2c, as opengl_renderer.render passes t * 1000)
+        K            [3,3] shared or [B,3,3] per image; size (width, height)
+    Each instance is rendered as opengl_renderer.render renders it (pvb_render_depth at clip planes near / far) into a
+    slot of a scratch window that holds whole images within max_render_bytes, then the window's images are composed as
+    instance_masks_from_depth does.  B is K's first dimension, else max(image_index) + 1.  Returns (label int16 [B,H,W],
+    a_pixel_num int64 [n], pixel_num int64 [n], bbox int32 [n,4]) on the device of poses (the current CUDA device when
+    it is not a CUDA tensor).  Nothing is copied back to the host; with the meshes, poses and K on the device nothing
+    waits for it either (the host tables go up through pinned, non-blocking copies)."""
+    mi, obj, img = _host_ints(mesh_index, "mesh_index"), _host_ints(obj_ids, "obj_ids"), _host_ints(image_index,
+                                                                                                    "image_index")
+    ms = [_mesh(p, f) for p, f in meshes]
+    pz, km = torch.as_tensor(poses), torch.as_tensor(K)
+    n = len(img)
+    if pz.dim() != 3 or tuple(pz.shape) != (n, 3, 4):
+        raise RuntimeError(f"poses must be [{n},3,4], got {list(pz.shape)}")
+    if len(mi) != n:
+        raise RuntimeError(f"mesh_index must have one entry per instance, got {len(mi)} for {n}")
+    if n and (mi.min() < 0 or mi.max() >= len(ms)):
+        raise RuntimeError(f"mesh_index must index the {len(ms)} meshes")
+    if km.dim() == 3 and tuple(km.shape[1:]) == (3, 3):
+        B = int(km.shape[0])
+    elif tuple(km.shape) == (3, 3):
+        B = int(img[-1]) + 1 if n else 0
+    else:
+        raise RuntimeError(f"K must be [3,3] or [B,3,3], got {list(km.shape)}")
+    W, H = _size(size)
+    if not (0 < float(near) <= float(far) < float("inf")):
+        raise RuntimeError(f"need 0 < near <= far < inf, got {near}, {far}")
+    first = _instance_plan(obj, img, B)
+    dev = _device(pz, km, *(t for m in ms for t in m))
+    out = _mask_outputs(B, n, H, W, first, dev)
+    if n == 0 or H * W == 0:
+        if n:
+            _compose(None, 1, np.zeros(n, np.int64), obj, first, 0, B, H, W, *out, dev)
+        return out
+    # windows of whole images within max_render_bytes (at least one image each)
+    per = H * W * 4
+    windows, b0 = [], 0
+    while b0 < B:
+        b1 = b0 + 1
+        while b1 < B and (first[b1 + 1] - first[b0]) * per <= max_render_bytes:
+            b1 += 1
+        windows.append((b0, b1))
+        b0 = b1
+    # within a window the instances are rendered mesh by mesh: order = window-major, then mesh, then instance
+    order = np.concatenate([first[w0] + np.argsort(mi[first[w0]:first[w1]], kind="stable") for w0, w1 in windows])
+    pos = np.empty(n, np.int64)
+    pos[order] = np.arange(n)
+    identity = bool(np.all(order == np.arange(n)))
+    perm = None if identity else _upload(order, dev)
+    pz = _to(pz, dev, torch.float64)
+    pz = pz if identity else pz.index_select(0, perm)
+    km = _to(km, dev, torch.float64)
+    if km.dim() == 3:
+        kimg = _upload(img[order], dev)
+        km, kst = km.index_select(0, kimg).contiguous(), 9
+    else:
+        kst = 0
+    mesh_dev = {}
+    width = max(int(first[w1] - first[w0]) for w0, w1 in windows)
+    buf = torch.empty((width, H, W), dtype=torch.float32, device=dev)
+    for w0, w1 in windows:
+        s0, s1 = int(first[w0]), int(first[w1])
+        if s0 == s1:
+            continue                                   # images without instances: their label maps are zero-filled
+        sorted_mesh = mi[order[s0:s1]]
+        starts = np.flatnonzero(np.r_[True, sorted_mesh[1:] != sorted_mesh[:-1]])
+        for a, z in zip(starts, np.r_[starts[1:], s1 - s0]):
+            k = int(sorted_mesh[a])
+            if k not in mesh_dev:
+                mesh_dev[k] = (_to(ms[k][0], dev, torch.float32), _to(ms[k][1], dev, torch.int32))
+            p, f = mesh_dev[k]
+            _render(p, f, pz[s0 + a:s0 + z], km[s0 + a:s0 + z] if kst else km, kst, W, H, near, far, buf[a:z])
+        _compose(buf, s1 - s0, pos - s0, obj, first, w0, w1, H, W, *out, dev)
+    return out
+
+
 # ---- drop-in twins of the reference's OpenGL renderers (depth only) --------------------------------------------------
 
 def _pose(R, t):
@@ -209,4 +391,17 @@ def install_depth_renderer_as_reference():
         parent = reference_package(parent_name)
         sys.modules[f"{parent_name}.{leaf}"] = this
         setattr(parent, leaf, this)
+    return this
+
+
+def install_tless_renderer_as_reference():
+    """Makes `from lib.datasets.tless import opengl_backend` (lib/datasets/tless/opengl_renderer.py:3) bind this module,
+    so opengl_renderer, handle_test_data and handle_ag_data import without glumpy, and opengl_renderer.render(model, pose,
+    K, w, h) returns this renderer's depth / 1000 (its render(..., clip_near=10, clip_far=10000, mode='depth')).  Only
+    the leaf module is replaced; `lib.datasets.tless` stays the real package whenever it exists.  Idempotent."""
+    from ._dropin import reference_package
+    this = sys.modules[__name__]
+    parent = reference_package("lib.datasets.tless")
+    sys.modules["lib.datasets.tless.opengl_backend"] = this
+    setattr(parent, "opengl_backend", this)
     return this

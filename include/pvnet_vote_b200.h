@@ -36,6 +36,8 @@
  *   utils/renderer/opengl_utils.py:405-490  DepthRender.render     pvb_render_depth (n poses per call, no OpenGL)
  *   utils/vsd/vsd_utils.py:5-48  vsd (cost 'step'), as
  *   evaluators/tless_test/pvnet.py:66-105  vsd_metric calls it     pvb_vsd (n pose pairs per call)
+ *   datasets/tless/handle_test_data.py:81-134  get_mask's
+ *     render + update_mask loop, pixel_num.pkl, boundingRect       pvb_instance_masks (B images per call)
  *   utils/tless/tless_test_utils.py:57-77  pvnet_transform,
  *   networks/ct_pvnet/res.py:14-31  _crop                           pvb_crop_inputs (n boxes per call)
  *   evaluators/tless_test/pvnet.py:229-239  keypoint un-crop        pvb_uncrop_keypoints (n boxes per call)
@@ -396,6 +398,34 @@ PVB_API int pvb_vsd(const float *depth_test, int32_t B, const float *depth_est, 
                     const float *depth_gt, int32_t n_gt, int32_t gt_base, const int32_t *pairs, int32_t n, const double *K,
                     int64_t k_stride, int32_t H, int32_t W, double delta, double tau, double *e, void *workspace,
                     size_t workspace_bytes, pvb_stream_t stream);
+
+/* ---- T-LESS's instance masks without OpenGL (DESIGN.md section 8k) -------------------------------------------------
+ * Replaces the per-instance loop of lib/datasets/tless/handle_test_data.py:93-134 (get_mask: opengl_renderer.render
+ * + update_mask at :81-90 + np.sum(depth != 0)), and the counts and cv2.boundingRect that test_to_coco (:14-61) and
+ * record_scene_ann (:137-194) take from its mask PNGs and pixel_num.pkl, for B images at once.  Image b composes the
+ * instances [image_first[b], image_first[b+1]) in order; instance i, the (i - image_first[b])-th of its image, reads
+ * depth[slot[i]] (pvb_render_depth's mm depth, e.g. at clip planes 10 / 10000):
+ *   key = fp32(depth / 1000) (opengl_renderer.render's division); per pixel the label map starts at 0 and the depth map
+ *   at 10.0f, and the instance takes the pixel when key != 0 and key < depth map (ties go to the earlier instance; a key
+ *   of 10 or more never takes it); label[b] is then obj_id[i] * 1000 + (i - image_first[b]) where instance i took it.
+ *   a_pixel_num[i] = #(key != 0), pixel_num[i] = #(pixels labelled i), bbox[i] = cv2.boundingRect of those pixels as
+ *   (x, y, w, h), (0, 0, 0, 0) when there are none.
+ *   depth device fp32 [n_depth,H,W]; slot, obj_id HOST int32 [n]; image_first HOST int32 [B+1]; label device int16
+ *   [B,H,W], fully written; a_pixel_num, pixel_num device int64 [n] and bbox device int32 [n,4] are written for the
+ *   instances [image_first[0], image_first[B]) and left untouched elsewhere, so a caller can render the instances in
+ *   windows of whole images and call once per window.  No mask is stored; every output is an integer sum of per-CTA
+ *   integer reductions, so the result is exact and bit-identical run to run, and an image's outputs depend on nothing
+ *   else in the call.  Each range must be non-empty, within [0, n) and hold at most 2048 instances, each slot in
+ *   [0, n_depth), each label must fit int16, B <= 65535 and H * W < 2^31.  The table is copied to the device from host
+ *   memory within the call, so unlike the other entries this one cannot be captured into a CUDA graph.  workspace:
+ *   pvb_instance_masks_workspace_bytes(B, image_first[B] - image_first[0]) bytes of 256-byte aligned device memory.
+ *   B == 0 is a no-op.
+ * Bad arguments return PVB_ERR_INVALID, a missing or short workspace PVB_ERR_WORKSPACE, both before any CUDA call. */
+PVB_API size_t pvb_instance_masks_workspace_bytes(int32_t B, int32_t m);
+PVB_API int pvb_instance_masks(const float *depth, int32_t n_depth, const int32_t *slot, const int32_t *obj_id, int32_t n,
+                               const int32_t *image_first, int32_t B, int32_t H, int32_t W, int16_t *label,
+                               int64_t *a_pixel_num, int64_t *pixel_num, int32_t *bbox, void *workspace,
+                               size_t workspace_bytes, pvb_stream_t stream);
 
 /* ---- T-LESS's PVNet crop and un-crop (DESIGN.md section 8g) ---------------------------------------------------------
  * Shared: img device uint8 [B,H,W,C] at element strides img_stride (HOST int64[4], for B, H, W, C), H, W <= 32767;
