@@ -28,6 +28,8 @@ Public surface (same names/signatures as the reference):
     install_ct_loss_as_reference
     ct_decode.decode_detections (twin of lib/networks/ct/dla.py's Network.decode_detection for B images),
     detection_boxes (the consumers' un-crop of the boxes to the image), install_ct_decode_as_reference
+    fps.farthest_point_sampling (twin of lib/csrc/fps/fps_utils.py, the custom-object keypoint pick),
+    farthest_point_sampling_batch (B ragged clouds per launch), install_fps_as_reference_module
 """
 from . import _lib  # noqa: F401
 from . import nn  # noqa: F401
@@ -56,6 +58,8 @@ from .ct_loss import (ct_focal_loss, ct_target_batch, ct_radius, CtNetworkWrappe
                       install_ct_loss_as_reference)
 from . import ct_decode  # noqa: F401
 from .ct_decode import decode_detections, detection_boxes, install_ct_decode_as_reference  # noqa: F401
+from . import fps  # noqa: F401
+from .fps import farthest_point_sampling, farthest_point_sampling_batch, install_fps_as_reference_module  # noqa: F401
 from .ransac_voting_gpu import (  # noqa: F401
     estimate_voting_distribution_with_mean,
     ransac_voting_layer,
@@ -78,4 +82,5 @@ __all__ = [
     "dcn", "dcn_v2_conv", "DCNv2", "DCN", "install_dcn_as_reference_module",
     "ct_loss", "ct_focal_loss", "ct_target_batch", "ct_radius", "CtNetworkWrapper", "install_ct_loss_as_reference",
     "ct_decode", "decode_detections", "detection_boxes", "install_ct_decode_as_reference",
+    "fps", "farthest_point_sampling", "farthest_point_sampling_batch", "install_fps_as_reference_module",
 ]

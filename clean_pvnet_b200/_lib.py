@@ -89,6 +89,8 @@ SIGNATURES = {
     "pvb_instance_masks_workspace_bytes": (_sz, [_i32, _i32]),
     "pvb_instance_masks": (ctypes.c_int, [_vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _sz,
                                           _vp]),
+    "pvb_fps_workspace_bytes": (_sz, [_i32, _i32]),
+    "pvb_farthest_point_sampling": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _vp, _sz, _vp]),
     "pvb_crop_inputs": (ctypes.c_int, [_vp, _i32, _i32, _i32, ctypes.POINTER(ctypes.c_int64), _vp, _vp, _i32, _i32, _i32,
                                        ctypes.c_double, ctypes.c_double, _i32, ctypes.POINTER(ctypes.c_float),
                                        ctypes.POINTER(ctypes.c_float), _vp, _vp, _vp, _vp, _vp, _vp, _vp]),

@@ -952,6 +952,32 @@ PVB_API int pvb_instance_masks(const float *depth, int32_t n_depth, const int32_
     return e == cudaSuccess ? PVB_OK : cuda_fail(e, "instance mask kernels");
 }
 
+PVB_API size_t pvb_fps_workspace_bytes(int32_t b, int32_t n)
+{
+    if (b <= 0 || n <= 0) return 0;
+    return fps_workspace_bytes(b, n);
+}
+
+PVB_API int pvb_farthest_point_sampling(const float *pts, const int32_t *counts, const int32_t *starts, int32_t init_center,
+                                        int32_t *idxs, int32_t b, int32_t n, int32_t sn, void *workspace,
+                                        size_t workspace_bytes, pvb_stream_t stream)
+{
+    if (b < 0 || n < 0 || sn < 0) return fail(PVB_ERR_INVALID, "negative size (b=%d n=%d sn=%d)", b, n, sn);
+    if (b > 0x7fffffff / 8) return fail(PVB_ERR_INVALID, "b too large (got %d)", b);
+    if (b == 0 || sn == 0) return PVB_OK;
+    if (!pts || !idxs || !counts || (!init_center && !starts)) return fail(PVB_ERR_INVALID, "NULL pointer");
+    for (int32_t i = 0; i < b; ++i) {
+        if (counts[i] < 1 || counts[i] > n)
+            return fail(PVB_ERR_INVALID, "cloud %d has %d points (must be in [1, %d])", i, counts[i], n);
+        if (!init_center && (starts[i] < 0 || starts[i] >= counts[i]))
+            return fail(PVB_ERR_INVALID, "cloud %d starts at %d (must be in [0, %d))", i, starts[i], counts[i]);
+    }
+    if (int rc = nn_check_workspace(fps_workspace_bytes(b, n), workspace, workspace_bytes)) return rc;
+    cudaError_t e = launch_fps(pts, counts, starts, init_center != 0, idxs, b, n, sn, workspace,
+                               static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "farthest point sampling kernel");
+}
+
 namespace {
 
 // the image and output arguments the crop and the warp share; fills the image and size fields of `a`

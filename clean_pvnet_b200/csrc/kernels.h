@@ -321,6 +321,13 @@ DcnPlan dcn_plan(const DcnArgs &a, int chunk);
 cudaError_t launch_dcn_forward(const DcnArgs &a, cudaStream_t st);
 cudaError_t launch_dcn_backward(DcnArgs a, const DcnPlan &plan, void *workspace, cudaStream_t st);
 
+// farthest-point sampling (fps.cu): the counts [b] and starts [b] (unused under init_center) tables, then the min_dist of
+// every cloud's points past the first CTA's on-chip slice
+size_t fps_workspace_bytes(int b, int n);
+// pts [b][n][3] fp32, counts / starts HOST int32 [b] (validated by the caller) -> idxs [b][sn]
+cudaError_t launch_fps(const float *pts, const int *counts, const int *starts, int init_center, int *idxs, int b, int n,
+                       int sn, void *workspace, cudaStream_t st);
+
 // twins of the reference extension on its own layouts
 cudaError_t launch_compat_generate(const float *direct, const float *coords, const int32_t *idxs, float *hyp,
                                    int tn, int vn, int hn, bool vanishing, cudaStream_t st);

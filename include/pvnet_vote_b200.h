@@ -38,6 +38,7 @@
  *   evaluators/tless_test/pvnet.py:66-105  vsd_metric calls it     pvb_vsd (n pose pairs per call)
  *   datasets/tless/handle_test_data.py:81-134  get_mask's
  *     render + update_mask loop, pixel_num.pkl, boundingRect       pvb_instance_masks (B images per call)
+ *   lib/csrc/fps/src/ext.h  farthest_point_sampling{,_init_center}  pvb_farthest_point_sampling (b clouds per call)
  *   utils/tless/tless_test_utils.py:57-77  pvnet_transform,
  *   networks/ct_pvnet/res.py:14-31  _crop                           pvb_crop_inputs (n boxes per call)
  *   evaluators/tless_test/pvnet.py:229-239  keypoint un-crop        pvb_uncrop_keypoints (n boxes per call)
@@ -426,6 +427,26 @@ PVB_API int pvb_instance_masks(const float *depth, int32_t n_depth, const int32_
                                const int32_t *image_first, int32_t B, int32_t H, int32_t W, int16_t *label,
                                int64_t *a_pixel_num, int64_t *pixel_num, int32_t *bbox, void *workspace,
                                size_t workspace_bytes, pvb_stream_t stream);
+
+/* ---- farthest-point sampling (DESIGN.md section 8l) ------------------------------------------------------------------
+ * The batched device twin of the reference's two cffi entries (lib/csrc/fps/src/ext.h, farthest_point_sampling.cpp)
+ *   farthest_point_sampling(pts, idxs, pn, sn)               (random start: rand() % pn after srand(time(0)))
+ *   farthest_point_sampling_init_center(pts, idxs, pn, sn)   (start: the point farthest from the bounding box's centre)
+ * for b clouds at once.  Cloud i is the first counts[i] rows of pts[i]; idxs[i] are the reference's indices for it, element
+ * for element, with its fp32 arithmetic (no contraction), its index-order tie rule and its fallback to index 0 when no
+ * unselected point has a distance > 0 (so sn > counts[i] repeats index 0).  init_center == 0 starts cloud i at
+ * starts[i], the value the reference draws with rand(); everything after the start is bit-equal.
+ *   pts device fp32 [b,n,3]; counts HOST int32 [b], each in [1, n]; starts HOST int32 [b], each in [0, counts[i])
+ *   (ignored, and NULL allowed, when init_center != 0); idxs device int32 [b,sn].  workspace:
+ *   pvb_fps_workspace_bytes(b, n) bytes of 256-byte aligned device memory.  The tables are copied to the device from host
+ *   memory within the call, so, like pvb_instance_masks, it cannot be captured into a CUDA graph; it does not synchronise
+ *   with the host.  b == 0 or sn == 0 is a no-op.
+ * Bad arguments (NULL pointers, negative sizes, a count or start out of range) return PVB_ERR_INVALID, a missing or short
+ * workspace PVB_ERR_WORKSPACE, both before any CUDA call. */
+PVB_API size_t pvb_fps_workspace_bytes(int32_t b, int32_t n);
+PVB_API int pvb_farthest_point_sampling(const float *pts, const int32_t *counts, const int32_t *starts, int32_t init_center,
+                                        int32_t *idxs, int32_t b, int32_t n, int32_t sn, void *workspace,
+                                        size_t workspace_bytes, pvb_stream_t stream);
 
 /* ---- T-LESS's PVNet crop and un-crop (DESIGN.md section 8g) ---------------------------------------------------------
  * Shared: img device uint8 [B,H,W,C] at element strides img_stride (HOST int64[4], for B, H, W, C), H, W <= 32767;
