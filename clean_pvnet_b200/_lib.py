@@ -134,6 +134,7 @@ SIGNATURES = {
     "pvb_profile_enable": (ctypes.c_int, [_i32]),
     "pvb_profile_reset": (ctypes.c_int, []),
     "pvb_set_tuning": (ctypes.c_int, [_i32, _i32]),
+    "pvb_set_pass1_stats": (ctypes.c_int, [_vp]),
     "pvb_set_group_tuning": (ctypes.c_int, [_i32, _i32]),
     "pvb_profile_read": (ctypes.c_int, [ctypes.POINTER(ctypes.c_double), _i32]),
     "pvb_generate_hypothesis": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),

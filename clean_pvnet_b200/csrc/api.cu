@@ -1530,6 +1530,12 @@ PVB_API int pvb_set_tuning(int32_t gather_mode, int32_t vote_variant)
     return PVB_OK;
 }
 
+PVB_API int pvb_set_pass1_stats(void *dev_counts)
+{
+    set_pass1_stats(static_cast<unsigned long long *>(dev_counts));
+    return PVB_OK;
+}
+
 PVB_API int pvb_set_group_tuning(int32_t max_groups, int32_t streams)
 {
     if (max_groups < 0 || max_groups > 65535) return fail(PVB_ERR_INVALID, "max_groups must be 0..65535");

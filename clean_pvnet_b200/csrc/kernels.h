@@ -91,6 +91,7 @@ cudaError_t launch_vote_list(const VoteArgs &a, const int *list, const int *len,
 // Pass 1: vote_kernel, hypotheses in registers, in slices of 128 entries
 cudaError_t launch_vote_list_slices(const VoteArgs &a, const int *list, const int *len, int max_len, cudaStream_t st);
 void set_vote_tuning(int variant);   // tooling: pixel-tile size per CTA
+void set_pass1_stats(unsigned long long *dev);   // tooling: pass 1's per-box test counts (NULL: off)
 void set_gather_tuning(int mode);    // tooling: gather access pattern (select.cu)
 // argmax + winner refit -> out_kpt [B][K][2], win [B][K].  The pixels of one (image,keypoint) are split
 // over `splits` CTAs; partial normal equations meet in `partial`, the last CTA to arrive (ticket) adds

@@ -82,6 +82,7 @@ struct VoteK {
     ConeParams cone;
     const int *list;   // optional [B][K][hn]: slot s of (b,k) scores hypothesis list[s] (NULL: slot s is hypothesis s)
     const int *len;    // [B][K] slots in use (with list)
+    unsigned long long *stats;   // optional, BOX: [3] tests resolved per box as inliers, all tests resolved per box, tests scored
 };
 
 constexpr int VOTE_BLOCK = 16;    // pixels per unrolled block (one guard-band check per block)
@@ -101,6 +102,26 @@ __device__ __forceinline__ float cone_margin(const float4 ra, const float2 rb, f
     const float ap = fmaf(ra.x, hxc, fmaf(ra.y, hyc, ra.z));
     const float pp = fmaf(ra.w, hxc, fmaf(rb.x, hyc, rb.y));
     return ap - fabsf(pp);
+}
+
+// Pass 1's per-box classification of one pixel record (DESIGN.md 4.2, "Pass 1 per box"): the record's two affine forms
+// a = kappa*u.(h-c) and p = u_perp.(h-c) are evaluated at the four corners (x0|x1, y0|y1) of the box of the CTA's
+// hypotheses with cone_margin's operations.  1: every hypothesis of the box is an inlier (m = a - |p| > d at all
+// corners: m is concave); -1: none is (a + p or a - p < -d at all corners: both are affine and bound m from above);
+// 0: undecided, each hypothesis is tested on its own.  d = inf (an unbounded hypothesis in the box) decides nothing.
+__device__ __forceinline__ int box_class(const float4 ra, const float2 rb, float x0, float x1, float y0, float y1, float d)
+{
+    float mn = CUDART_INF_F, lp = -CUDART_INF_F, lm = -CUDART_INF_F;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        const float x = (q & 1) ? x1 : x0, y = (q & 2) ? y1 : y0;
+        const float ap = fmaf(ra.x, x, fmaf(ra.y, y, ra.z));
+        const float pp = fmaf(ra.w, x, fmaf(rb.x, y, rb.y));
+        mn = fminf(mn, ap - fabsf(pp));
+        lp = fmaxf(lp, ap + pp);
+        lm = fmaxf(lm, ap - pp);
+    }
+    return (mn > d) ? 1 : (lp < -d || lm < -d) ? -1 : 0;
 }
 
 // Loads a tile's n pixels, pixel i = threadIdx.x + r*NT to slot r (zeros past n), and returns the tile-local origin (ox, oy),
@@ -176,10 +197,15 @@ __device__ __forceinline__ float3 hyp_frame(float2 q, float ox, float oy, float 
 // WS = warps that together hold one hypothesis slice (HPT*WS*32 hypotheses).  With fewer than 512 hypotheses per
 // keypoint the remaining NT/32/WS warp teams of the CTA split the tile's 16-pixel blocks between them, so every
 // thread still owns HPT hypotheses and the inner loop keeps its instruction mix.
-template <int HPT, int NT, int MINB, int VOTE_TILE, int WS>
+// BOX (pass 1): every warp holds the whole slice, so each warp finds the box of its hypotheses on its own.  The tile's
+// pixels are classified once against that box (box_class); certain inliers count for every hypothesis without a test,
+// certain outliers are dropped, and the undecided ones are compacted to the front of the tile's records, which the inner
+// loop then scores as before, guard band and exact path included.
+template <int HPT, int NT, int MINB, int VOTE_TILE, int WS, bool BOX>
 __global__ void __launch_bounds__(NT, MINB)
 vote_kernel(const VoteK p)
 {
+    static_assert(!BOX || WS == 1, "the box path needs every warp to hold the whole slice");
     constexpr int PPT = VOTE_TILE / NT;               // pixels staged per thread
     constexpr int NW = NT / 32;
     constexpr int TEAM = WS * 32;                     // threads per hypothesis slice
@@ -187,6 +213,8 @@ vote_kernel(const VoteK p)
     __shared__ __align__(16) float4 s_a[VOTE_TILE];   // (A1, A2, A3, B1)
     __shared__ __align__(16) float2 s_b[VOTE_TILE];   // (B2, B3)
     __shared__ float s_box[4][NW];
+    __shared__ uint16_t s_idx[BOX ? VOTE_TILE : 1];   // BOX: tile index of each compacted record
+    __shared__ int s_nu[BOX ? PPT : 1][NW];           // BOX: undecided pixels per round and warp
     const VoteArgs &a = p.a;
     const int b = blockIdx.z;
     const int k = blockIdx.y % a.K, slice = blockIdx.y / a.K;
@@ -197,7 +225,7 @@ vote_kernel(const VoteK p)
     const int *lst = p.list ? p.list + bk * a.hn : nullptr;
     const int n = min(VOTE_TILE, tn - t0);
     const int npad = (n + VOTE_BLOCK - 1) / VOTE_BLOCK * VOTE_BLOCK;
-    const int tid = threadIdx.x, lane = tid & 31;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const float kappa = p.cone.kappa, thresh = p.cone.thresh;
     const float2 *hyp = a.hyp + bk * a.hn;
     const float2 *xy = a.xy + (size_t)b * a.cap + t0;
@@ -242,10 +270,68 @@ vote_kernel(const VoteK p)
     }
     __syncthreads();
 
+    int nl = n;     // records scored one hypothesis at a time: the first nl of the tile's (after compaction, with BOX)
+    int cin = 0;    // BOX: certain inliers among the pixels this warp classified
+    if constexpr (BOX) {
+        float x0 = CUDART_INF_F, x1 = -CUDART_INF_F, y0 = CUDART_INF_F, y1 = -CUDART_INF_F;
+        bool unb = false;
+#pragma unroll
+        for (int j = 0; j < HPT; ++j) {
+            if (hbase + j * TEAM < nh) {
+                x0 = fminf(x0, hxc[j]); x1 = fmaxf(x1, hxc[j]); y0 = fminf(y0, hyc[j]); y1 = fmaxf(y1, hyc[j]);
+                unb |= !(dl[j] < CUDART_INF_F);
+            }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            x0 = fminf(x0, __shfl_xor_sync(0xffffffffu, x0, o)); x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, o));
+            y0 = fminf(y0, __shfl_xor_sync(0xffffffffu, y0, o)); y1 = fmaxf(y1, __shfl_xor_sync(0xffffffffu, y1, o));
+        }
+        // the box's guard band: hyp_frame's at the corner of largest |h-o|_1
+        const float S = fmaxf(fabsf(x0), fabsf(x1)) + fmaxf(fabsf(y0), fabsf(y1)) + cmax;
+        float d = fmaxf(p.cone.band * S, p.cone.floor);
+        if (__any_sync(0xffffffffu, unb) || !(d < CUDART_INF_F)) d = CUDART_INF_F;
+        int base = 0;
+#pragma unroll
+        for (int r = 0; r < PPT; ++r) {
+            const int i = tid + r * NT;
+            float4 ra = make_float4(0.f, 0.f, 0.f, 0.f);
+            float2 rb = make_float2(0.f, 0.f);
+            int cls = -1;   // beyond the tile: nothing to score
+            if (i < n) { ra = s_a[i]; rb = s_b[i]; cls = box_class(ra, rb, x0, x1, y0, y1, d); }
+            const unsigned um = __ballot_sync(0xffffffffu, cls == 0);
+            cin += __popc(__ballot_sync(0xffffffffu, cls == 1));
+            if (lane == 0) s_nu[r][warp] = __popc(um);
+            // every read of this round's records comes before the barrier.  The round's writes below go to slots below
+            // (r+1)*NT, which no later round reads
+            __syncthreads();
+            int off = base;
+#pragma unroll
+            for (int w = 0; w < NW; ++w) {
+                const int c = s_nu[r][w];
+                off += (w < warp) ? c : 0;
+                base += c;
+            }
+            if (cls == 0) {
+                const int o = off + __popc(um & ((1u << lane) - 1u));
+                s_a[o] = ra; s_b[o] = rb; s_idx[o] = (uint16_t)i;
+            }
+        }
+        nl = base;
+        if (p.stats) {   // tooling (pvb_set_pass1_stats): off in production
+            if (lane == 0) atomicAdd(p.stats, (unsigned long long)cin * nh);
+            if (tid == 0) { atomicAdd(p.stats + 1, (unsigned long long)(n - nl) * nh); atomicAdd(p.stats + 2, (unsigned long long)nl * nh); }
+        }
+        const int pad = (nl + VOTE_BLOCK - 1) / VOTE_BLOCK * VOTE_BLOCK - nl;
+        if (tid < pad) { s_a[nl + tid] = make_float4(0.f, 0.f, -1e30f, 0.f); s_b[nl + tid] = make_float2(0.f, 0.f); }
+        __syncthreads();
+    }
+    const int nlpad = (nl + VOTE_BLOCK - 1) / VOTE_BLOCK * VOTE_BLOCK;
+
     const uint32_t sa0 = (uint32_t)__cvta_generic_to_shared(s_a);
     const uint32_t sb0 = (uint32_t)__cvta_generic_to_shared(s_b);
     int mine = 0;   // pixels (padding included) this team has scored
-    for (int i0 = team * VOTE_BLOCK; i0 < npad; i0 += TEAMS * VOTE_BLOCK) {
+    for (int i0 = team * VOTE_BLOCK; i0 < nlpad; i0 += TEAMS * VOTE_BLOCK) {
         mine += VOTE_BLOCK;
         const uint32_t sa = sa0 + (uint32_t)i0 * 16u, sb = sb0 + (uint32_t)i0 * 8u;
         float mn[HPT];   // smallest |margin| of each hypothesis over this block
@@ -271,12 +357,13 @@ vote_kernel(const VoteK p)
             // rare, warp-cooperative: for every (lane, j) whose block has a margin inside the guard band, 16 lanes
             // re-test one pixel each against that hypothesis with the reference's exact operation sequence; the
             // reduced correction goes back to the owning lane (fast verdict = sign bit of m)
-            const int nb = min(VOTE_BLOCK, n - i0);      // padding stays "not an inlier"
+            const int nb = min(VOTE_BLOCK, nl - i0);     // padding stays "not an inlier"
             float4 ra = make_float4(0.f, 0.f, -1e30f, 0.f);
             float2 rb = make_float2(0.f, 0.f), vv = make_float2(0.f, 0.f), cc = make_float2(0.f, 0.f);
             if (lane < nb) {
+                const int px = BOX ? (int)s_idx[i0 + lane] : i0 + lane;
                 ra = s_a[i0 + lane]; rb = s_b[i0 + lane];
-                vv = __ldg(dk + i0 + lane); cc = __ldg(xy + i0 + lane);
+                vv = __ldg(dk + px); cc = __ldg(xy + px);
             }
 #pragma unroll
             for (int j = 0; j < HPT; ++j) {
@@ -306,7 +393,7 @@ vote_kernel(const VoteK p)
 #pragma unroll
     for (int j = 0; j < HPT; ++j) {
         const int s = hbase + j * TEAM;
-        const int cnt = mine - neg[j];
+        const int cnt = mine - neg[j] + cin;
         if (s < nh && cnt) atomicAdd(counts + (lst ? __ldcg(lst + s) : s), cnt);
     }
 }
@@ -347,6 +434,12 @@ static std::atomic<int> g_vote_variant{0};
 
 void set_vote_tuning(int variant) { g_vote_variant.store(variant, std::memory_order_relaxed); }
 
+// Tooling: pass 1's per-box test counts (VoteK::stats), summed into a device buffer of 3 words while it is set.  Atomic:
+// may be set while other host threads launch.
+static std::atomic<unsigned long long *> g_pass1_stats{nullptr};
+
+void set_pass1_stats(unsigned long long *dev) { g_pass1_stats.store(dev, std::memory_order_relaxed); }
+
 cudaError_t launch_vote(const VoteArgs &a, bool zero_counts, bool chained, cudaStream_t st)
 {
     if (zero_counts) {     // callers that did not run generate_kernel (which zeroes the counts it creates hypotheses for)
@@ -358,13 +451,14 @@ cudaError_t launch_vote(const VoteArgs &a, bool zero_counts, bool chained, cudaS
     p.cone = make_cone(a.thresh);
     p.list = nullptr;
     p.len = nullptr;
+    p.stats = nullptr;
     const int variant = g_vote_variant.load(std::memory_order_relaxed);
     cudaError_t e = cudaSuccess;
 #define PVB_VOTE(HPT, NT, MINB, TILE, WS)                                               \
     do {                                                                                \
         const int slices = (a.hn + (HPT) * (WS) * 32 - 1) / ((HPT) * (WS) * 32);        \
         dim3 g((a.cap + (TILE) - 1) / (TILE), a.K * slices, a.B);                       \
-        e = launch_chained(chained, vote_kernel<HPT, NT, MINB, TILE, WS>, g, NT, 0, st, p); \
+        e = launch_chained(chained, vote_kernel<HPT, NT, MINB, TILE, WS, false>, g, NT, 0, st, p); \
     } while (0)
     if (a.hn <= 32) PVB_VOTE(1, 128, 8, 512, 1);
     else if (a.hn <= 64) PVB_VOTE(2, 128, 8, 512, 1);
@@ -513,7 +607,8 @@ cudaError_t launch_vote_list(const VoteArgs &a, const int *list, const int *len,
 }
 
 // Pass 1: vote_kernel over a full list, in (HPT*32)-hypothesis slices (WS = 1) whose four warps split the 1024-pixel tile.
-// With a whole slice per list it scores faster than vote_list_kernel (H100, cfg-2: 192 against 238 us).
+// With a whole slice per list it scores faster than vote_list_kernel (H100, cfg-2: 192 against 238 us).  BOX: each tile's
+// pixels are classified once against the box of the list (box_class); the model predicts 2.1x fewer instructions at cfg-2.
 cudaError_t launch_vote_list_slices(const VoteArgs &a, const int *list, const int *len, int max_len, cudaStream_t st)
 {
     constexpr int HPT = 4, NT = 128, TILE = 1024;
@@ -524,9 +619,10 @@ cudaError_t launch_vote_list_slices(const VoteArgs &a, const int *list, const in
     p.cone = make_cone(a.thresh);
     p.list = list;
     p.len = len;
+    p.stats = g_pass1_stats.load(std::memory_order_relaxed);
     const int slices = (max_len + HPT * 32 - 1) / (HPT * 32);
     dim3 g((a.cap + TILE - 1) / TILE, a.K * slices, a.B);
-    return launch_chained(true, vote_kernel<HPT, NT, 8, TILE, 1>, g, NT, 0, st, p);
+    return launch_chained(true, vote_kernel<HPT, NT, 8, TILE, 1, true>, g, NT, 0, st, p);
 }
 
 // Multi-GPU exchange tail shared by the refit and the covariance kernel: one thread stores NV floats of unit `bk` into every

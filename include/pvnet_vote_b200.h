@@ -710,6 +710,10 @@ PVB_API int pvb_profile_enable(int32_t every);
  *   vote_variant pixel tile of the vote kernel above 256 hypotheses per keypoint: 0 = 1 = 1024 pixels (default),
  *                2 = 256, 3 = 512; up to 256 hypotheses the tile is always 512 */
 PVB_API int pvb_set_tuning(int32_t gather_mode, int32_t vote_variant);
+/* Pass 1's per-box test counts (tooling, DESIGN.md 4.2; process-wide, atomic, results do not depend on it): while
+ * dev_counts (device memory, 3 zeroed uint64) is set, pass 1 of the pruned vote adds to it the tests it resolved per box
+ * as inliers, all tests it resolved per box, and the tests it scored one hypothesis at a time.  NULL turns it off. */
+PVB_API int pvb_set_pass1_stats(void *dev_counts);
 /* Grouped launch of the pruned v3 entries (pvb_ransac_voting_v3, _push, pvb_decode_v3; DESIGN.md 4.4): a call whose every
  * group still prunes runs as up to max_groups groups of consecutive images on `streams` internal streams of the calling
  * host thread, joined back into the caller's stream before the entry returns.  0 = the default (2 groups, 2 streams);
