@@ -11,9 +11,7 @@ is labelled a bound, not a measurement.
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 import torch
@@ -23,14 +21,9 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import clean_pvnet_b200 as pvb  # noqa: E402
 import crop_cases as cc  # noqa: E402
+from devtime import card_line, device_ms, host_ms  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12          # H100 SXM data sheet
-
-
-def gpu_info():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
 
 
 def host_path(imgs, boxes, index, size, scale_ratio, box_ratio):
@@ -65,7 +58,7 @@ def main():
     rng = np.random.default_rng(2026)
     imgs_h = cc.random_images(rng, 4)
     imgs = torch.from_numpy(imgs_h).cuda()
-    info = gpu_info()
+    info = card_line()
     results = []
     for size, scale_ratio, box_ratio in cc.CONFIGS.values():
         for n in (1, 16, 256):
@@ -73,25 +66,13 @@ def main():
             index = rng.integers(0, len(imgs_h), n)
             bd = torch.from_numpy(boxes).cuda()
             ix = torch.from_numpy(index).cuda()
-            for _ in range(5):
-                pvb.crop_inputs(imgs, bd, ix, size, scale_ratio, box_ratio)
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(args.reps):
-                pvb.crop_inputs(imgs, bd, ix, size, scale_ratio, box_ratio)
-            e1.record()
-            torch.cuda.synchronize()
-            dev_ms = e0.elapsed_time(e1) / args.reps
+            dev_ms = device_ms(lambda: pvb.crop_inputs(imgs, bd, ix, size, scale_ratio, box_ratio), args.reps, 5)
             host_path(imgs_h, boxes[:1], index[:1], size, scale_ratio, box_ratio)      # warm cv2 and the copy path
-            hreps = max(1, min(args.reps, 2000 // n))
-            t0 = time.perf_counter()
-            for _ in range(hreps):
-                host_path(imgs_h, boxes, index, size, scale_ratio, box_ratio)
-            host_ms = (time.perf_counter() - t0) * 1e3 / hreps
+            host = host_ms(lambda: host_path(imgs_h, boxes, index, size, scale_ratio, box_ratio),
+                           reps=max(1, min(args.reps, 2000 // n)), warmup=0)
             written = n * 3 * size[0] * size[1] * 4
             r = {"gpu": info, "input": f"{size[0]}x{size[1]}", "n": n, "device_ms": round(dev_ms, 4),
-                 "host_per_box_path_ms": round(host_ms, 3), "speedup": round(host_ms / dev_ms, 1),
+                 "host_per_box_path_ms": round(host, 3), "speedup": round(host / dev_ms, 1),
                  "written_bytes": written, "write_bound_ms": round(written / HBM_BYTES_PER_S * 1e3, 4),
                  "write_bound_share": round(written / HBM_BYTES_PER_S * 1e3 / dev_ms, 3)}
             print(json.dumps(r), flush=True)

@@ -11,7 +11,6 @@ and max SM clock in the same run:
 import argparse
 import json
 import os
-import subprocess
 import sys
 import types
 
@@ -24,30 +23,9 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import clean_pvnet_b200 as pvb  # noqa: E402
 import crop_cases as cc  # noqa: E402
 import ct_decode_cases as dc  # noqa: E402
+from devtime import card_line, device_ms  # noqa: E402
 
 SHAPES = [(1, 1, (136, 184)), (1, 30, (136, 184)), (16, 1, (136, 184)), (32, 30, (104, 128))]
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           stdout=subprocess.PIPE, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:                                 # noqa: BLE001
-        q = f"nvidia-smi unavailable: {e}"
-    return q
-
-
-def timed(fn, iters, warmup=20):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    b.synchronize()
-    return a.elapsed_time(b) / iters * 1e3           # us per call
 
 
 def stand_in_res():
@@ -66,14 +44,14 @@ def main():
     ap.add_argument("--iters", type=int, default=200)
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
-    out = {"card": card(), "decode": [], "chain": None}
+    out = {"card": card_line(), "decode": [], "chain": None}
     print("card:", out["card"])
     rng = np.random.default_rng(0)
     for B, C, hw in SHAPES:
         lg = torch.from_numpy(dc.blobs(rng, B, C, *hw, noise=0.3)).cuda()
         wh = torch.from_numpy(dc._wh(rng, B, *hw)).cuda()
-        t_torch = timed(lambda: dc.restate_decode(lg, wh, 100), args.iters)
-        t_fused = timed(lambda: pvb.decode_detections(lg, wh), args.iters)
+        t_torch = device_ms(lambda: dc.restate_decode(lg, wh, 100), args.iters, 20) * 1e3
+        t_fused = device_ms(lambda: pvb.decode_detections(lg, wh), args.iters, 20) * 1e3
         bound = lg.numel() * 4 / 3.35e12 * 1e6
         row = {"B": B, "C": C, "H": hw[0], "W": hw[1], "torch_us": round(t_torch, 2), "fused_us": round(t_fused, 2),
                "logit_read_bound_us": round(bound, 3)}
@@ -101,8 +79,8 @@ def main():
             batch = {'meta': {'center': meta_c[b:b + 1], 'scale': meta_s[b:b + 1]}, 'inp': inp0}
             pvb.crop.cascade_crop(imgs[b:b + 1], None, batch, {'detection': det})
 
-    out["chain"] = {"B": B, "C": 30, "batched_us": round(timed(chain, max(20, args.iters // 4)), 1),
-                    "per_image_host_sync_us": round(timed(per_image, max(5, args.iters // 20), warmup=3), 1)}
+    out["chain"] = {"B": B, "C": 30, "batched_us": round(device_ms(chain, max(20, args.iters // 4), 20) * 1e3, 1),
+                    "per_image_host_sync_us": round(device_ms(per_image, max(5, args.iters // 20), 3) * 1e3, 1)}
     print(json.dumps(out["chain"]))
     if args.json:
         os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)

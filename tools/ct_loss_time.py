@@ -10,7 +10,6 @@ a lower bound on their time, and the bytes per batch each form sends through the
 limit and SM clock beside the numbers."""
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -19,31 +18,11 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 import clean_pvnet_b200 as pvb  # noqa: E402
+from devtime import card_line, device_ms  # noqa: E402
 
 HBM_BPS = 3.35e12
 C, M = 30, 20
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:        # the numbers below stand without it, but say so
-        q = f"(nvidia-smi unavailable: {e})"
-    return q
-
-
-def per_call_ms(fn, reps=50):
-    for _ in range(5):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
+REPS, WARMUP = 50, 5           # per timing: calls in the event window, calls before it
 
 
 def focal_loss(logits, gt):
@@ -81,12 +60,12 @@ def run(B, H, W):
     want = torch.autograd.grad(focal_loss(x, dense_d), x)[0]
     r = {"B": B, "C": C, "H": H, "W": W, "M": M, "grad_bit_equal": bool(torch.equal(got, want)),
          "loss_fused": float(pvb.ct_focal_loss(x.detach(), *objs)), "loss_torch": float(focal_loss(x.detach(), dense_d))}
-    r["ref_h2d_ms"] = per_call_ms(lambda: dense_d.copy_(dense_h, non_blocking=True))
-    r["ref_fwd_ms"] = per_call_ms(lambda: focal_loss(x.detach(), dense_d))
-    r["ref_fwd_bwd_ms"] = per_call_ms(lambda: torch.autograd.grad(focal_loss(x, dense_d), x))
-    r["fused_fwd_ms"] = per_call_ms(lambda: pvb.ct_focal_loss(x.detach(), *objs))
-    r["fused_fwd_bwd_ms"] = per_call_ms(lambda: torch.autograd.grad(pvb.ct_focal_loss(x, *objs), x))
-    r["target_kernel_ms"] = per_call_ms(lambda: pvb.ct_target_batch(*objs, C, H, W))
+    r["ref_h2d_ms"] = device_ms(lambda: dense_d.copy_(dense_h, non_blocking=True), REPS, WARMUP)
+    r["ref_fwd_ms"] = device_ms(lambda: focal_loss(x.detach(), dense_d), REPS, WARMUP)
+    r["ref_fwd_bwd_ms"] = device_ms(lambda: torch.autograd.grad(focal_loss(x, dense_d), x), REPS, WARMUP)
+    r["fused_fwd_ms"] = device_ms(lambda: pvb.ct_focal_loss(x.detach(), *objs), REPS, WARMUP)
+    r["fused_fwd_bwd_ms"] = device_ms(lambda: torch.autograd.grad(pvb.ct_focal_loss(x, *objs), x), REPS, WARMUP)
+    r["target_kernel_ms"] = device_ms(lambda: pvb.ct_target_batch(*objs, C, H, W), REPS, WARMUP)
     n = B * C * H * W
     r["fused_fwd_hbm_bytes"] = 4 * n
     r["fused_fwd_bwd_hbm_bytes"] = 3 * 4 * n
@@ -98,7 +77,7 @@ def run(B, H, W):
 
 def main():
     assert torch.cuda.is_available(), "ct_loss_time.py measures on a CUDA device"
-    print(f"card: {card()}  torch {torch.__version__}")
+    print(f"card: {card_line()}  torch {torch.__version__}")
     for H, W in ((104, 128), (136, 184)):
         for B in (4, 32):
             r = run(B, H, W)

@@ -21,7 +21,6 @@ import argparse
 import ctypes
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -30,34 +29,12 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import torch  # noqa: E402
 import clean_pvnet_b200 as pvb  # noqa: E402
 import dcn_cases as dc  # noqa: E402
+from devtime import card, device_ms  # noqa: E402
 
 REF_LIB = os.path.join(ROOT, "oracle", "_ref", "libdcn_ref.so")
 PEAK_FP32 = 67e12
 DEV = "cuda:0"
-
-
-def _smi():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader",
-                              "-i", "0"], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True,
-                             timeout=30).stdout.strip()
-        name, power, clock = (s.strip() for s in out.splitlines()[0].split(","))
-        return dict(name=name, power_limit=power, max_sm_clock=clock)
-    except Exception as e:
-        return dict(error=str(e))
-
-
-def _time_ms(fn, reps):
-    for _ in range(2):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
+WARMUP = 2
 
 
 class RefAlgo:
@@ -125,7 +102,7 @@ def main():
                           padding=1, mask=torch.ones((1, 9, 3, 3), device=DEV))
     except Exception:
         tvo = None
-    result = dict(gpu=_smi(), peak_fp32_tflops=PEAK_FP32 / 1e12, configs=[])
+    result = dict(gpu=card(), peak_fp32_tflops=PEAK_FP32 / 1e12, configs=[])
     for key, B in (("544x736", 1), ("512x512", 1), ("512x512", 16)):
         rows, tot = [], {}
         for layer, c0 in enumerate(dc.DETECTOR[key]):
@@ -134,18 +111,19 @@ def main():
             go = torch.randn((B, c.Co) + dc.out_hw(c), device=DEV)
             flop = 2.0 * c.Co * c.C * c.kh * c.kw * c.H * c.W * B
             st = (c.stride, c.pad, c.dil, c.dg)
-            t = dict(ours_fwd=_time_ms(lambda: pvb.dcn.dcn_forward(x, off, m, w, b, *st), args.reps),
-                     ours_fwd_bwd=_time_ms(lambda: (pvb.dcn.dcn_forward(x, off, m, w, b, *st),
-                                                    pvb.dcn.dcn_backward(x, off, m, w, b, go, *st)), args.reps))
+            t = dict(ours_fwd=device_ms(lambda: pvb.dcn.dcn_forward(x, off, m, w, b, *st), args.reps, WARMUP),
+                     ours_fwd_bwd=device_ms(lambda: (pvb.dcn.dcn_forward(x, off, m, w, b, *st),
+                                                     pvb.dcn.dcn_backward(x, off, m, w, b, go, *st)), args.reps, WARMUP))
             if ref is not None:
-                t["ref_fwd"] = _time_ms(lambda: ref.forward(c, x, off, m, w, b), args.reps)
-                t["ref_fwd_bwd"] = _time_ms(lambda: (ref.forward(c, x, off, m, w, b),
-                                                     ref.backward(c, x, off, m, w, b, go)), args.reps)
+                t["ref_fwd"] = device_ms(lambda: ref.forward(c, x, off, m, w, b), args.reps, WARMUP)
+                t["ref_fwd_bwd"] = device_ms(lambda: (ref.forward(c, x, off, m, w, b),
+                                                      ref.backward(c, x, off, m, w, b, go)), args.reps, WARMUP)
             if tvo is not None:
                 xs, offs, ms, ws, bs = (v.clone().requires_grad_() for v in (x, off, m, w, b))
-                t["tv_fwd"] = _time_ms(lambda: tvo.deform_conv2d(x, off, w, b, padding=1, mask=m), args.reps)
-                t["tv_fwd_bwd"] = _time_ms(lambda: torch.autograd.grad(
-                    tvo.deform_conv2d(xs, offs, ws, bs, padding=1, mask=ms), (xs, offs, ms, ws, bs), go), args.reps)
+                t["tv_fwd"] = device_ms(lambda: tvo.deform_conv2d(x, off, w, b, padding=1, mask=m), args.reps, WARMUP)
+                t["tv_fwd_bwd"] = device_ms(lambda: torch.autograd.grad(
+                    tvo.deform_conv2d(xs, offs, ws, bs, padding=1, mask=ms), (xs, offs, ms, ws, bs), go),
+                    args.reps, WARMUP)
             row = dict(layer=layer, C=c.C, H=c.H, W=c.W, C_out=c.Co, gflop_fwd=flop / 1e9,
                        **{k: round(v, 4) for k, v in t.items()},
                        ours_fwd_tflops=round(flop / t["ours_fwd"] / 1e9, 2),
@@ -159,7 +137,7 @@ def main():
         tot["ours_fwd_share_of_peak"] = round(tot["gflop_fwd"] * 1e9 / (tot["ours_fwd"] * 1e-3) / PEAK_FP32, 4)
         tot["ours_fwd_bwd_share_of_peak"] = round(3 * tot["gflop_fwd"] * 1e9 / (tot["ours_fwd_bwd"] * 1e-3) / PEAK_FP32, 4)
         result["configs"].append(dict(input=key, B=B, layers=rows, sum=tot))
-    result["gpu_after"] = _smi()
+    result["gpu_after"] = card()
     text = json.dumps(result)
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)

@@ -5,6 +5,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import clean_pvnet_b200 as pvb
 from clean_pvnet_b200 import synth
+from devtime import device_ms
 
 mask, vertex, _ = synth.make_inputs("cfg2", device="cuda", seed=1236)
 mh, vh = mask.cpu().pin_memory(), vertex.cpu().pin_memory()
@@ -15,10 +16,7 @@ for zc in ("auto", "inplace", "staged"):
         for i in range(3):
             o = pvb.ransac_voting_layer_v3_host(mh, vh, 512, inlier_thresh=0.99, seed=3, chunk_images=chunk, out=oh, mode=zc)
         ok = bool(torch.equal(o, ref))
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for i in range(20):
-            pvb.ransac_voting_layer_v3_host(mh, vh, 512, inlier_thresh=0.99, seed=100 + i, chunk_images=chunk, out=oh, mode=zc)
-        e1.record(); torch.cuda.synchronize()
-        print(f"mode={zc} chunk={chunk:2d}  {e0.elapsed_time(e1)/20:.3f} ms/step  same_as_device={ok}")
+        seeds = iter(range(100, 120))
+        ms = device_ms(lambda: pvb.ransac_voting_layer_v3_host(mh, vh, 512, inlier_thresh=0.99, seed=next(seeds),
+                                                               chunk_images=chunk, out=oh, mode=zc), 20, 0)
+        print(f"mode={zc} chunk={chunk:2d}  {ms:.3f} ms/step  same_as_device={ok}")

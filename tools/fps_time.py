@@ -16,7 +16,6 @@ indices must equal the reference's (or, without the reference build, the numpy r
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -27,30 +26,9 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 import clean_pvnet_b200 as pvb  # noqa: E402
 import fps_cases  # noqa: E402
+from devtime import card, device_ms  # noqa: E402
 
 SHAPES = ((5000, 8), (100000, 8), (1000000, 8), (100000, 64), (100000, 1024))
-
-
-def _smi(field):
-    try:
-        out = subprocess.run(["nvidia-smi", f"--query-gpu={field}", "--format=csv,noheader,nounits", "-i", "0"],
-                             stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, timeout=30).stdout.strip()
-        return out.splitlines()[0]
-    except Exception:
-        return None
-
-
-def _events_us(fn, reps):
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps * 1e3
 
 
 def _ref_us(lib, clouds, sn, reps):
@@ -73,7 +51,8 @@ def main():
     dev = torch.device("cuda", 0)
     lib = fps_cases.ref_lib()
     rng = np.random.default_rng(0)
-    res = dict(gpu=torch.cuda.get_device_name(dev), power_limit_w=_smi("power.limit"),
+    cd = card()
+    res = dict(gpu=cd["name"], power_limit_w=cd["power_limit_w"], sm_clock_max_mhz=cd["sm_clock_max_mhz"],
                reference="libfps_ref.so" if lib is not None else "not measured", rows=[])
     rows = [(f"{pn} points, sn {sn}", [rng.standard_normal((pn, 3)).astype(np.float32)], sn) for pn, sn in SHAPES]
     counts = np.linspace(2000, 60000, 30).astype(np.int32)
@@ -87,7 +66,7 @@ def main():
         x = torch.from_numpy(pad).to(dev)
         cnt = np.array([len(c) for c in clouds], np.int32)
         reps = max(3, min(args.reps, int(2e6 // (n * sn) + 3)))
-        us = _events_us(lambda: pvb.farthest_point_sampling_batch(x, sn, counts=cnt), reps)
+        us = device_ms(lambda: pvb.farthest_point_sampling_batch(x, sn, counts=cnt), reps, 3) * 1e3
         got = pvb.farthest_point_sampling_batch(x, sn, counts=cnt).cpu().numpy()
         row = dict(shape=name, clouds=len(clouds), points=int(cnt.sum()), sn=sn, device_us=us, device_reps=reps)
         if lib is not None:

@@ -10,7 +10,6 @@ import argparse
 import json
 import os
 import re
-import subprocess
 import sys
 import tempfile
 
@@ -37,6 +36,7 @@ def main():
     import torch
     import clean_pvnet_b200 as pvb
     from clean_pvnet_b200 import _lib, synth
+    from devtime import card_line
     if not torch.cuda.is_available():
         raise SystemExit("group_overlap.py needs a CUDA device")
     lib = _lib.load()
@@ -72,9 +72,7 @@ def main():
         s = stats.setdefault(name, [0, 0.0, 0.0])
         s[0] += 1; s[1] += t1 - t0; s[2] += under
     span = (max(k[3] for k in kern) - min(k[2] for k in kern)) / STEPS
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
-                         stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True).stdout.strip()
-    print(f"{smi}; {args.workload}, groups <= {args.groups or 'default'}, streams {args.streams or 'default'}; "
+    print(f"{card_line()}; {args.workload}, groups <= {args.groups or 'default'}, streams {args.streams or 'default'}; "
           f"{STEPS} profiled steps, {span:.1f} us of kernels per step (first start to last end)")
     print(f"{'kernel':<28} {'per step':>8} {'mean us':>8} {'under pass 1':>13}")
     first = {}

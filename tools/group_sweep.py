@@ -6,6 +6,7 @@ so that clock drift hits them alike; prints the median and range of ms per step 
     python tools/group_sweep.py [--workload cfg2|cfg4] [--settings 1x1 2x2 4x2 ...] [--steps 200] [--reps 3]
 """
 import argparse
+import itertools
 import os
 import sys
 
@@ -24,6 +25,7 @@ def main():
     import torch
     import clean_pvnet_b200 as pvb
     from clean_pvnet_b200 import _lib, synth
+    from devtime import card_line, device_ms
     if not torch.cuda.is_available():
         raise SystemExit("group_sweep.py needs a CUDA device")
     lib = _lib.load()
@@ -33,18 +35,11 @@ def main():
     for rep in range(args.reps):
         for g, s in settings:
             _lib.check(lib.pvb_set_group_tuning(g, s))
-            for i in range(10):
-                pvb.ransac_voting_layer_v3(mask, vertex, 512, inlier_thresh=0.99, seed=i)
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for i in range(args.steps):
-                pvb.ransac_voting_layer_v3(mask, vertex, 512, inlier_thresh=0.99, seed=1000 + i)
-            e1.record()
-            torch.cuda.synchronize()
-            times[(g, s)].append(e0.elapsed_time(e1) / args.steps)
+            seeds = itertools.chain(range(10), range(1000, 1000 + args.steps))      # warm-up seeds, then timed ones
+            times[(g, s)].append(device_ms(lambda: pvb.ransac_voting_layer_v3(mask, vertex, 512, inlier_thresh=0.99,
+                                                                              seed=next(seeds)), args.steps, 10))
     _lib.check(lib.pvb_set_group_tuning(0, 0))
-    print(f"{args.workload} on {torch.cuda.get_device_name()}: ms per step, median [min, max] of {args.reps}")
+    print(f"{args.workload} on {card_line()}: ms per step, median [min, max] of {args.reps}")
     for (g, s), t in times.items():
         t = sorted(t)
         print(f"  groups <= {g:2d}, streams {s}: {t[len(t) // 2]:.4f} [{t[0]:.4f}, {t[-1]:.4f}]")

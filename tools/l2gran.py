@@ -13,6 +13,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import clean_pvnet_b200 as pvb
 from clean_pvnet_b200 import _lib, synth
+from devtime import device_ms
 
 gran = int(sys.argv[1]) if len(sys.argv) > 1 else 0
 torch.cuda.init()
@@ -31,11 +32,8 @@ for i in range(3):
     pvb.ransac_voting_layer_v3(mask, vertex, 512, inlier_thresh=0.99, seed=i)
 torch.cuda.synchronize()
 lib.pvb_profile_reset(); lib.pvb_profile_enable(1)
-e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-e0.record()
-for i in range(20):
-    pvb.ransac_voting_layer_v3(mask, vertex, 512, inlier_thresh=0.99, seed=100 + i)
-e1.record(); torch.cuda.synchronize()
+seeds = iter(range(100, 120))
+ms = device_ms(lambda: pvb.ransac_voting_layer_v3(mask, vertex, 512, inlier_thresh=0.99, seed=next(seeds)), 20, 0)
 st = (ctypes.c_double * 4)()
 n = lib.pvb_profile_read(st, 4)
-print(f"gran={cur.value} step {e0.elapsed_time(e1)/20:.4f} ms  select {st[0]/n:.4f} generate {st[1]/n:.4f} vote {st[2]/n:.4f} refit {st[3]/n:.4f}")
+print(f"gran={cur.value} step {ms:.4f} ms  select {st[0]/n:.4f} generate {st[1]/n:.4f} vote {st[2]/n:.4f} refit {st[3]/n:.4f}")

@@ -13,7 +13,6 @@ SXM data sheet's 3.35 TB/s.
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -28,26 +27,9 @@ import clean_pvnet_b200 as pvb                         # noqa: E402
 from clean_pvnet_b200.render import _compose           # noqa: E402
 from tless_mask_cases import compose_restated           # noqa: E402
 from vsd_cases import K_TLESS, icosphere, poses, soup   # noqa: E402
+from devtime import card_line, device_ms                # noqa: E402
 
 W, H = 720, 540
-
-
-def gpu_info():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                              stdout=subprocess.PIPE, text=True, timeout=30).stdout.strip()
-    except Exception as e:             # noqa: BLE001
-        return f"unknown ({e})"
-
-
-def cuda_ms(fn, iters):
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    for _ in range(iters):
-        fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e) / iters
 
 
 def main():
@@ -87,12 +69,11 @@ def main():
 
             def compose():
                 _compose(depth, n, np.arange(n), obj, first, 0, B, H, W, *out, dev)
-            for fn in (batch, render, compose):
+            for fn in (batch, render, compose):            # one warm-up call each, before any window
                 fn()
-            torch.cuda.synchronize()
-            t_batch = cuda_ms(batch, max(2, args.iters // 2))
-            t_render = cuda_ms(render, max(2, args.iters // 2))
-            t_compose = cuda_ms(compose, args.iters)
+            t_batch = device_ms(batch, max(2, args.iters // 2), 0)
+            t_render = device_ms(render, max(2, args.iters // 2), 0)
+            t_compose = device_ms(compose, args.iters, 0)
             # the numpy update_mask loop on the same depths, a few images, per image
             nh = min(B, 4)
             dh = depth[:nh * per].cpu().numpy()
@@ -105,7 +86,7 @@ def main():
                              compose_hbm_bound_ms=bound_ms, numpy_ms_per_image=t_np, numpy_ms_total=t_np * B,
                              visible_pixels=int(out[2].sum()), rendered_pixels=int(out[1].sum())))
             print(json.dumps(rows[-1]))
-    res = dict(gpu=gpu_info(), size=[W, H], faces=[int(m[1].shape[0]) for m in meshes], rows=rows)
+    res = dict(gpu=card_line(), size=[W, H], faces=[int(m[1].shape[0]) for m in meshes], rows=rows)
     print(json.dumps(dict(gpu=res["gpu"], faces=res["faces"])))
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)

@@ -17,17 +17,17 @@ The model sizes pn are ASSUMPTIONS spanning a plausible range: the LINEMOD verte
 """
 import argparse
 import ctypes
+import itertools
 import json
 import os
-import subprocess
 import sys
-import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 import clean_pvnet_b200 as pvb  # noqa: E402
+from devtime import card, card_line, device_ms, host_ms  # noqa: E402
 
 PAIRS = (1, 64, 1024)
 SIZES = (1000, 5000, 20000)          # assumed model vertex counts (see above)
@@ -37,36 +37,11 @@ HBM_BYTES_PER_S = 3.35e12            # H100 SXM data sheet; a bound, not an expe
 K = np.array([[572.4114, 0.0, 325.2611], [0.0, 573.57043, 242.04899], [0.0, 0.0, 1.0]])
 
 
-def _smi():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                              stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, timeout=30).stdout.strip()
-    except Exception as e:
-        return f"nvidia-smi failed: {e}"
-
-
-def _events_us(fn, reps):
-    for i in range(5):
-        fn(i)
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for i in range(reps):
-        fn(i)
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps * 1e3
-
-
-def _host_us(fn, min_s=0.2):
-    fn()
-    reps, t0 = 0, time.perf_counter()
-    while True:
-        fn()
-        reps += 1
-        dt = time.perf_counter() - t0
-        if dt >= min_s:
-            return dt / reps * 1e6
+def _device_us(fn, reps):
+    """devtime.device_ms of fn(i), 5 warm-up calls: i counts 0..4 over the warm-up, then again 0..reps-1 over the
+    timed calls, so the timed calls start from the first input copy."""
+    i = itertools.chain(range(5), range(reps))
+    return device_ms(lambda: fn(next(i)), reps, 5) * 1e3
 
 
 def _poses(rng, n):
@@ -110,10 +85,11 @@ def main():
     lib = pvb._lib.load()
     dev = torch.device("cuda", 0)
     stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-    res = dict(gpu=torch.cuda.get_device_name(dev), nvidia_smi_power_limit_and_max_sm_clock=_smi(),
+    cd = card()
+    res = dict(gpu=cd["name"], power_limit_w=cd["power_limit_w"], sm_clock_max_mhz=cd["sm_clock_max_mhz"],
                sizes_are_assumptions=True, pose=[], mask=[])
     rng = np.random.default_rng(0)
-    lines = [f"GPU: {res['gpu']}; power.limit, clocks.max.sm: {res['nvidia_smi_power_limit_and_max_sm_clock']}", "",
+    lines = [f"GPU: {card_line(cd)}", "",
              "pvb_pose_metrics          device (us)   numpy loop (us)   speed-up"]
     for pn in SIZES:
         model_h = rng.normal(size=(pn, 3)) * [0.05, 0.03, 0.04]
@@ -125,10 +101,10 @@ def main():
             outs = [torch.empty(n, dtype=torch.float64, device=dev) for _ in range(3)]
             nb = lib.pvb_pose_metrics_workspace_bytes(n, pn)
             ws = torch.empty(max(nb, 1), dtype=torch.uint8, device=dev)
-            us = _events_us(lambda i: pvb._lib.check(lib.pvb_pose_metrics(
+            us = _device_us(lambda i: pvb._lib.check(lib.pvb_pose_metrics(
                 model.data_ptr(), pp.data_ptr(), pg.data_ptr(), km.data_ptr(), 0, outs[0].data_ptr(), outs[1].data_ptr(),
                 outs[2].data_ptr(), n, pn, ws.data_ptr(), nb, stream)), args.reps)
-            np_us = _host_us(lambda: _numpy_pose(model_h, pred_h, gt_h))
+            np_us = host_ms(lambda: _numpy_pose(model_h, pred_h, gt_h), warmup=1, min_s=0.2) * 1e3
             res["pose"].append(dict(n=n, pn=pn, device_us=us, numpy_us=np_us))
             lines.append(f"  n={n:5d} pn={pn:6d}   {us:12.1f}   {np_us:15.0f}   {np_us / us:8.0f}x")
     lines += ["", "pvb_mask_iou (int64 pred, uint8 gt, 480x640)   device (us)   GB/s   of 3.35 TB/s   numpy + .cpu() (us)"]
@@ -141,13 +117,13 @@ def main():
         inter = torch.empty(B, dtype=torch.int64, device=dev)
         uni = torch.empty(B, dtype=torch.int64, device=dev)
         st = (ctypes.c_int64 * 3)(H * W, W, 1)
-        us = _events_us(lambda i: pvb._lib.check(lib.pvb_mask_iou(
+        us = _device_us(lambda i: pvb._lib.check(lib.pvb_mask_iou(
             preds[i % copies].data_ptr(), pvb._lib.PVB_MASK_I64, st, gts[i % copies].data_ptr(), pvb._lib.PVB_MASK_U8, st,
             inter.data_ptr(), uni.data_ptr(), B, H, W, stream)), args.reps)
         p0, g0 = preds[(args.reps - 1) % copies].cpu().numpy(), gts[(args.reps - 1) % copies].cpu().numpy()
         assert inter.tolist() == [int((p0[b] & g0[b]).sum()) for b in range(B)]
         assert uni.tolist() == [int((p0[b] | g0[b]).sum()) for b in range(B)]
-        np_us = _host_us(lambda: _numpy_mask(preds[0], gts[0]))
+        np_us = host_ms(lambda: _numpy_mask(preds[0], gts[0]), warmup=1, min_s=0.2) * 1e3
         rate = nbytes / (us * 1e-6)
         res["mask"].append(dict(B=B, bytes=nbytes, device_us=us, bytes_per_s=rate, fraction_of_hbm_datasheet=rate /
                                 HBM_BYTES_PER_S, hbm_bound_us=nbytes / HBM_BYTES_PER_S * 1e6, numpy_with_copies_us=np_us))

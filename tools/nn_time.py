@@ -18,42 +18,19 @@ import argparse
 import ctypes
 import json
 import os
-import subprocess
 import sys
-import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 import clean_pvnet_b200 as pvb  # noqa: E402
+from devtime import card, device_ms, host_ms  # noqa: E402
 
 SIZES = (1000, 5000, 20000)        # assumed model vertex counts (see above)
 BATCHES = (1, 64)
 INSTR_PER_PAIR = 9                 # estimate from SASS, see above
 REF_LIB = os.path.join(ROOT, "oracle", "_ref", "libnn_ref.so")
-
-
-def _smi(field):
-    try:
-        out = subprocess.run(["nvidia-smi", f"--query-gpu={field}", "--format=csv,noheader,nounits", "-i", "0"],
-                             stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, timeout=30).stdout.strip()
-        return float(out.splitlines()[0])
-    except Exception:
-        return None
-
-
-def _events_us(fn, reps):
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps * 1e3
 
 
 def _poses(rng, n):
@@ -75,15 +52,17 @@ def main():
     lib = pvb._lib.load()
     dev = torch.device("cuda", 0)
     props = torch.cuda.get_device_properties(dev)
-    sm_clock_mhz = _smi("clocks.max.sm")
-    bound = props.multi_processor_count * 128 * sm_clock_mhz * 1e6 / INSTR_PER_PAIR if sm_clock_mhz else None
+    cd = card()
+    sm_clock_mhz = cd["sm_clock_max_mhz"]
+    bound = (props.multi_processor_count * 128 * sm_clock_mhz * 1e6 / INSTR_PER_PAIR
+             if isinstance(sm_clock_mhz, float) else None)
     stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
     ref_lib = None
     if os.path.exists(REF_LIB):
         ref_lib = ctypes.CDLL(REF_LIB)
         ref_lib.findNearestPointIdxLauncher.restype = None
         ref_lib.findNearestPointIdxLauncher.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_int] * 5
-    res = dict(gpu=torch.cuda.get_device_name(dev), power_limit_w=_smi("power.limit"), sm_clock_max_mhz=sm_clock_mhz,
+    res = dict(gpu=cd["name"], power_limit_w=cd["power_limit_w"], sm_clock_max_mhz=sm_clock_mhz,
                sms=props.multi_processor_count, sizes_are_assumptions=True,
                fp32_issue_bound_estimate_pairs_per_s=bound, rows=[])
     for pn in SIZES:
@@ -93,18 +72,15 @@ def main():
             idx_h = np.zeros((1, pn), np.int32)
             call = lambda: ref_lib.findNearestPointIdxLauncher(r_h.ctypes.data, q_h.ctypes.data, idx_h.ctypes.data,  # noqa: E731
                                                                1, pn, pn, 3, 0)
-            for _ in range(3):
-                call()                                   # the first call JIT-compiles the reference's compute_52 PTX
-            t0 = time.perf_counter()
-            for _ in range(args.reps):
-                call()
-            row["reference_host_us"] = (time.perf_counter() - t0) / args.reps * 1e6
+            # the warm-up's first call JIT-compiles the reference's compute_52 PTX
+            row["reference_host_us"] = host_ms(call, reps=args.reps, warmup=3) * 1e3
         r, q = torch.from_numpy(r_h).to(dev), torch.from_numpy(q_h).to(dev)
         idx = torch.empty((1, pn), dtype=torch.int32, device=dev)
         nb = lib.pvb_nearest_point_workspace_bytes(1, pn, pn)
         ws = torch.empty(max(nb, 1), dtype=torch.uint8, device=dev)
-        us = _events_us(lambda: pvb._lib.check(lib.pvb_nearest_point_idx(r.data_ptr(), q.data_ptr(), idx.data_ptr(), 1, pn, pn,
-                                                                         3, 0, ws.data_ptr(), nb, stream)), args.reps)
+        us = device_ms(lambda: pvb._lib.check(lib.pvb_nearest_point_idx(r.data_ptr(), q.data_ptr(), idx.data_ptr(), 1, pn,
+                                                                        pn, 3, 0, ws.data_ptr(), nb, stream)),
+                       args.reps, 3) * 1e3
         row["device_us"] = us
         row["device_pairs_per_s"] = pn * pn / (us * 1e-6)
         if ref_lib is not None:
@@ -116,9 +92,9 @@ def main():
             for syn in (1, 0):
                 nb = lib.pvb_add_metric_workspace_bytes(n, pn, syn)
                 w = torch.empty(max(nb, 1), dtype=torch.uint8, device=dev)
-                us = _events_us(lambda: pvb._lib.check(lib.pvb_add_metric(model.data_ptr(), pp.data_ptr(), pg.data_ptr(),
-                                                                          out.data_ptr(), n, pn, syn, w.data_ptr(), nb,
-                                                                          stream)), args.reps)
+                us = device_ms(lambda: pvb._lib.check(lib.pvb_add_metric(model.data_ptr(), pp.data_ptr(), pg.data_ptr(),
+                                                                         out.data_ptr(), n, pn, syn, w.data_ptr(), nb,
+                                                                         stream)), args.reps, 3) * 1e3
                 key = f"add{'s' if syn else ''}_n{n}"
                 row[key + "_us"] = us
                 if syn:

@@ -18,7 +18,6 @@ import argparse
 import json
 import os
 import re
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -27,19 +26,11 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 import clean_pvnet_b200 as pvb  # noqa: E402
 from clean_pvnet_b200 import _lib, synth, ransac_voting_gpu as rv  # noqa: E402
+from devtime import card, card_line  # noqa: E402
 
 HN, THRESH = 512, 0.99          # bench.py's step
 WARMUP, STEPS = 20, 30
 PASS1 = re.compile(r"vote_kernel<4, ?128, ?8, ?1024, ?1(, ?true)?>")
-
-
-def _smi(field):
-    try:
-        out = subprocess.run(["nvidia-smi", f"--query-gpu={field}", "--format=csv,noheader,nounits", "-i", "0"],
-                             stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, timeout=30).stdout.strip()
-        return float(out.splitlines()[0])
-    except Exception:
-        return None
 
 
 def main():
@@ -94,13 +85,14 @@ def main():
         _lib.check(lib.pvb_set_pass1_stats(None))
     s = stats.cpu().numpy().astype(np.float64) / STEPS
     tests = total / STEPS
-    res = dict(gpu=torch.cuda.get_device_name(dev), power_limit_w=_smi("power.limit"), sm_clock_max_mhz=_smi("clocks.max.sm"),
+    cd = card()
+    res = dict(gpu=cd["name"], power_limit_w=cd["power_limit_w"], sm_clock_max_mhz=cd["sm_clock_max_mhz"],
                workload=args.workload, B=B, K=K, hn=HN, thresh=THRESH, groups=args.groups, warmup=WARMUP, steps=STEPS,
                pass1_launches_per_step=len(p1) // STEPS, pass1_us=us, pass1_tests=tests,
                tests_resolved_per_box=float(s[1]) if counters else 0.0,
                tests_resolved_as_inliers=float(s[0]) if counters else 0.0,
                tests_scored=float(s[2]) if counters else tests, per_box_counters=counters)
-    print(f"{res['gpu']}, power limit {res['power_limit_w']} W, max SM clock {res['sm_clock_max_mhz']} MHz; "
+    print(f"{card_line(cd)}; "
           f"{args.workload} (B={B}, K={K}, hn={HN}, t={THRESH}), groups {args.groups or 'default'}, "
           f"mean of {STEPS} steps after {WARMUP} warm-up steps")
     print(f"pass 1: {us:.1f} us per step in {res['pass1_launches_per_step']} launch(es); {tests / 1e6:.1f} M tests, "

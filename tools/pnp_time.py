@@ -16,6 +16,7 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 import clean_pvnet_b200 as pvb  # noqa: E402
 from util import pnp_case  # noqa: E402
+from devtime import device_ms  # noqa: E402
 
 cases = [pnp_case(1000 + s, pn=9, noise=2.0) for s in range(256)]
 so = os.path.join(ROOT, "tests", "_build", "libpnp_host.so")
@@ -34,27 +35,14 @@ cpu_us = (time.perf_counter() - t0) / len(cases) * 1e6
 print(f"host build of the same core, 1 core: {cpu_us:.1f} us per problem (incl. ctypes call)")
 
 
-def per_call_us(fn, reps=20):
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps * 1e3
-
-
 for n in (1, 16, 256, 4096):
     reps = [cases[i % 256] for i in range(n)]
     f = lambda i: torch.from_numpy(np.stack([c[i] for c in reps])).cuda()  # noqa: E731
     uv, p3, W, K, init = f(0), f(1), f(2), f(3), f(4)
     uv32, W32 = uv.float(), W.float()
     _, inf = pvb.uncertainty_pnp_batch(uv, W, p3, K, init, return_info=True)
-    t_batch = per_call_us(lambda: pvb.uncertainty_pnp_batch(uv, W, p3, K, init))
-    t_p3p = per_call_us(lambda: pvb.p3p_init_batch(uv, W, p3, K))
-    t_votes = per_call_us(lambda: pvb.uncertainty_pnp_from_votes(uv32, None, p3, K, init, weights=W32))
+    t_batch = device_ms(lambda: pvb.uncertainty_pnp_batch(uv, W, p3, K, init), 20, 3) * 1e3
+    t_p3p = device_ms(lambda: pvb.p3p_init_batch(uv, W, p3, K), 20, 3) * 1e3
+    t_votes = device_ms(lambda: pvb.uncertainty_pnp_from_votes(uv32, None, p3, K, init, weights=W32), 20, 3) * 1e3
     print(f"n={n:5d}: uncertainty_pnp_batch {t_batch:8.1f} us ({t_batch / n:7.2f} us/problem, mean iterations "
           f"{inf[:, 0].float().mean().item():.2f})  p3p_init_batch {t_p3p:8.1f} us  uncertainty_pnp_from_votes {t_votes:8.1f} us")

@@ -47,6 +47,8 @@ def loop(exchange, sampler_period, profile, reasons_every=1, clock=True):
     torch.cuda.synchronize()
     if smp:
         smp.start()
+    # its own event pair, not devtime.device_ms: the window also holds the host clock around the enqueue and the
+    # exchange's drain, and the clock sampler starts between the synchronise and the first event
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     t0 = time.perf_counter()

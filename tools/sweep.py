@@ -15,6 +15,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
 import clean_pvnet_b200 as pvb  # noqa: E402
 from clean_pvnet_b200 import _lib, synth  # noqa: E402
+from devtime import device_ms  # noqa: E402
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--B", type=int, default=64)
@@ -46,14 +47,10 @@ for name, cfg in cases:
         pvb.ransac_voting_layer_v3(mask, vertex, hn, inlier_thresh=0.99, seed=2 + i)
     torch.cuda.synchronize()
     lib.pvb_profile_reset(); lib.pvb_profile_enable(1)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for i in range(args.steps):
-        pvb.ransac_voting_layer_v3(mask, vertex, hn, inlier_thresh=0.99, seed=10 + i)
-    e1.record(); torch.cuda.synchronize()
+    seeds = iter(range(10, 10 + args.steps))
+    ms = device_ms(lambda: pvb.ransac_voting_layer_v3(mask, vertex, hn, inlier_thresh=0.99, seed=next(seeds)), args.steps, 0)
     st = (ctypes.c_double * 4)()
     n = lib.pvb_profile_read(st, 4); lib.pvb_profile_enable(0)
-    ms = e0.elapsed_time(e1) / args.steps
     stage = [st[i] / n for i in range(4)]
     alg = B * H * W * 8 + tn_sum * K * 8 + B * K * 8
     tests = K * hn * tn_sum

@@ -9,6 +9,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
 import clean_pvnet_b200 as pvb  # noqa: E402
 from clean_pvnet_b200 import _lib, synth  # noqa: E402
+from devtime import device_ms  # noqa: E402
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--cfg", default="cfg2")
@@ -31,13 +32,11 @@ for variant in [int(v) for v in args.variants.split(",")]:
         same = bool(torch.equal(ref, out))
         torch.cuda.synchronize()
         lib.pvb_profile_reset(); lib.pvb_profile_enable(1)
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for i in range(args.steps):
-            pvb.ransac_voting_layer_v3(mask, vertex, args.hn, inlier_thresh=0.99, seed=100 + i)
-        e1.record(); torch.cuda.synchronize()
+        seeds = iter(range(100, 100 + args.steps))
+        step = device_ms(lambda: pvb.ransac_voting_layer_v3(mask, vertex, args.hn, inlier_thresh=0.99, seed=next(seeds)),
+                         args.steps, 0)
         ms = (ctypes.c_double * 4)()
         n = lib.pvb_profile_read(ms, 4)
         lib.pvb_profile_enable(0)
-        print(f"variant={variant} gather={chunk} step={e0.elapsed_time(e1)/args.steps:.4f} ms  "
+        print(f"variant={variant} gather={chunk} step={step:.4f} ms  "
               f"select={ms[0]/n:.4f} gen={ms[1]/n:.4f} vote={ms[2]/n:.4f} refit={ms[3]/n:.4f}  same_result={same}")

@@ -11,7 +11,6 @@ restatement of compute_vertex, tests/vote_target_cases.py, against the compact k
 each form sends through the loader.  Prints the card, its power limit and SM clock beside the numbers."""
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -24,31 +23,11 @@ import torch.nn.functional as F  # noqa: E402
 import clean_pvnet_b200 as pvb  # noqa: E402
 from clean_pvnet_b200.vote_loss import compact_vertex  # noqa: E402
 from vote_target_cases import restate_vertex  # noqa: E402
+from devtime import card_line, device_ms  # noqa: E402
 
 HBM_BPS = 3.35e12
 B, K = 32, 9
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:        # the numbers below stand without it, but say so
-        q = f"(nvidia-smi unavailable: {e})"
-    return q
-
-
-def per_call_ms(fn, reps=30):
-    for _ in range(5):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
+REPS, WARMUP = 30, 5           # per timing: calls in the event window, calls before it
 
 
 def masks(H, W, seed):
@@ -109,13 +88,13 @@ def run(H, W):
     got = torch.autograd.grad(pvb.vote_loss(pred, mask, kpt_d), pred)[0]
     want = torch.autograd.grad(reference_loss(pred, mask, dense_d), pred)[0]
     r = {"H": H, "W": W, "B": B, "K": K, "fill": float(mask_np.mean()), "grad_bit_equal": bool(torch.equal(got, want))}
-    r["ref_h2d_ms"] = per_call_ms(ref_h2d)
-    r["ref_fwd_bwd_ms"] = per_call_ms(ref_loss)
-    r["ref_total_ms"] = per_call_ms(lambda: (ref_h2d(), ref_loss()))
-    r["fused_h2d_ms"] = per_call_ms(fused_h2d)
-    r["fused_fwd_ms"] = per_call_ms(fused_fwd)
-    r["fused_fwd_bwd_ms"] = per_call_ms(fused_loss)
-    r["fused_total_ms"] = per_call_ms(lambda: (fused_h2d(), fused_loss()))
+    r["ref_h2d_ms"] = device_ms(ref_h2d, REPS, WARMUP)
+    r["ref_fwd_bwd_ms"] = device_ms(ref_loss, REPS, WARMUP)
+    r["ref_total_ms"] = device_ms(lambda: (ref_h2d(), ref_loss()), REPS, WARMUP)
+    r["fused_h2d_ms"] = device_ms(fused_h2d, REPS, WARMUP)
+    r["fused_fwd_ms"] = device_ms(fused_fwd, REPS, WARMUP)
+    r["fused_fwd_bwd_ms"] = device_ms(fused_loss, REPS, WARMUP)
+    r["fused_total_ms"] = device_ms(lambda: (fused_h2d(), fused_loss()), REPS, WARMUP)
     hbm = (2 * B * 2 * K * H * W * 4) + (B * 2 * K * H * W * 4) + 2 * B * H * W * mask.element_size()
     r["fused_hbm_bytes"] = hbm
     r["fused_hbm_bound_ms"] = hbm / HBM_BPS * 1e3
@@ -129,7 +108,7 @@ def run(H, W):
 
 def main():
     assert torch.cuda.is_available(), "vote_loss_time.py measures on a CUDA device"
-    print(f"card: {card()}  torch {torch.__version__}")
+    print(f"card: {card_line()}  torch {torch.__version__}")
     for H, W in ((480, 640), (256, 256)):
         r = run(H, W)
         print(json.dumps(r))

@@ -14,7 +14,6 @@ import argparse
 import json
 import os
 import re
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -23,18 +22,10 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 import clean_pvnet_b200 as pvb  # noqa: E402
 from clean_pvnet_b200 import _lib, synth, ransac_voting_gpu as rv  # noqa: E402
+from devtime import card, card_line  # noqa: E402
 
 HN, THRESH = 512, 0.99          # bench.py's step
 WARMUP, STEPS = 20, 30
-
-
-def _smi(field):
-    try:
-        out = subprocess.run(["nvidia-smi", f"--query-gpu={field}", "--format=csv,noheader,nounits", "-i", "0"],
-                             stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, timeout=30).stdout.strip()
-        return float(out.splitlines()[0])
-    except Exception:
-        return None
 
 
 def _kernel_name(name):
@@ -113,7 +104,8 @@ def main():
     for r, t in zip(votes, tests):
         r["tests"] = float(t)
         r["tests_per_s"] = float(t / (r["us"] * 1e-6))
-    res = dict(gpu=torch.cuda.get_device_name(dev), power_limit_w=_smi("power.limit"), sm_clock_max_mhz=_smi("clocks.max.sm"),
+    cd = card()
+    res = dict(gpu=cd["name"], power_limit_w=cd["power_limit_w"], sm_clock_max_mhz=cd["sm_clock_max_mhz"],
                workload=args.workload, B=B, K=K, hn=HN, thresh=THRESH, pruned=pruned, warmup=WARMUP, steps=STEPS,
                kernels=rows)
     if pruned:
@@ -121,7 +113,7 @@ def main():
         last = votes[-1]
         res["vote_stage_us"] = float(sum(r["us"] + r["gap_before_us"] for r in rows[first["launch"]:last["launch"] + 1])
                                      - first["gap_before_us"])
-    print(f"{res['gpu']}, power limit {res['power_limit_w']} W, max SM clock {res['sm_clock_max_mhz']} MHz; "
+    print(f"{card_line(cd)}; "
           f"{args.workload} (B={B}, K={K}, hn={HN}, t={THRESH}), {'full' if not pruned else 'pruned'} vote, "
           f"mean of {STEPS} steps after {WARMUP} warm-up steps")
     print(f"{'#':>2}  {'kernel':<58} {'us':>8} {'gap':>6} {'tests':>10} {'T tests/s':>9}")

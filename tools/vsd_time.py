@@ -11,7 +11,6 @@ per pair) over the H100 SXM data sheet's 3.35 TB/s.
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -25,26 +24,9 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import clean_pvnet_b200 as pvb                       # noqa: E402
 from clean_pvnet_b200.nn import _call, _workspace   # noqa: E402
 from vsd_cases import K_TLESS, icosphere, poses, soup, vsd_restated   # noqa: E402
+from devtime import card_line, device_ms                               # noqa: E402
 
 W, H = 720, 540
-
-
-def gpu_info():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                              stdout=subprocess.PIPE, text=True, timeout=30).stdout.strip()
-    except Exception as e:             # noqa: BLE001
-        return f"unknown ({e})"
-
-
-def cuda_ms(fn, iters):
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    for _ in range(iters):
-        fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e) / iters
 
 
 def main():
@@ -76,12 +58,11 @@ def main():
 
             def vsd():
                 _call("pvb_vsd", dev, dt, B, de, n, 0, gt, n, 0, pairs, n, K, 0, H, W, 15.0, 20.0, e, ws, nbytes)
-            for fn in (render, vsd):
+            for fn in (render, vsd):                       # one warm-up call each, before either window
                 fn()
-            torch.cuda.synchronize()
-            t_render = cuda_ms(render, args.iters)
-            t_vsd = cuda_ms(vsd, args.iters)
-            t_all = cuda_ms(lambda: pvb.vsd_batch(pts, faces, pe, pg, K, dt, pairs), max(2, args.iters // 4))
+            t_render = device_ms(render, args.iters, 0)
+            t_vsd = device_ms(vsd, args.iters, 0)
+            t_all = device_ms(lambda: pvb.vsd_batch(pts, faces, pe, pg, K, dt, pairs), max(2, args.iters // 4), 0)
             # numpy restatement of the evaluator's VSD on the same depths, a few pairs, per pair
             de_h, gt_h, dt_h = de[:4].cpu().numpy(), gt[:4].cpu().numpy(), dt[:4].cpu().numpy()
             t0 = time.perf_counter()
@@ -93,7 +74,7 @@ def main():
                              vsd_ms=t_vsd, vsd_hbm_bound_ms=bound_ms, vsd_batch_ms=t_all, numpy_vsd_ms_per_pair=t_np,
                              numpy_vsd_ms_total=t_np * n))
             print(json.dumps(rows[-1]))
-    res = dict(gpu=gpu_info(), size=[W, H], rows=rows)
+    res = dict(gpu=card_line(), size=[W, H], rows=rows)
     print(json.dumps(dict(gpu=res["gpu"])))
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
