@@ -3,6 +3,8 @@
 //   direct [tn,vn,2] f32, coords [tn,2] f32, idxs [hn,vn,2] i32, hyp [hn,vn,2|3] f32, inliers [hn,vn,tn] u8.
 // The layer itself never materialises `inliers`; these exist so that code written against the
 // reference extension (and the kernel-level parity tests) keeps working.
+#include <cstring>
+#include "api.h"
 #include "common.cuh"
 #include "kernels.h"
 
@@ -85,6 +87,36 @@ compat_vote_kernel(const float *__restrict__ direct, const float *__restrict__ c
     }
 }
 
+// reference layouts -> layer layouts, so pvb_vote_count can run the layer's own vote kernel
+__global__ void __launch_bounds__(256)
+compat_repack_kernel(const float *__restrict__ direct, const float *__restrict__ coords,
+                     const float *__restrict__ hyp, int tn, int vn, int hn, float2 *__restrict__ dirs,
+                     float2 *__restrict__ xy, float2 *__restrict__ hyp_k, int *__restrict__ meta)
+{
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i < tn) {
+        const float2 c = make_float2(coords[(size_t)i * 2], coords[(size_t)i * 2 + 1]);
+        xy[i] = c;
+        for (int k = 0; k < vn; ++k)
+            dirs[(size_t)k * tn + i] = make_float2(direct[((size_t)i * vn + k) * 2], direct[((size_t)i * vn + k) * 2 + 1]);
+    }
+    if (i < hn)
+        for (int k = 0; k < vn; ++k)
+            hyp_k[(size_t)k * hn + i] = make_float2(hyp[((size_t)i * vn + k) * 2], hyp[((size_t)i * vn + k) * 2 + 1]);
+    if (i == 0) { meta[0] = tn; meta[1] = 0; }
+}
+
+__global__ void __launch_bounds__(256)
+compat_unpack_counts_kernel(const int *__restrict__ counts_k, int *__restrict__ counts, int vn, int hn)
+{
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= hn * vn) return;
+    const int h = i / vn, k = i - h * vn;
+    counts[i] = counts_k[(size_t)k * hn + h];
+}
+
+namespace {
+
 cudaError_t launch_compat_generate(const float *direct, const float *coords, const int32_t *idxs, float *hyp,
                                    int tn, int vn, int hn, bool vanishing, cudaStream_t st)
 {
@@ -106,50 +138,112 @@ cudaError_t launch_compat_vote(const float *direct, const float *coords, const f
     return cudaGetLastError();
 }
 
-// reference layouts -> layer layouts, so pvb_vote_count can run the layer's own vote kernel
-__global__ void __launch_bounds__(256)
-compat_repack_kernel(const float *__restrict__ direct, const float *__restrict__ coords,
-                     const float *__restrict__ hyp, int tn, int vn, int hn, float2 *__restrict__ dirs,
-                     float2 *__restrict__ xy, float2 *__restrict__ hyp_k, int *__restrict__ meta)
+int check_compat(const void *a, const void *b, const void *c, const void *d_, int tn, int vn, int hn)
 {
-    const int i = blockIdx.x * 256 + threadIdx.x;
-    if (i < tn) {
-        const float2 c = make_float2(coords[(size_t)i * 2], coords[(size_t)i * 2 + 1]);
-        xy[i] = c;
-        for (int k = 0; k < vn; ++k)
-            dirs[(size_t)k * tn + i] = make_float2(direct[((size_t)i * vn + k) * 2], direct[((size_t)i * vn + k) * 2 + 1]);
-    }
-    if (i < hn)
-        for (int k = 0; k < vn; ++k)
-            hyp_k[(size_t)k * hn + i] = make_float2(hyp[((size_t)i * vn + k) * 2], hyp[((size_t)i * vn + k) * 2 + 1]);
-    if (i == 0) { meta[0] = tn; meta[1] = 0; }
+    if (tn < 0 || vn < 0 || hn < 0) return fail(PVB_ERR_INVALID, "negative size");
+    if ((long long)hn * vn > (1ll << 30) || (long long)tn * vn > (1ll << 30)) return fail(PVB_ERR_INVALID, "problem too large");
+    if (((tn && vn) && (!a || !b)) || ((hn && vn) && (!c || !d_))) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (vn > 65535) return fail(PVB_ERR_INVALID, "vn must be <= 65535");
+    return PVB_OK;
 }
 
-cudaError_t launch_compat_repack(const float *direct, const float *coords, const float *hyp, int tn, int vn,
-                                 int hn, float2 *dirs, float2 *xy, float2 *hyp_k, int *meta, cudaStream_t st)
-{
-    cudaError_t e = cudaMemsetAsync(meta, 0, 4 * sizeof(int), st);
-    if (e != cudaSuccess) return e;
-    const int n = tn > hn ? tn : hn;
-    compat_repack_kernel<<<(n + 255) / 256 + 1, 256, 0, st>>>(direct, coords, hyp, tn, vn, hn, dirs, xy, hyp_k, meta);
-    return cudaGetLastError();
-}
-
-__global__ void __launch_bounds__(256)
-compat_unpack_counts_kernel(const int *__restrict__ counts_k, int *__restrict__ counts, int vn, int hn)
-{
-    const int i = blockIdx.x * 256 + threadIdx.x;
-    if (i >= hn * vn) return;
-    const int h = i / vn, k = i - h * vn;
-    counts[i] = counts_k[(size_t)k * hn + h];
-}
-
-cudaError_t launch_compat_unpack_counts(const int *counts_k, int *counts, int vn, int hn, cudaStream_t st)
-{
-    const int n = hn * vn;
-    if (n == 0) return cudaSuccess;
-    compat_unpack_counts_kernel<<<(n + 255) / 256, 256, 0, st>>>(counts_k, counts, vn, hn);
-    return cudaGetLastError();
-}
+} // namespace
 
 } // namespace pvb
+
+using namespace pvb;
+
+extern "C" {
+
+PVB_API int pvb_generate_hypothesis(const float *direct, const float *coords, const int32_t *idxs, float *hyp, int32_t tn,
+                            int32_t vn, int32_t hn, pvb_stream_t stream)
+{
+    int rc = check_compat(direct, coords, idxs, hyp, tn, vn, hn);
+    if (rc) return rc;
+    cudaError_t e = launch_compat_generate(direct, coords, idxs, hyp, tn, vn, hn, false, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "generate_hypothesis");
+}
+
+PVB_API int pvb_generate_hypothesis_vanishing_point(const float *direct, const float *coords, const int32_t *idxs, float *hyp,
+                                            int32_t tn, int32_t vn, int32_t hn, pvb_stream_t stream)
+{
+    int rc = check_compat(direct, coords, idxs, hyp, tn, vn, hn);
+    if (rc) return rc;
+    cudaError_t e = launch_compat_generate(direct, coords, idxs, hyp, tn, vn, hn, true, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "generate_hypothesis_vanishing_point");
+}
+
+PVB_API int pvb_voting_for_hypothesis(const float *direct, const float *coords, const float *hyp, uint8_t *inliers, int32_t tn,
+                              int32_t vn, int32_t hn, float inlier_thresh, pvb_stream_t stream)
+{
+    int rc = check_compat(direct, coords, hyp, inliers, tn, vn, hn);
+    if (rc) return rc;
+    if (tn && vn && hn && !inliers) return fail(PVB_ERR_INVALID, "NULL tensor");
+    cudaError_t e = launch_compat_vote(direct, coords, hyp, inliers, tn, vn, hn, inlier_thresh, false, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "voting_for_hypothesis");
+}
+
+PVB_API int pvb_voting_for_hypothesis_vanishing_point(const float *direct, const float *coords, const float *hyp,
+                                              uint8_t *inliers, int32_t tn, int32_t vn, int32_t hn,
+                                              float inlier_thresh, pvb_stream_t stream)
+{
+    int rc = check_compat(direct, coords, hyp, inliers, tn, vn, hn);
+    if (rc) return rc;
+    if (tn && vn && hn && !inliers) return fail(PVB_ERR_INVALID, "NULL tensor");
+    cudaError_t e = launch_compat_vote(direct, coords, hyp, inliers, tn, vn, hn, inlier_thresh, true, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "voting_for_hypothesis_vanishing_point");
+}
+
+PVB_API size_t pvb_vote_count_workspace_bytes(int32_t tn, int32_t vn, int32_t hn)
+{
+    if (tn < 0 || vn < 0 || hn < 0) return 0;
+    size_t off = align_up(4 * sizeof(int));
+    off += align_up((size_t)tn * sizeof(float2));
+    off += align_up((size_t)tn * vn * sizeof(float2));
+    off += align_up((size_t)hn * vn * sizeof(float2));
+    off += align_up((size_t)hn * vn * sizeof(int));
+    return off;
+}
+
+PVB_API int pvb_vote_count(const float *direct, const float *coords, const float *hyp, int32_t *counts, int32_t tn, int32_t vn,
+                   int32_t hn, float inlier_thresh, void *workspace, size_t workspace_bytes, pvb_stream_t stream)
+{
+    int rc = check_compat(direct, coords, hyp, counts, tn, vn, hn);
+    if (rc) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (hn == 0 || vn == 0) return PVB_OK;
+    if (tn == 0) {
+        cudaError_t e = cudaMemsetAsync(counts, 0, sizeof(int) * (size_t)hn * vn, st);
+        return e == cudaSuccess ? PVB_OK : cuda_fail(e, "memset");
+    }
+    if ((long long)vn * ((hn + 511) / 512) > 65535) return fail(PVB_ERR_INVALID, "vn*ceil(hn/512) must be <= 65535");
+    rc = check_workspace(pvb_vote_count_workspace_bytes(tn, vn, hn), workspace, workspace_bytes);
+    if (rc) return rc;
+    // the reference layout -> the layer's (pixels, directions and hypotheses k-major); meta = { tn, state 0, unused, unused }
+    char *w = static_cast<char *>(workspace);
+    size_t off = 0;
+    int *meta = reinterpret_cast<int *>(w + off); off += align_up(4 * sizeof(int));
+    float2 *xy = reinterpret_cast<float2 *>(w + off); off += align_up((size_t)tn * sizeof(float2));
+    float2 *dirs = reinterpret_cast<float2 *>(w + off); off += align_up((size_t)tn * vn * sizeof(float2));
+    float2 *hyp_k = reinterpret_cast<float2 *>(w + off); off += align_up((size_t)hn * vn * sizeof(float2));
+    int *counts_k = reinterpret_cast<int *>(w + off);
+    cudaError_t e = cudaMemsetAsync(meta, 0, 4 * sizeof(int), st);
+    if (e == cudaSuccess) {
+        const int n = tn > hn ? tn : hn;
+        compat_repack_kernel<<<(n + 255) / 256 + 1, 256, 0, st>>>(direct, coords, hyp, tn, vn, hn, dirs, xy, hyp_k, meta);
+        e = cudaGetLastError();
+    }
+    if (e != cudaSuccess) return cuda_fail(e, "repack");
+    VoteArgs v;
+    memset(&v, 0, sizeof(v));
+    v.B = 1; v.K = vn; v.hn = hn; v.cap = tn; v.W = 0; v.H = 0; v.thresh = inlier_thresh;
+    v.tn = meta; v.state = meta + 1; v.xy = xy;
+    v.dirs = dirs; v.idxs = nullptr; v.hyp = hyp_k; v.counts = counts_k;
+    e = launch_vote(v, true, false, st);
+    if (e != cudaSuccess) return cuda_fail(e, "vote kernel");
+    compat_unpack_counts_kernel<<<(hn * vn + 255) / 256, 256, 0, st>>>(counts_k, counts, vn, hn);
+    e = cudaGetLastError();
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "unpack");
+}
+
+} // extern "C"

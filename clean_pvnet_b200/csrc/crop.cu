@@ -17,9 +17,41 @@
 // sum is integer arithmetic, so the output byte is exact in any order.  The crop then zeroes what lies outside the
 // magnified box (magnify_box of the box corners through the matrix) and normalises (u8 / 255 - mean) / std in fp32,
 // writing NCHW, and optionally the uint8 HWC crop.  No intermediate image exists.
-#include "kernels.h"
+#include <cmath>
+#include "api.h"
 
 namespace pvb {
+
+// Setup: one thread per box -> centre, scale, forward (and inverse) crop matrix.
+struct CropArgs {
+    const double *boxes;          // [n][4] xyxy, image coordinates
+    int n, out_w, out_h, center_f64;  // center_f64: the cascade's fp64 centre, else pvnet_transform's fp32 one
+    double scale_ratio;
+    double *center, *scale;       // [n][2], [n]: as the reference computes them (fp64)
+    double *M, *Minv;             // [n][6] forward crop matrix; inverse (inv=1) or NULL
+};
+// Warp: one CTA per (box, output row) over [n][out_h]; the crop variant masks, normalises and writes NCHW fp32.
+struct WarpArgs {
+    const unsigned char *img;     // [B][H][W][C] at element strides sb, sh, sw, sc
+    long long sb, sh, sw, sc;
+    int B, H, W, C;
+    const double *M;              // [n][6] forward matrices (warpAffine inverts them)
+    const int *image_index;       // [n] or NULL (every row reads image 0)
+    int n, out_w, out_h;
+    const double *boxes;          // crop: [n][4], for the box mask
+    int mask;                     // crop: zero what lies outside the magnified box
+    double box_ratio;
+    float mean[3], stdv[3];       // crop: normalisation
+    float *inp;                   // crop: [n][3][out_h][out_w]
+    unsigned char *out_u8;        // [n][out_h][out_w][C]: the warp's output; optional for the crop
+};
+struct UncropArgs {
+    const float *kpt;             // [n][K][2], crop frame
+    const double *center, *scale; // [n][2], [n]
+    int n, K, in_w, in_h;
+    double *out;                  // [n][K][2], image frame
+};
+
 namespace {
 
 constexpr int CROP_SETUP_THREADS = 128;
@@ -218,11 +250,15 @@ __global__ void __launch_bounds__(CROP_SETUP_THREADS) uncrop_kernel(const Uncrop
 
 } // namespace
 
+// External linkage on purpose: nvcc names this file's anonymous namespace, and so its kernels, after the first
+// externally visible definition in the file.
 cudaError_t launch_crop_setup(const CropArgs &a, cudaStream_t st)
 {
     crop_setup_kernel<<<(unsigned)((a.n + CROP_SETUP_THREADS - 1) / CROP_SETUP_THREADS), CROP_SETUP_THREADS, 0, st>>>(a);
     return cudaGetLastError();
 }
+
+namespace {
 
 cudaError_t launch_warp(const WarpArgs &a, bool crop, cudaStream_t st)
 {
@@ -232,10 +268,88 @@ cudaError_t launch_warp(const WarpArgs &a, bool crop, cudaStream_t st)
     return cudaGetLastError();
 }
 
-cudaError_t launch_uncrop(const UncropArgs &a, cudaStream_t st)
+// the image and output arguments the crop and the warp share; fills the image and size fields of `a`
+int warp_common(WarpArgs &a, const uint8_t *img, int32_t B, int32_t H, int32_t W, int32_t C, const int64_t *img_stride,
+                int32_t n, int32_t out_w, int32_t out_h)
 {
-    uncrop_kernel<<<(unsigned)((a.n + CROP_SETUP_THREADS - 1) / CROP_SETUP_THREADS), CROP_SETUP_THREADS, 0, st>>>(a);
-    return cudaGetLastError();
+    if (n < 0 || B < 0) return fail(PVB_ERR_INVALID, "negative size (n=%d B=%d)", n, B);
+    if (H < 1 || W < 1 || H > 32767 || W > 32767) return fail(PVB_ERR_INVALID, "image must be 1..32767 pixels a side (got %dx%d)", W, H);
+    if (C < 1 || C > 4) return fail(PVB_ERR_INVALID, "C must be in [1,4] (got %d)", C);
+    if (out_w < 1 || out_h < 1) return fail(PVB_ERR_INVALID, "output size must be >= 1 (got %dx%d)", out_w, out_h);
+    if ((long long)n * out_h > 0x7fffffffll) return fail(PVB_ERR_INVALID, "n * out_h too large (>= 2^31)");
+    if (!img_stride) return fail(PVB_ERR_INVALID, "NULL stride array");
+    for (int i = 0; i < 4; ++i)
+        if (img_stride[i] < 0) return fail(PVB_ERR_INVALID, "negative stride");
+    if (n > 0 && B > 0 && !img) return fail(PVB_ERR_INVALID, "NULL tensor");
+    a.img = img; a.sb = img_stride[0]; a.sh = img_stride[1]; a.sw = img_stride[2]; a.sc = img_stride[3];
+    a.B = B; a.H = H; a.W = W; a.C = C; a.n = n; a.out_w = out_w; a.out_h = out_h;
+    return PVB_OK;
 }
 
+} // namespace
+
 } // namespace pvb
+
+using namespace pvb;
+
+extern "C" {
+
+PVB_API int pvb_crop_inputs(const uint8_t *img, int32_t B, int32_t H, int32_t W, const int64_t *img_stride,
+                            const double *boxes, const int32_t *image_index, int32_t n, int32_t out_w, int32_t out_h,
+                            double scale_ratio, double box_ratio, int32_t flags, const float *mean, const float *std,
+                            float *inp, uint8_t *crop_u8, double *center, double *scale, double *matrix,
+                            double *matrix_inv, pvb_stream_t stream)
+{
+    WarpArgs w = {};
+    if (int rc = warp_common(w, img, B, H, W, 3, img_stride, n, out_w, out_h)) return rc;
+    if (!std::isfinite(scale_ratio) || !std::isfinite(box_ratio))
+        return fail(PVB_ERR_INVALID, "scale_ratio and box_ratio must be finite (got %g, %g)", scale_ratio, box_ratio);
+    if (box_ratio < 0) return fail(PVB_ERR_INVALID, "box_ratio must be >= 0 (got %g)", box_ratio);
+    if (flags & ~(PVB_CROP_MASK_TO_BOX | PVB_CROP_CENTER_F64)) return fail(PVB_ERR_INVALID, "unknown flags 0x%x", flags);
+    if (!mean || !std) return fail(PVB_ERR_INVALID, "NULL mean / std");
+    for (int c = 0; c < 3; ++c)
+        if (!(std[c] != 0.0f) || !std::isfinite(mean[c])) return fail(PVB_ERR_INVALID, "std must be non-zero and mean finite");
+    if (!img || !boxes || !inp || !center || !scale || !matrix) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (n == 0) return PVB_OK;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CropArgs c;
+    c.boxes = boxes; c.n = n; c.out_w = out_w; c.out_h = out_h; c.center_f64 = (flags & PVB_CROP_CENTER_F64) != 0;
+    c.scale_ratio = scale_ratio; c.center = center; c.scale = scale; c.M = matrix; c.Minv = matrix_inv;
+    cudaError_t e = launch_crop_setup(c, st);
+    if (e != cudaSuccess) return cuda_fail(e, "crop setup kernel");
+    w.M = matrix; w.image_index = image_index; w.boxes = boxes; w.mask = (flags & PVB_CROP_MASK_TO_BOX) != 0;
+    w.box_ratio = box_ratio; w.inp = inp; w.out_u8 = crop_u8;
+    for (int k = 0; k < 3; ++k) { w.mean[k] = mean[k]; w.stdv[k] = std[k]; }
+    e = launch_warp(w, true, st);
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "crop warp kernel");
+}
+
+PVB_API int pvb_uncrop_keypoints(const float *kpt_2d, const double *center, const double *scale, int32_t n, int32_t K,
+                                 int32_t in_w, int32_t in_h, double *out, pvb_stream_t stream)
+{
+    if (n < 0 || K < 0) return fail(PVB_ERR_INVALID, "negative size (n=%d K=%d)", n, K);
+    if (in_w < 1 || in_h < 1) return fail(PVB_ERR_INVALID, "input size must be >= 1 (got %dx%d)", in_w, in_h);
+    if (n == 0 || K == 0) return PVB_OK;
+    if (!kpt_2d || !center || !scale || !out) return fail(PVB_ERR_INVALID, "NULL tensor");
+    UncropArgs a;
+    a.kpt = kpt_2d; a.center = center; a.scale = scale; a.n = n; a.K = K; a.in_w = in_w; a.in_h = in_h; a.out = out;
+    uncrop_kernel<<<(unsigned)((n + CROP_SETUP_THREADS - 1) / CROP_SETUP_THREADS), CROP_SETUP_THREADS, 0,
+                    static_cast<cudaStream_t>(stream)>>>(a);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "uncrop kernel");
+}
+
+PVB_API int pvb_warp_affine_linear(const uint8_t *img, int32_t B, int32_t H, int32_t W, int32_t C, const int64_t *img_stride,
+                                   const double *M, const int32_t *image_index, int32_t n, int32_t out_w, int32_t out_h,
+                                   uint8_t *out, pvb_stream_t stream)
+{
+    WarpArgs w = {};
+    if (int rc = warp_common(w, img, B, H, W, C, img_stride, n, out_w, out_h)) return rc;
+    if (n == 0) return PVB_OK;
+    if (!img || !M || !out) return fail(PVB_ERR_INVALID, "NULL tensor");
+    w.M = M; w.image_index = image_index; w.out_u8 = out;
+    cudaError_t e = launch_warp(w, false, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "warp kernel");
+}
+
+} // extern "C"

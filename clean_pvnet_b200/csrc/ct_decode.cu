@@ -24,10 +24,24 @@
 //   clip: x0, y0 = clamp(min=0), x1 = clamp(max=W-1), y1 = clamp(max=H-1), NaN passed through as torch.clamp does.
 // Nothing depends on CTA scheduling: the lists are written per CTA, every selection step counts exactly, and the
 // output position of a key is its rank.
+#include "api.h"
 #include "common.cuh"
-#include "kernels.h"
 
 namespace pvb {
+
+struct CtDecodeArgs {
+    const float *hm;          // [B][C][H][W] logits at element strides hs
+    long long hs[4];
+    const float *wh;          // [B][2][H][W] at element strides ws
+    long long ws[4];
+    int B, C, H, W, K, clip;
+    int T, Lk;                // tiles per class and entries per list
+    long long L;              // lists per image, C * T
+    unsigned long long *lists;   // workspace [B][L][Lk]: each tile's largest keys, descending
+    unsigned long long *sel;     // workspace [B][K]: the image's K selected keys, unordered
+    float *ct;                // [B][K][2] (xs, ys)
+    float *det;               // [B][K][6] (x0, y0, x1, y1, score, class)
+};
 
 constexpr int CD_T = 32;                           // tile side
 constexpr int CD_N = CD_T * CD_T;                  // keys per tile
@@ -247,6 +261,9 @@ __global__ void __launch_bounds__(CD_SEL_THREADS) ct_decode_select_kernel(CtDeco
     }
 }
 
+namespace {
+
+// the lists at offset 0, then sel, 256-byte aligned
 size_t ct_decode_workspace_bytes(int B, int C, int H, int W, int K, size_t *sel_offset)
 {
     const size_t T = (size_t)((W + CD_T - 1) / CD_T) * (size_t)((H + CD_T - 1) / CD_T);
@@ -256,17 +273,68 @@ size_t ct_decode_workspace_bytes(int B, int C, int H, int W, int K, size_t *sel_
     return lists + ((size_t)B * K * sizeof(unsigned long long) + 255) / 256 * 256;
 }
 
-cudaError_t launch_ct_decode(CtDecodeArgs a, cudaStream_t st)
+// the sizes pvb_ct_decode accepts (the limits keep every index exact in fp32 and every key unique)
+int ct_decode_sizes(int32_t B, int32_t C, int32_t H, int32_t W, int32_t K)
 {
-    if (a.B == 0) return cudaSuccess;
-    a.T = ((a.W + CD_T - 1) / CD_T) * ((a.H + CD_T - 1) / CD_T);
-    a.L = (long long)a.C * a.T;
-    a.Lk = a.K < CD_N ? a.K : CD_N;
-    ct_decode_tile_kernel<<<dim3((unsigned)a.T, (unsigned)a.C, (unsigned)a.B), CD_THREADS, 0, st>>>(a);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    ct_decode_select_kernel<<<(unsigned)a.B, CD_SEL_THREADS, 0, st>>>(a);
-    return cudaGetLastError();
+    if (B < 0 || B > 65535) return fail(PVB_ERR_INVALID, "B must be in [0, 65535], got %d", B);
+    if (C < 1 || C > 65535 || H < 1 || W < 1)
+        return fail(PVB_ERR_INVALID, "C, H and W must be >= 1 and C <= 65535 (got C=%d H=%d W=%d)", C, H, W);
+    const long long HW = (long long)H * W;
+    if (HW >= (1ll << 24)) return fail(PVB_ERR_INVALID, "H*W must be < 2^24, got %lld", HW);
+    if (K < 1 || K > HW) return fail(PVB_ERR_INVALID, "K must be in [1, H*W = %lld], got %d", HW, K);
+    if ((long long)C * K >= (1ll << 24)) return fail(PVB_ERR_INVALID, "C*K must be < 2^24, got %lld", (long long)C * K);
+    if ((long long)C * HW >= (1ll << 31)) return fail(PVB_ERR_INVALID, "C*H*W must be < 2^31, got %lld", (long long)C * HW);
+    return PVB_OK;
 }
 
+} // namespace
+
 } // namespace pvb
+
+using namespace pvb;
+
+extern "C" {
+
+PVB_API size_t pvb_ct_decode_workspace_bytes(int32_t B, int32_t C, int32_t H, int32_t W, int32_t K)
+{
+    if (B < 0 || C < 0 || H < 0 || W < 0 || K < 0) return 0;
+    return ct_decode_workspace_bytes(B, C, H, W, K, nullptr);
+}
+
+// lib/networks/ct/dla.py:20-26 Network.decode_detection: sigmoid, ct_decode.decode_ct_hm, data_utils.clip_to_image
+PVB_API int pvb_ct_decode(const float *ct_hm, const int64_t *hm_stride, const float *wh, const int64_t *wh_stride,
+                          int32_t B, int32_t C, int32_t H, int32_t W, int32_t K, int32_t clip, float *ct,
+                          float *detection, void *workspace, size_t workspace_bytes, pvb_stream_t stream)
+{
+    if (int rc = ct_decode_sizes(B, C, H, W, K)) return rc;
+    if (clip != 0 && clip != 1) return fail(PVB_ERR_INVALID, "clip must be 0 or 1 (got %d)", clip);
+    if (!hm_stride || !wh_stride) return fail(PVB_ERR_INVALID, "NULL stride array");
+    CtDecodeArgs a = {};
+    for (int i = 0; i < 4; ++i) {
+        if (hm_stride[i] < 0 || wh_stride[i] < 0) return fail(PVB_ERR_INVALID, "negative stride");
+        a.hs[i] = hm_stride[i];
+        a.ws[i] = wh_stride[i];
+    }
+    if (B == 0) return PVB_OK;
+    if (!ct_hm || !wh || !ct || !detection) return fail(PVB_ERR_INVALID, "NULL tensor");
+    size_t so = 0;
+    if (int rc = check_workspace(ct_decode_workspace_bytes(B, C, H, W, K, &so), workspace, workspace_bytes)) return rc;
+    char *ws = static_cast<char *>(workspace);
+    a.hm = ct_hm; a.wh = wh; a.B = B; a.C = C; a.H = H; a.W = W; a.K = K; a.clip = clip;
+    a.lists = reinterpret_cast<unsigned long long *>(ws);
+    a.sel = reinterpret_cast<unsigned long long *>(ws + so);
+    a.ct = ct; a.det = detection;
+    a.T = ((W + CD_T - 1) / CD_T) * ((H + CD_T - 1) / CD_T);
+    a.L = (long long)C * a.T;
+    a.Lk = K < CD_N ? K : CD_N;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    ct_decode_tile_kernel<<<dim3((unsigned)a.T, (unsigned)C, (unsigned)B), CD_THREADS, 0, st>>>(a);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) {
+        ct_decode_select_kernel<<<(unsigned)B, CD_SEL_THREADS, 0, st>>>(a);
+        e = cudaGetLastError();
+    }
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "ct decode kernels");
+}
+
+} // extern "C"

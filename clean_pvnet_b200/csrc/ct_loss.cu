@@ -17,10 +17,28 @@
 // The backward pass repeats autograd's chain op by op (ct_grad), including the order in which autograd adds the
 // gradients of p's four uses: ((pow(p, 2) + (1 - p) of log) + (1 - p) of pow) + log(p).  Every operation is an explicit
 // round-to-nearest intrinsic or the libdevice function torch's kernel calls, so nvcc contracts nothing into an FMA.
+#include "api.h"
 #include "common.cuh"
-#include "kernels.h"
 
 namespace pvb {
+
+// One CTA per (32x16 pixel tile, class, image); the image's objects of that class whose window meets the tile are staged
+// in shared memory.
+struct CtArgs {
+    const float *logits;      // [B][C][H][W] at element strides ls (forward, backward)
+    long long ls[4];
+    const long long *ct_ind;  // [B][M] cy * W + cx
+    const int *ct_radius;     // [B][M]
+    const long long *ct_cls;  // [B][M]
+    const float *ct_01;       // [B][M] an object counts where ct_01 == 1
+    int B, M, C, H, W;
+    float *out;               // contiguous [B][C][H][W]: the target (target) or grad_logits (backward)
+    double *pos_part, *neg_part;   // [nparts] per-CTA fp64 sums of the pos and neg terms (forward)
+    int *cnt_part;            // [nparts] per-CTA counts of target == 1 (forward)
+    long long *num_pos;       // exact count of target == 1: written by the forward pass, read by the backward pass
+    float *loss;              // the scalar loss (forward)
+    const float *grad_loss;   // the scalar upstream gradient (backward)
+};
 
 constexpr int CT_TW = 32, CT_TH = 16;      // one CTA per (32x16 pixel tile, class, image)
 constexpr int CT_THREADS = 256;            // each thread owns two pixels of a column: rows ty and ty + 8
@@ -255,8 +273,7 @@ long long ct_nparts(int B, int C, int H, int W)
     return (long long)B * C * (((long long)W + CT_TW - 1) / CT_TW) * (((long long)H + CT_TH - 1) / CT_TH);
 }
 
-} // namespace
-
+// num_pos at offset 0, then the three partial arrays, each 256-byte aligned
 size_t ct_loss_workspace_bytes(int B, int C, int H, int W, size_t *pos_offset, size_t *neg_offset, size_t *cnt_offset)
 {
     const size_t n = (size_t)ct_nparts(B, C, H, W);
@@ -267,30 +284,123 @@ size_t ct_loss_workspace_bytes(int B, int C, int H, int W, size_t *pos_offset, s
     return co + (n * sizeof(int) + 255) / 256 * 256;
 }
 
+constexpr int CT_MAX_M = 1024;      // the tile's staged objects take at most 24 KB of shared memory
 size_t ct_smem_bytes(int M) { return (size_t)(M > 0 ? M : 1) * sizeof(CtObj); }
 
-cudaError_t launch_ct_target(const CtArgs &a, cudaStream_t st)
+// the arguments every CenterNet-loss entry shares; fills the object and size fields of `a`
+int ct_common(CtArgs &a, const int64_t *ct_ind, const int32_t *ct_radius, const int64_t *ct_cls, const float *ct_01,
+              int32_t B, int32_t M, int32_t C, int32_t H, int32_t W)
 {
-    if ((long long)a.B * a.C * a.H * a.W == 0) return cudaSuccess;
-    ct_target_kernel<<<ct_grid(a), CT_THREADS, ct_smem_bytes(a.M), st>>>(a);
-    return cudaGetLastError();
+    if (B < 0 || M < 0 || C < 0 || H < 0 || W < 0)
+        return fail(PVB_ERR_INVALID, "negative size (B=%d M=%d C=%d H=%d W=%d)", B, M, C, H, W);
+    if (M > CT_MAX_M) return fail(PVB_ERR_INVALID, "M must be at most %d objects per image, got %d", CT_MAX_M, M);
+    if (B > 65535) return fail(PVB_ERR_INVALID, "B must be at most 65535, got %d", B);
+    if (C > 65535) return fail(PVB_ERR_INVALID, "C must be at most 65535, got %d", C);
+    if ((long long)H * W > 0x7fffffffll) return fail(PVB_ERR_INVALID, "image too large (H*W >= 2^31)");
+    if ((long long)B * M > 0 && (!ct_ind || !ct_radius || !ct_cls || !ct_01)) return fail(PVB_ERR_INVALID, "NULL tensor");
+    a = CtArgs{};
+    a.ct_ind = reinterpret_cast<const long long *>(ct_ind);
+    a.ct_radius = ct_radius;
+    a.ct_cls = reinterpret_cast<const long long *>(ct_cls);
+    a.ct_01 = ct_01;
+    a.B = B; a.M = M; a.C = C; a.H = H; a.W = W;
+    return PVB_OK;
 }
 
-cudaError_t launch_ct_loss_forward(const CtArgs &a, cudaStream_t st)
+int ct_logits(CtArgs &a, const float *logits, const int64_t *logit_stride)
 {
-    const long long nparts = ct_nparts(a.B, a.C, a.H, a.W);
-    if (nparts > 0) ct_loss_fwd_kernel<<<ct_grid(a), CT_THREADS, ct_smem_bytes(a.M), st>>>(a);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    ct_loss_final_kernel<<<1, CT_FINAL_THREADS, 0, st>>>(a.pos_part, a.neg_part, a.cnt_part, nparts, a.num_pos, a.loss);
-    return cudaGetLastError();
+    if (!logit_stride) return fail(PVB_ERR_INVALID, "NULL stride array");
+    for (int i = 0; i < 4; ++i) {
+        if (logit_stride[i] < 0) return fail(PVB_ERR_INVALID, "negative stride");
+        a.ls[i] = logit_stride[i];
+    }
+    if ((long long)a.B * a.C * a.H * a.W > 0 && !logits) return fail(PVB_ERR_INVALID, "NULL tensor");
+    a.logits = logits;
+    return PVB_OK;
 }
 
-cudaError_t launch_ct_loss_backward(const CtArgs &a, cudaStream_t st)
+// checks the workspace and fills the workspace fields of `a`
+int ct_workspace(CtArgs &a, const void *workspace, size_t workspace_bytes)
 {
-    if ((long long)a.B * a.C * a.H * a.W == 0) return cudaSuccess;
-    ct_loss_bwd_kernel<<<ct_grid(a), CT_THREADS, ct_smem_bytes(a.M), st>>>(a);
-    return cudaGetLastError();
+    size_t po = 0, no = 0, co = 0;
+    if (int rc = check_workspace(ct_loss_workspace_bytes(a.B, a.C, a.H, a.W, &po, &no, &co), workspace, workspace_bytes))
+        return rc;
+    char *ws = static_cast<char *>(const_cast<void *>(workspace));
+    a.num_pos = reinterpret_cast<long long *>(ws);
+    a.pos_part = reinterpret_cast<double *>(ws + po);
+    a.neg_part = reinterpret_cast<double *>(ws + no);
+    a.cnt_part = reinterpret_cast<int *>(ws + co);
+    return PVB_OK;
 }
+
+} // namespace
 
 } // namespace pvb
+
+using namespace pvb;
+
+extern "C" {
+
+// lib/datasets/tless*/ct.py ct_hm: data_utils.draw_umich_gaussian per object
+PVB_API int pvb_ct_target(const int64_t *ct_ind, const int32_t *ct_radius, const int64_t *ct_cls, const float *ct_01,
+                          float *ct_hm, int32_t B, int32_t M, int32_t C, int32_t H, int32_t W, pvb_stream_t stream)
+{
+    CtArgs a;
+    if (int rc = ct_common(a, ct_ind, ct_radius, ct_cls, ct_01, B, M, C, H, W)) return rc;
+    if ((long long)B * C * H * W == 0) return PVB_OK;
+    if (!ct_hm) return fail(PVB_ERR_INVALID, "NULL tensor");
+    a.out = ct_hm;
+    ct_target_kernel<<<ct_grid(a), CT_THREADS, ct_smem_bytes(M), static_cast<cudaStream_t>(stream)>>>(a);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "ct target kernel");
+}
+
+PVB_API size_t pvb_ct_loss_workspace_bytes(int32_t B, int32_t C, int32_t H, int32_t W)
+{
+    if (B < 0 || C < 0 || H < 0 || W < 0) return 0;
+    return ct_loss_workspace_bytes(B, C, H, W, nullptr, nullptr, nullptr);
+}
+
+// lib/train/trainers/ct.py:20-21, the forward pass
+PVB_API int pvb_ct_loss_forward(const float *logits, const int64_t *logit_stride, const int64_t *ct_ind,
+                                const int32_t *ct_radius, const int64_t *ct_cls, const float *ct_01, float *loss,
+                                int32_t B, int32_t M, int32_t C, int32_t H, int32_t W, void *workspace,
+                                size_t workspace_bytes, pvb_stream_t stream)
+{
+    CtArgs a;
+    if (int rc = ct_common(a, ct_ind, ct_radius, ct_cls, ct_01, B, M, C, H, W)) return rc;
+    if (int rc = ct_logits(a, logits, logit_stride)) return rc;
+    if (!loss) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (int rc = ct_workspace(a, workspace, workspace_bytes)) return rc;
+    a.loss = loss;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const long long nparts = ct_nparts(B, C, H, W);
+    if (nparts > 0) ct_loss_fwd_kernel<<<ct_grid(a), CT_THREADS, ct_smem_bytes(M), st>>>(a);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) {
+        ct_loss_final_kernel<<<1, CT_FINAL_THREADS, 0, st>>>(a.pos_part, a.neg_part, a.cnt_part, nparts, a.num_pos, loss);
+        e = cudaGetLastError();
+    }
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "ct loss forward kernels");
+}
+
+// lib/train/trainers/ct.py:20-21, autograd's backward pass of it
+PVB_API int pvb_ct_loss_backward(const float *logits, const int64_t *logit_stride, const int64_t *ct_ind,
+                                 const int32_t *ct_radius, const int64_t *ct_cls, const float *ct_01,
+                                 const float *grad_loss, float *grad_logits, int32_t B, int32_t M, int32_t C, int32_t H,
+                                 int32_t W, const void *workspace, size_t workspace_bytes, pvb_stream_t stream)
+{
+    CtArgs a;
+    if (int rc = ct_common(a, ct_ind, ct_radius, ct_cls, ct_01, B, M, C, H, W)) return rc;
+    if (int rc = ct_logits(a, logits, logit_stride)) return rc;
+    if ((long long)B * C * H * W == 0) return PVB_OK;
+    if (!grad_loss || !grad_logits) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (int rc = ct_workspace(a, workspace, workspace_bytes)) return rc;
+    a.grad_loss = grad_loss;
+    a.out = grad_logits;
+    ct_loss_bwd_kernel<<<ct_grid(a), CT_THREADS, ct_smem_bytes(M), static_cast<cudaStream_t>(stream)>>>(a);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "ct loss backward kernel");
+}
+
+} // extern "C"

@@ -14,9 +14,24 @@
 // reference kernel's bit for bit: nvcc contracts its `w1*v1 + w2*v2 + w3*v3 + w4*v4` (dcn_v2_im2col_cuda.cu:52) into
 // fma(w4,v4, fma(w3,v3, fma(w1,v1, w2*v2))) at sm_90a (read off the reference build's SASS), written out below with
 // explicit intrinsics; the mask multiplies after the bilinear sum.
-#include "kernels.h"
+#include "api.h"
 
 namespace pvb {
+
+// Contiguous fp32 NCHW; shapes validated by dcn_args.
+struct DcnArgs {
+    const float *input;       // [B][C][H][W]
+    const float *offset;      // [B][dg*2*kh*kw][Ho][Wo]
+    const float *mask;        // [B][dg*kh*kw][Ho][Wo]
+    const float *weight;      // [Co][C][kh][kw]
+    const float *bias;        // [Co]
+    float *out;               // [B][Co][Ho][Wo] (forward)
+    const float *grad_out;    // [B][Co][Ho][Wo] (backward)
+    float *grad_input, *grad_offset, *grad_mask, *grad_weight, *grad_bias;   // shaped like their inputs (backward)
+    float *cols;              // grad_cols [chunk][C*kh*kw][Ho*Wo] (backward workspace)
+    int B, C, H, W, Co, kh, kw, sh, sw, ph, pw, dh, dw, dg, Ho, Wo;
+};
+
 namespace {
 
 constexpr int BM = 64, BN = 128, BK = 16, NT = 256;   // CTA tile (rows x columns x depth), threads
@@ -385,10 +400,15 @@ __global__ void __launch_bounds__(256) dcn_grad_bias_kernel(DcnArgs a)
     }
 }
 
-size_t align256(size_t n) { return (n + 255) & ~size_t(255); }
-
 } // namespace
 
+// backward plan: images per grad_cols chunk, and grad_weight's split of the (image, pixel) reduction into `splits`
+// ranges of `span` pixels over `ntile_n` column tiles.  Workspace: cols_bytes of grad_cols, then part_bytes of
+// grad_weight partials (0 when splits == 1), each 256-byte aligned.  A function of the shapes only.
+struct DcnPlan { int chunk, splits; long long span, ntile_n; size_t cols_bytes, part_bytes; };
+
+// External linkage on purpose: nvcc names this file's anonymous namespace, and so its kernels, after the first
+// externally visible definition in the file.
 DcnPlan dcn_plan(const DcnArgs &a, int chunk)
 {
     DcnPlan pl;
@@ -403,27 +423,97 @@ DcnPlan dcn_plan(const DcnArgs &a, int chunk)
     if (S > 65535) S = 65535;
     pl.span = ((Q + S - 1) / S + BK - 1) / BK * BK;
     pl.splits = (int)((Q + pl.span - 1) / pl.span);
-    pl.cols_bytes = align256((size_t)pl.chunk * K * P * sizeof(float));
-    pl.part_bytes = pl.splits > 1 ? align256((size_t)pl.splits * a.Co * K * sizeof(float)) : 0;
+    pl.cols_bytes = align_up((size_t)pl.chunk * K * P * sizeof(float));
+    pl.part_bytes = pl.splits > 1 ? align_up((size_t)pl.splits * a.Co * K * sizeof(float)) : 0;
     return pl;
 }
 
-cudaError_t launch_dcn_forward(const DcnArgs &a, cudaStream_t st)
+namespace {
+
+size_t dcn_workspace_bytes(const DcnPlan &p) { return p.cols_bytes + p.part_bytes; }
+
+// checks a DCN descriptor and fills the kernels' argument block; PVB_OK or PVB_ERR_INVALID (no CUDA call)
+int dcn_args(const pvb_dcn_desc *d, DcnArgs &a)
 {
-    const int P = a.Ho * a.Wo;
-    dim3 grid((P + BN - 1) / BN, (a.Co + BM - 1) / BM, a.B);
-    dcn_forward_kernel<<<grid, NT, 0, st>>>(a);
-    return cudaGetLastError();
+    if (!d) return fail(PVB_ERR_INVALID, "descriptor is NULL");
+    if (d->B < 0 || d->C < 1 || d->H < 1 || d->W < 1 || d->C_out < 1 || d->kh < 1 || d->kw < 1)
+        return fail(PVB_ERR_INVALID, "bad shape B=%d C=%d H=%d W=%d C_out=%d kh=%d kw=%d", d->B, d->C, d->H, d->W,
+                    d->C_out, d->kh, d->kw);
+    if (d->stride_h < 1 || d->stride_w < 1 || d->pad_h < 0 || d->pad_w < 0 || d->dilation_h < 1 || d->dilation_w < 1)
+        return fail(PVB_ERR_INVALID, "bad stride/pad/dilation (%d,%d)/(%d,%d)/(%d,%d)", d->stride_h, d->stride_w,
+                    d->pad_h, d->pad_w, d->dilation_h, d->dilation_w);
+    if (d->deformable_groups < 1 || d->C % d->deformable_groups)
+        return fail(PVB_ERR_INVALID, "deformable_groups=%d must be >= 1 and divide C=%d", d->deformable_groups, d->C);
+    const long long ext_h = (long long)d->dilation_h * (d->kh - 1) + 1, ext_w = (long long)d->dilation_w * (d->kw - 1) + 1;
+    const long long span_h = d->H + 2ll * d->pad_h, span_w = d->W + 2ll * d->pad_w;
+    if (span_h > (1ll << 30) || span_w > (1ll << 30) || ext_h > (1ll << 30) || ext_w > (1ll << 30))
+        return fail(PVB_ERR_INVALID, "padded input or dilated kernel extent >= 2^30");
+    if (span_h < ext_h || span_w < ext_w) return fail(PVB_ERR_INVALID, "the dilated kernel does not fit the padded input");
+    const long long Ho = (span_h - ext_h) / d->stride_h + 1, Wo = (span_w - ext_w) / d->stride_w + 1;
+    const long long K = (long long)d->C * d->kh * d->kw, T = (long long)d->kh * d->kw;
+    if (d->B > 65535) return fail(PVB_ERR_INVALID, "B=%d > 65535", d->B);
+    if ((long long)d->H * d->W >= (1ll << 31) || Ho * Wo >= (1ll << 31)) return fail(PVB_ERR_INVALID, "H*W or Ho*Wo >= 2^31");
+    if (K > 65535ll * 64 || d->C_out > 65535 * 64) return fail(PVB_ERR_INVALID, "C*kh*kw or C_out > 4194240");
+    if (T * d->deformable_groups > 65535) return fail(PVB_ERR_INVALID, "deformable_groups*kh*kw > 65535");
+    a = DcnArgs{};
+    a.B = d->B; a.C = d->C; a.H = d->H; a.W = d->W; a.Co = d->C_out; a.kh = d->kh; a.kw = d->kw;
+    a.sh = d->stride_h; a.sw = d->stride_w; a.ph = d->pad_h; a.pw = d->pad_w; a.dh = d->dilation_h; a.dw = d->dilation_w;
+    a.dg = d->deformable_groups; a.Ho = (int)Ho; a.Wo = (int)Wo;
+    return PVB_OK;
 }
 
-cudaError_t launch_dcn_backward(DcnArgs a, const DcnPlan &pl, void *workspace, cudaStream_t st)
+} // namespace
+
+} // namespace pvb
+
+using namespace pvb;
+
+extern "C" {
+
+PVB_API int pvb_dcn_forward(const pvb_dcn_desc *d, const float *input, const float *offset, const float *mask,
+                            const float *weight, const float *bias, float *output, pvb_stream_t stream)
 {
+    DcnArgs a;
+    if (int rc = dcn_args(d, a)) return rc;
+    if (a.B == 0) return PVB_OK;
+    if (!input || !offset || !mask || !weight || !bias || !output) return fail(PVB_ERR_INVALID, "NULL tensor");
+    a.input = input; a.offset = offset; a.mask = mask; a.weight = weight; a.bias = bias; a.out = output;
+    const dim3 grid((a.Ho * a.Wo + BN - 1) / BN, (a.Co + BM - 1) / BM, a.B);
+    dcn_forward_kernel<<<grid, NT, 0, static_cast<cudaStream_t>(stream)>>>(a);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "dcn forward kernel");
+}
+
+PVB_API size_t pvb_dcn_backward_workspace_bytes(const pvb_dcn_desc *d, int32_t chunk)
+{
+    DcnArgs a;
+    if (!d || d->B < 1 || dcn_args(d, a) != PVB_OK) return 0;
+    return dcn_workspace_bytes(dcn_plan(a, chunk));
+}
+
+PVB_API int pvb_dcn_backward(const pvb_dcn_desc *d, const float *input, const float *offset, const float *mask,
+                             const float *weight, const float *grad_output, float *grad_input, float *grad_offset,
+                             float *grad_mask, float *grad_weight, float *grad_bias, int32_t chunk, void *workspace,
+                             size_t workspace_bytes, pvb_stream_t stream)
+{
+    DcnArgs a;
+    if (int rc = dcn_args(d, a)) return rc;
+    if (a.B == 0) return PVB_OK;
+    if (!input || !offset || !mask || !weight || !grad_output || !grad_input || !grad_offset || !grad_mask ||
+        !grad_weight || !grad_bias)
+        return fail(PVB_ERR_INVALID, "NULL tensor");
+    const DcnPlan pl = dcn_plan(a, chunk);
+    if (int rc = check_workspace(dcn_workspace_bytes(pl), workspace, workspace_bytes)) return rc;
+    a.input = input; a.offset = offset; a.mask = mask; a.weight = weight; a.grad_out = grad_output;
+    a.grad_input = grad_input; a.grad_offset = grad_offset; a.grad_mask = grad_mask; a.grad_weight = grad_weight;
+    a.grad_bias = grad_bias;
+    a.cols = static_cast<float *>(workspace);
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int P = a.Ho * a.Wo, T = a.kh * a.kw;
     const long long K = (long long)a.C * T;
-    a.cols = static_cast<float *>(workspace);
     float *part = pl.splits > 1 ? reinterpret_cast<float *>(static_cast<char *>(workspace) + pl.cols_bytes) : a.grad_weight;
     cudaError_t e = cudaMemsetAsync(a.grad_input, 0, (size_t)a.B * a.C * a.H * a.W * sizeof(float), st);
-    if (e != cudaSuccess) return e;
+    if (e != cudaSuccess) return cuda_fail(e, "dcn backward kernels");
     for (int b0 = 0; b0 < a.B; b0 += pl.chunk) {
         const int nb = a.B - b0 < pl.chunk ? a.B - b0 : pl.chunk;
         dcn_grad_cols_kernel<<<dim3((P + BN - 1) / BN, (unsigned)((K + BM - 1) / BM), nb), NT, 0, st>>>(a, b0);
@@ -436,7 +526,8 @@ cudaError_t launch_dcn_backward(DcnArgs a, const DcnPlan &pl, void *workspace, c
         dcn_reduce_splits_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(part, a.grad_weight, n, pl.splits);
     }
     dcn_grad_bias_kernel<<<a.Co, 256, 0, st>>>(a);
-    return cudaGetLastError();
+    e = cudaGetLastError();
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "dcn backward kernels");
 }
 
-} // namespace pvb
+} // extern "C"

@@ -11,7 +11,7 @@
 // is never updated); when no unselected value is > 0 the answer is index 0, selected or not, so sn > pn repeats index 0.
 //
 // Layout: one thread-block cluster of C CTAs per cloud, C in {1,2,4,8} for the whole launch: the smallest that holds the
-// largest cloud on chip, halved while the clusters would not all be resident at once (launch_fps).  CTA `rank` keeps points [rank * FPS_CTA_PTS, (rank+1) * FPS_CTA_PTS) in registers, FPS_PTS per
+// largest cloud on chip, halved while the clusters would not all be resident at once (pvb_farthest_point_sampling).  CTA `rank` keeps points [rank * FPS_CTA_PTS, (rank+1) * FPS_CTA_PTS) in registers, FPS_PTS per
 // thread (point rank * FPS_CTA_PTS + j * FPS_THREADS + t in slot j of thread t), with their min_dist.  Points from
 // cap = C * FPS_CTA_PTS on are streamed every iteration from the cloud and a min_dist array in the workspace, cap + g +
 // k * C * FPS_THREADS by cluster thread g.  A selected point's min_dist becomes -1: no distance is < -1 and -1 is not
@@ -30,7 +30,7 @@
 #include <cfloat>
 #include <climits>
 #include <vector>
-#include "kernels.h"
+#include "api.h"
 
 namespace cg = cooperative_groups;
 
@@ -278,47 +278,79 @@ int fps_max_active_clusters(int dev, int size)
 
 } // namespace
 
+// the counts [b] and starts [b] (unused under init_center) tables, then the min_dist of every cloud's points past the first
+// CTA's on-chip slice
+// External linkage on purpose: nvcc names this file's anonymous namespace, and so its kernels, after the first
+// externally visible definition in the file.
 size_t fps_workspace_bytes(int b, int n)
 {
     return fps_table_bytes(b) + (size_t)b * (size_t)std::max(0, n - FPS_CTA_PTS) * sizeof(float);
 }
 
-cudaError_t launch_fps(const float *pts, const int *counts, const int *starts, int init_center, int *idxs, int b, int n,
-                       int sn, void *workspace, cudaStream_t st)
+} // namespace pvb
+
+using namespace pvb;
+
+extern "C" {
+
+PVB_API size_t pvb_fps_workspace_bytes(int32_t b, int32_t n)
 {
+    if (b <= 0 || n <= 0) return 0;
+    return fps_workspace_bytes(b, n);
+}
+
+PVB_API int pvb_farthest_point_sampling(const float *pts, const int32_t *counts, const int32_t *starts, int32_t init_center,
+                                        int32_t *idxs, int32_t b, int32_t n, int32_t sn, void *workspace,
+                                        size_t workspace_bytes, pvb_stream_t stream)
+{
+    if (b < 0 || n < 0 || sn < 0) return fail(PVB_ERR_INVALID, "negative size (b=%d n=%d sn=%d)", b, n, sn);
+    if (b > 0x7fffffff / 8) return fail(PVB_ERR_INVALID, "b too large (got %d)", b);
+    if (b == 0 || sn == 0) return PVB_OK;
+    if (!pts || !idxs || !counts || (!init_center && !starts)) return fail(PVB_ERR_INVALID, "NULL pointer");
+    for (int32_t i = 0; i < b; ++i) {
+        if (counts[i] < 1 || counts[i] > n)
+            return fail(PVB_ERR_INVALID, "cloud %d has %d points (must be in [1, %d])", i, counts[i], n);
+        if (!init_center && (starts[i] < 0 || starts[i] >= counts[i]))
+            return fail(PVB_ERR_INVALID, "cloud %d starts at %d (must be in [0, %d))", i, starts[i], counts[i]);
+    }
+    if (int rc = check_workspace(fps_workspace_bytes(b, n), workspace, workspace_bytes)) return rc;
+    const int init = init_center != 0;
     std::vector<int> table((size_t)2 * b, 0);
     int max_count = 0;
     for (int i = 0; i < b; ++i) {
         table[i] = counts[i];
-        table[(size_t)b + i] = init_center ? 0 : starts[i];
+        table[(size_t)b + i] = init ? 0 : starts[i];
         max_count = std::max(max_count, counts[i]);
     }
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
+    if (e != cudaSuccess) return cuda_fail(e, "farthest point sampling kernel");
     int size = 1;
     while (size < FPS_MAX_CLUSTER && (long long)size * FPS_CTA_PTS < max_count) size *= 2;
     // a narrower cluster that streams more of each cloud, rather than a second wave of clusters
     while (size > 1 && b > fps_max_active_clusters(dev, size)) size /= 2;
 
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
     int *d_table = static_cast<int *>(workspace);
     float *spill = reinterpret_cast<float *>(static_cast<char *>(workspace) + fps_table_bytes(b));
     // the table is pageable host memory: the copy stages it before returning, so it may go out of scope at once
     e = cudaMemcpyAsync(d_table, table.data(), table.size() * sizeof(int), cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) return e;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)((long long)b * size));
-    cfg.blockDim = dim3(FPS_THREADS);
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = (unsigned)size;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, fps_kernel, pts, (const int *)d_table, b, n, sn, init_center, idxs, spill,
-                              (long long)std::max(0, n - FPS_CTA_PTS));
+    if (e == cudaSuccess) {
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3((unsigned)((long long)b * size));
+        cfg.blockDim = dim3(FPS_THREADS);
+        cfg.stream = st;
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = (unsigned)size;
+        attr[0].val.clusterDim.y = 1;
+        attr[0].val.clusterDim.z = 1;
+        cfg.attrs = attr;
+        cfg.numAttrs = 1;
+        e = cudaLaunchKernelEx(&cfg, fps_kernel, pts, (const int *)d_table, b, n, sn, init, idxs, spill,
+                               (long long)std::max(0, n - FPS_CTA_PTS));
+    }
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "farthest point sampling kernel");
 }
 
-} // namespace pvb
+} // extern "C"

@@ -15,10 +15,27 @@
 // multiplication by RN(1 / 2K), which is how torch divides a CUDA tensor by a CPU scalar.  The backward pass repeats
 // autograd's chain:  g2 = RN(RN(g * RN(1/2K)) / wsum);  gin = -g2 if x < -1, g2 if x > 1, else RN(x * g2);  grad = RN(gin*w).
 // Every operation is an explicit round-to-nearest intrinsic, so nvcc contracts nothing into an FMA.
+#include "api.h"
 #include "common.cuh"
-#include "kernels.h"
 
 namespace pvb {
+
+// One thread per pixel over a (ceil(H*W / 256), B) grid; the image's keypoints are staged in shared memory.
+struct VoteLossArgs {
+    const float *pred;        // [B][2K][H][W] at element strides ps (forward, backward)
+    long long ps[4];
+    const void *mask;         // [B][H][W] integer pvb_mask_dtype at element strides msb, msy, msx
+    int mask_dtype;
+    long long msb, msy, msx;
+    const double *kpt;        // [B][K][2] contiguous, (x, y) per keypoint
+    int B, H, W, K;
+    float *out;               // contiguous [B][2K][H][W]: the target field (target) or grad_pred (backward)
+    double *partial;          // [B * ceil(H*W / 256)] per-CTA sums of the smooth-l1 terms (forward)
+    long long *wpart;         // [B * ceil(H*W / 256)] per-CTA sums of the mask values (forward)
+    float *wsum;              // fp32 weight sum: written by the forward pass, read by the backward pass
+    float *loss;              // the scalar loss (forward)
+    const float *grad_loss;   // the scalar upstream gradient (backward)
+};
 
 constexpr int VL_THREADS = 256;     // one thread per pixel, consecutive pixels of a row on consecutive lanes
 
@@ -168,6 +185,11 @@ __global__ void __launch_bounds__(VL_THREADS) vote_loss_bwd_kernel(VoteLossArgs 
     }
 }
 
+namespace {
+
+constexpr int VOTE_LOSS_MAX_K = 1024;      // the image's keypoints live in 16 KB of shared memory
+
+// wsum at offset 0, then the two partial arrays, each 256-byte aligned
 size_t vote_loss_workspace_bytes(int B, int H, int W, size_t *partial_offset, size_t *wpart_offset)
 {
     const size_t nparts = (size_t)B * (((size_t)H * W + VL_THREADS - 1) / VL_THREADS);
@@ -176,8 +198,6 @@ size_t vote_loss_workspace_bytes(int B, int H, int W, size_t *partial_offset, si
     if (wpart_offset) *wpart_offset = wo;
     return wo + (nparts * sizeof(long long) + 255) / 256 * 256;
 }
-
-namespace {
 
 enum class VoteOp { Target, Forward, Backward };
 
@@ -207,19 +227,115 @@ cudaError_t launch_vote_op(VoteOp op, const VoteLossArgs &a, cudaStream_t st)
     }
 }
 
-} // namespace
-
-cudaError_t launch_vote_target(const VoteLossArgs &a, cudaStream_t st) { return launch_vote_op(VoteOp::Target, a, st); }
-
-cudaError_t launch_vote_loss_forward(const VoteLossArgs &a, cudaStream_t st)
+// the arguments every vote-loss entry shares; fills the mask, keypoint and size fields of `a`
+int vote_loss_common(VoteLossArgs &a, const void *mask, int32_t mask_dtype, const int64_t *mask_stride, const double *kpt_2d,
+                     int32_t B, int32_t H, int32_t W, int32_t K)
 {
-    cudaError_t e = launch_vote_op(VoteOp::Forward, a, st);
-    if (e != cudaSuccess) return e;
-    const long long nparts = (long long)a.B * (((long long)a.H * a.W + VL_THREADS - 1) / VL_THREADS);
-    vote_loss_final_kernel<<<1, VL_FINAL_THREADS, 0, st>>>(a.partial, a.wpart, nparts, a.K, a.wsum, a.loss);
-    return cudaGetLastError();
+    if (B < 0 || H < 0 || W < 0) return fail(PVB_ERR_INVALID, "negative size (B=%d H=%d W=%d)", B, H, W);
+    if (K < 1 || K > VOTE_LOSS_MAX_K) return fail(PVB_ERR_INVALID, "K must be in [1, %d], got %d", VOTE_LOSS_MAX_K, K);
+    if (B > 65535) return fail(PVB_ERR_INVALID, "B must be at most 65535, got %d", B);
+    if ((long long)H * W > 0x7fffffffll) return fail(PVB_ERR_INVALID, "image too large (H*W >= 2^31)");
+    if (mask_dtype < PVB_MASK_U8 || mask_dtype > PVB_MASK_I64)
+        return fail(PVB_ERR_INVALID, "mask dtype must be an integer pvb_mask_dtype (U8..I64), got %d", mask_dtype);
+    if (!mask_stride) return fail(PVB_ERR_INVALID, "NULL stride array");
+    for (int i = 0; i < 3; ++i)
+        if (mask_stride[i] < 0) return fail(PVB_ERR_INVALID, "negative stride");
+    if ((long long)B * H * W > 0 && (!mask || !kpt_2d)) return fail(PVB_ERR_INVALID, "NULL tensor");
+    a = VoteLossArgs{};
+    a.mask = mask; a.mask_dtype = mask_dtype;
+    a.msb = mask_stride[0]; a.msy = mask_stride[1]; a.msx = mask_stride[2];
+    a.kpt = kpt_2d;
+    a.B = B; a.H = H; a.W = W; a.K = K;
+    return PVB_OK;
 }
 
-cudaError_t launch_vote_loss_backward(const VoteLossArgs &a, cudaStream_t st) { return launch_vote_op(VoteOp::Backward, a, st); }
+int vote_loss_pred(VoteLossArgs &a, const float *pred, const int64_t *pred_stride)
+{
+    if (!pred_stride) return fail(PVB_ERR_INVALID, "NULL stride array");
+    for (int i = 0; i < 4; ++i) {
+        if (pred_stride[i] < 0) return fail(PVB_ERR_INVALID, "negative stride");
+        a.ps[i] = pred_stride[i];
+    }
+    if ((long long)a.B * a.H * a.W > 0 && !pred) return fail(PVB_ERR_INVALID, "NULL tensor");
+    a.pred = pred;
+    return PVB_OK;
+}
+
+// checks the workspace and fills the workspace fields of `a`
+int vote_loss_workspace(VoteLossArgs &a, const void *workspace, size_t workspace_bytes)
+{
+    size_t po = 0, wo = 0;
+    if (int rc = check_workspace(vote_loss_workspace_bytes(a.B, a.H, a.W, &po, &wo), workspace, workspace_bytes)) return rc;
+    char *ws = static_cast<char *>(const_cast<void *>(workspace));
+    a.wsum = reinterpret_cast<float *>(ws);
+    a.partial = reinterpret_cast<double *>(ws + po);
+    a.wpart = reinterpret_cast<long long *>(ws + wo);
+    return PVB_OK;
+}
+
+} // namespace
 
 } // namespace pvb
+
+using namespace pvb;
+
+extern "C" {
+
+// pvnet_data_utils.py:30-44 compute_vertex
+PVB_API int pvb_vote_target(const void *mask, int32_t mask_dtype, const int64_t *mask_stride, const double *kpt_2d,
+                            float *vertex, int32_t B, int32_t H, int32_t W, int32_t K, pvb_stream_t stream)
+{
+    VoteLossArgs a;
+    if (int rc = vote_loss_common(a, mask, mask_dtype, mask_stride, kpt_2d, B, H, W, K)) return rc;
+    if ((long long)B * H * W > 0 && !vertex) return fail(PVB_ERR_INVALID, "NULL tensor");
+    a.out = vertex;
+    cudaError_t e = launch_vote_op(VoteOp::Target, a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "vote target kernel");
+}
+
+PVB_API size_t pvb_vote_loss_workspace_bytes(int32_t B, int32_t H, int32_t W)
+{
+    if (B < 0 || H < 0 || W < 0) return 0;
+    return vote_loss_workspace_bytes(B, H, W, nullptr, nullptr);
+}
+
+// lib/train/trainers/pvnet.py:25-27, the forward pass
+PVB_API int pvb_vote_loss_forward(const float *pred, const int64_t *pred_stride, const void *mask, int32_t mask_dtype,
+                                  const int64_t *mask_stride, const double *kpt_2d, float *loss, int32_t B, int32_t H,
+                                  int32_t W, int32_t K, void *workspace, size_t workspace_bytes, pvb_stream_t stream)
+{
+    VoteLossArgs a;
+    if (int rc = vote_loss_common(a, mask, mask_dtype, mask_stride, kpt_2d, B, H, W, K)) return rc;
+    if (int rc = vote_loss_pred(a, pred, pred_stride)) return rc;
+    if (!loss) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (int rc = vote_loss_workspace(a, workspace, workspace_bytes)) return rc;
+    a.loss = loss;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    cudaError_t e = launch_vote_op(VoteOp::Forward, a, st);
+    if (e == cudaSuccess) {
+        const long long nparts = (long long)B * (((long long)H * W + VL_THREADS - 1) / VL_THREADS);
+        vote_loss_final_kernel<<<1, VL_FINAL_THREADS, 0, st>>>(a.partial, a.wpart, nparts, K, a.wsum, loss);
+        e = cudaGetLastError();
+    }
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "vote loss forward kernels");
+}
+
+// lib/train/trainers/pvnet.py:25-27, autograd's backward pass of it
+PVB_API int pvb_vote_loss_backward(const float *pred, const int64_t *pred_stride, const void *mask, int32_t mask_dtype,
+                                   const int64_t *mask_stride, const double *kpt_2d, const float *grad_loss,
+                                   float *grad_pred, int32_t B, int32_t H, int32_t W, int32_t K, const void *workspace,
+                                   size_t workspace_bytes, pvb_stream_t stream)
+{
+    VoteLossArgs a;
+    if (int rc = vote_loss_common(a, mask, mask_dtype, mask_stride, kpt_2d, B, H, W, K)) return rc;
+    if (int rc = vote_loss_pred(a, pred, pred_stride)) return rc;
+    if ((long long)B * H * W == 0) return PVB_OK;
+    if (!grad_loss || !grad_pred) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (int rc = vote_loss_workspace(a, workspace, workspace_bytes)) return rc;
+    a.grad_loss = grad_loss;
+    a.out = grad_pred;
+    cudaError_t e = launch_vote_op(VoteOp::Backward, a, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "vote loss backward kernel");
+}
+
+} // extern "C"

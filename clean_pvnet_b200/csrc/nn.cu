@@ -23,10 +23,15 @@
 // first minimum of its range for the same reason, and when no slice reports, the initial key gives index 0.
 #include <algorithm>
 #include <cfloat>
+#include "api.h"
 #include "common.cuh"
-#include "kernels.h"
 
 namespace pvb {
+
+// A problem's pn2 queries go to `qchunks` CTAs, its pn1 reference points to `nsplit` slices of `slice` points; nsplit > 1
+// (chosen from the shapes by nn_plan when b * qchunks CTAs cannot fill the GPU) merges the slices through a 64-bit key per
+// query in the workspace.
+struct NnPlan { int qchunks, nsplit, slice; };
 
 namespace {
 
@@ -370,6 +375,8 @@ __global__ void pose_final_kernel(const double *partial, const double *pose_pred
 
 } // namespace
 
+// External linkage on purpose: nvcc names this file's anonymous namespace, and so its kernels, after the first
+// externally visible definition in the file.
 NnPlan nn_plan(int b, int pn1, int pn2)
 {
     NnPlan p;
@@ -387,12 +394,23 @@ NnPlan nn_plan(int b, int pn1, int pn2)
     return p;
 }
 
+namespace {
+
+// CTAs of the widest launch; the grid is one-dimensional
+bool nn_grid_fits(int b, int pn1, int pn2)
+{
+    const NnPlan p = nn_plan(b, pn1, pn2);
+    return (long long)b * p.nsplit * p.qchunks <= 0x7fffffffll;
+}
+
+// the split path's keys [b][pn2]
 size_t nn_workspace_bytes(int b, int pn1, int pn2)
 {
     const NnPlan p = nn_plan(b, pn1, pn2);
     return p.nsplit > 1 ? (size_t)b * pn2 * sizeof(unsigned long long) : 0;
 }
 
+// ADD-S keys [n][pn] (split path only), then the per-CTA partial sums [n][qchunks] at *partial_offset
 size_t add_metric_workspace_bytes(int n, int pn, int syn, size_t *partial_offset)
 {
     const NnPlan p = nn_plan(n, pn, pn);
@@ -401,15 +419,37 @@ size_t add_metric_workspace_bytes(int n, int pn, int syn, size_t *partial_offset
     return keys + (size_t)n * p.qchunks * sizeof(double);
 }
 
+// the per-CTA partial sums [n][ceil(pn / NN_QPB)] of the reprojection distances
 size_t pose_metrics_workspace_bytes(int n, int pn)
 {
     return (size_t)n * ((pn + NN_QPB - 1) / NN_QPB) * sizeof(double);
 }
 
-cudaError_t launch_nearest_point(const float *ref, const float *que, int *idxs, int b, int pn1, int pn2, int dim,
-                                 bool exclude_self, void *workspace, cudaStream_t st)
+} // namespace
+
+} // namespace pvb
+
+using namespace pvb;
+
+extern "C" {
+
+PVB_API size_t pvb_nearest_point_workspace_bytes(int32_t b, int32_t pn1, int32_t pn2)
 {
-    if (b <= 0 || pn2 <= 0) return cudaSuccess;
+    if (b <= 0 || pn1 < 0 || pn2 <= 0) return 0;
+    return nn_workspace_bytes(b, pn1, pn2);
+}
+
+PVB_API int pvb_nearest_point_idx(const float *ref, const float *que, int32_t *idxs, int32_t b, int32_t pn1, int32_t pn2,
+                                  int32_t dim, int32_t exclude_self, void *workspace, size_t workspace_bytes,
+                                  pvb_stream_t stream)
+{
+    if (b < 0 || pn1 < 0 || pn2 < 0) return fail(PVB_ERR_INVALID, "negative size (b=%d pn1=%d pn2=%d)", b, pn1, pn2);
+    if (dim != 2 && dim != 3) return fail(PVB_ERR_INVALID, "dim must be 2 or 3 (got %d)", dim);
+    if (b == 0 || pn2 == 0) return PVB_OK;
+    if (!que || !idxs || (pn1 > 0 && !ref)) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (!nn_grid_fits(b, pn1, pn2)) return fail(PVB_ERR_INVALID, "b * pn2 too large");
+    if (int rc = check_workspace(nn_workspace_bytes(b, pn1, pn2), workspace, workspace_bytes)) return rc;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
     NnArgs a;
     a.ref = ref; a.que = que; a.idxs = idxs; a.pn1 = pn1; a.pn2 = pn2;
     a.plan = nn_plan(b, pn1, pn2);
@@ -424,18 +464,30 @@ cudaError_t launch_nearest_point(const float *ref, const float *que, int *idxs, 
     else { if (exclude_self) PVB_NN_LAUNCH(2, true); else PVB_NN_LAUNCH(2, false); }
 #undef PVB_NN_LAUNCH
     if (split) nn_key_index_kernel<<<grid_stride_blocks(nq), 256, 0, st>>>(a.keys, idxs, nq);
-    return cudaGetLastError();
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "nearest point kernels");
 }
 
-cudaError_t launch_add_metric(const double *model, const double *pose_pred, const double *pose_gt, double *mean_dist, int n,
-                              int pn, bool syn, void *workspace, cudaStream_t st)
+PVB_API size_t pvb_add_metric_workspace_bytes(int32_t n, int32_t pn, int32_t syn)
 {
-    if (n <= 0) return cudaSuccess;
+    if (n <= 0 || pn < 0 || (syn != 0 && syn != 1)) return 0;
+    return add_metric_workspace_bytes(n, pn, syn, nullptr);
+}
+
+PVB_API int pvb_add_metric(const double *model, const double *pose_pred, const double *pose_gt, double *mean_dist, int32_t n,
+                           int32_t pn, int32_t syn, void *workspace, size_t workspace_bytes, pvb_stream_t stream)
+{
+    if (n < 0 || pn < 0) return fail(PVB_ERR_INVALID, "negative size (n=%d pn=%d)", n, pn);
+    if (syn != 0 && syn != 1) return fail(PVB_ERR_INVALID, "syn must be 0 or 1 (got %d)", syn);
+    if (n == 0) return PVB_OK;
+    if (!pose_pred || !pose_gt || !mean_dist || (pn > 0 && !model)) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (!nn_grid_fits(n, pn, pn)) return fail(PVB_ERR_INVALID, "n * pn too large");
+    size_t off;
+    if (int rc = check_workspace(add_metric_workspace_bytes(n, pn, syn, &off), workspace, workspace_bytes)) return rc;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
     AddArgs a;
     a.model = model; a.pose_pred = pose_pred; a.pose_gt = pose_gt; a.mean = mean_dist; a.pn = pn;
     a.plan = nn_plan(n, pn, pn);
-    size_t off;
-    add_metric_workspace_bytes(n, pn, syn, &off);
     a.keys = static_cast<unsigned long long *>(workspace);
     a.partial = reinterpret_cast<double *>(static_cast<char *>(workspace) + off);
     const unsigned dist_grid = (unsigned)((size_t)n * a.plan.qchunks);
@@ -452,14 +504,28 @@ cudaError_t launch_add_metric(const double *model, const double *pose_pred, cons
         }
     }
     add_mean_kernel<<<(n + 7) / 8, 256, 0, st>>>(a.partial, mean_dist, n, a.plan.qchunks, pn);
-    return cudaGetLastError();
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "add metric kernels");
 }
 
-cudaError_t launch_pose_metrics(const double *model, const double *pose_pred, const double *pose_gt, const double *K,
-                                long long k_stride, double *proj2d, double *trans_cm, double *angle_deg, int n, int pn,
-                                void *workspace, cudaStream_t st)
+PVB_API size_t pvb_pose_metrics_workspace_bytes(int32_t n, int32_t pn)
 {
-    if (n <= 0) return cudaSuccess;
+    if (n <= 0 || pn < 0) return 0;
+    return pose_metrics_workspace_bytes(n, pn);
+}
+
+PVB_API int pvb_pose_metrics(const double *model, const double *pose_pred, const double *pose_gt, const double *K,
+                             int64_t k_stride, double *proj2d, double *trans_cm, double *angle_deg, int32_t n, int32_t pn,
+                             void *workspace, size_t workspace_bytes, pvb_stream_t stream)
+{
+    if (n < 0 || pn < 0) return fail(PVB_ERR_INVALID, "negative size (n=%d pn=%d)", n, pn);
+    if (n == 0) return PVB_OK;
+    if (!pose_pred || !pose_gt || !K || !proj2d || !trans_cm || !angle_deg || (pn > 0 && !model))
+        return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (k_stride < 0) return fail(PVB_ERR_INVALID, "negative stride");
+    if (!nn_grid_fits(n, pn, pn)) return fail(PVB_ERR_INVALID, "n * pn too large");
+    if (int rc = check_workspace(pose_metrics_workspace_bytes(n, pn), workspace, workspace_bytes)) return rc;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
     AddArgs a = {};
     a.model = model; a.pose_pred = pose_pred; a.pose_gt = pose_gt; a.pn = pn;
     a.plan.qchunks = (pn + NN_QPB - 1) / NN_QPB; a.plan.nsplit = 1; a.plan.slice = pn;
@@ -467,7 +533,8 @@ cudaError_t launch_pose_metrics(const double *model, const double *pose_pred, co
     if (pn > 0) proj_dist_kernel<<<(unsigned)((size_t)n * a.plan.qchunks), NN_THREADS, 0, st>>>(a, K, k_stride);
     pose_final_kernel<<<(n + 7) / 8, 256, 0, st>>>(a.partial, pose_pred, pose_gt, proj2d, trans_cm, angle_deg, n,
                                                   a.plan.qchunks, pn);
-    return cudaGetLastError();
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "pose metric kernels");
 }
 
-} // namespace pvb
+} // extern "C"

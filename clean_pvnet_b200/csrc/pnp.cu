@@ -7,13 +7,36 @@
 // an XOR butterfly (every lane ends with the same bits, so all lanes run the identical trust-region state machine without
 // divergence or broadcasts).  Everything is fp64 like the reference.  Latency-bound by design: ~10 evaluations per problem.
 #include <math_constants.h>
+#include "api.h"
 #include "common.cuh"
-#include "kernels.h"
 #include "pnp_core.cuh"
 #include "p3p_core.cuh"
 #include "pnp_iter_core.cuh"
 
 namespace pvb {
+
+// Batched uncertainty PnP: n problems of pn points, one warp per problem, fp64 like the reference.  The 2D inputs are either
+// fp64 pts2d + wgt2d, read in place, or (kpt2d != NULL) the voting layer's fp32 keypoints with their covariances or
+// weights, converted into shared memory (pn <= PNP_FUSED_MAX_PN).
+constexpr int PNP_FUSED_MAX_PN = 64;
+struct PnpArgs {
+    const double *pts2d;      // [n][pn][2]
+    const double *wgt2d;      // [n][pn][3]  (wxx, wxy, wyy)
+    const float *kpt2d;       // [n][pn][2]  (the voting layer's kpt_2d)
+    const float *cov;         // [n][pn][2][2] (the voting layer's var), or NULL ...
+    const float *weights;     // ... then [n][pn][3] precomputed (wxx, wxy, wyy)
+    float *weights_out;       // optional [n][pn][3]: the fp32 weights used (kpt2d only)
+    const double *pts3d;      // [pn][3], problem p at pts3d + p*pts3d_stride (0: shared)
+    const double *K;          // [3][3] row-major, problem p at K + p*k_stride (0: shared)
+    const double *init_rt;    // optional [n][6]; NULL: P3P on the four best-weighted points
+    double *init_out;         // optional [n][6]: the initial pose that was used
+    double *result_rt;        // [n][6]: the refined pose; NULL: the P3P start alone (fp64 inputs, into init_out)
+    int *info;                // optional [n][2]: iterations, termination code
+    double *pose;             // [n][3][4]: the pose of pvb_pnp_iterative (pnp_iter_kernel only)
+    int n, pn;
+    long long pts3d_stride, k_stride;
+    PnpOptions opt;
+};
 
 // ---------------------------------------------------------------------------------
 // SURVEY 8f row 2: weights of the uncertainty PnP, inv(sqrtm(cov)) per keypoint packed as (wxx, wxy, wyy)
@@ -27,13 +50,6 @@ pnp_weights_kernel(const float *__restrict__ cov, float *__restrict__ w, int n)
     float o0, o1, o2;
     cov_to_weights(__ldg(reinterpret_cast<const float4 *>(cov) + i), o0, o1, o2);
     w[(size_t)i * 3] = o0; w[(size_t)i * 3 + 1] = o1; w[(size_t)i * 3 + 2] = o2;
-}
-
-cudaError_t launch_pnp_weights(const float *cov, float *w, int n, cudaStream_t st)
-{
-    if (n <= 0) return cudaSuccess;
-    pnp_weights_kernel<<<(n + 127) / 128, 128, 0, st>>>(cov, w, n);
-    return cudaGetLastError();
 }
 
 // sum of C numbers over the warp by an XOR butterfly, in place: every lane ends with the same bits
@@ -170,24 +186,125 @@ pnp_iter_kernel(PnpArgs a)
     if (a.info && lane == 31) { a.info[2 * prob] = iterations; a.info[2 * prob + 1] = status; }
 }
 
-cudaError_t launch_pnp_iterative(const PnpArgs &a, cudaStream_t st)
+namespace {
+
+// The checks every PnP entry point makes after its own ones on n and pn: NULL tensors (`given`: every required pointer is
+// set), then the strides.
+int pnp_check_inputs(int32_t n, bool given, int64_t pts3d_stride, int64_t k_stride)
 {
-    if (a.n <= 0) return cudaSuccess;
-    pnp_iter_kernel<<<(a.n + PNP_WARPS - 1) / PNP_WARPS, PNP_WARPS * 32, 0, st>>>(a);
-    return cudaGetLastError();
+    if (n && !given) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (pts3d_stride < 0 || k_stride < 0) return fail(PVB_ERR_INVALID, "negative stride");
+    return PVB_OK;
 }
 
-cudaError_t launch_pnp_batch(const PnpArgs &a, cudaStream_t st)
+// options == NULL: Ceres' defaults
+int pnp_read_options(const pvb_pnp_options *options, PnpOptions &opt)
 {
-    if (a.n <= 0) return cudaSuccess;
-    if (!a.result_rt) {
-        p3p_start_kernel<<<(a.n + 63) / 64, 64, 0, st>>>(a);
-        return cudaGetLastError();
-    }
-    const int blocks = (a.n + PNP_WARPS - 1) / PNP_WARPS;
-    if (a.kpt2d) pnp_batch_kernel<PnpInput::Fp32Staged><<<blocks, PNP_WARPS * 32, 0, st>>>(a);
-    else pnp_batch_kernel<PnpInput::Fp64><<<blocks, PNP_WARPS * 32, 0, st>>>(a);
-    return cudaGetLastError();
+    opt = pnp_default_options();
+    if (!options) return PVB_OK;
+    if (options->max_num_iterations < 0 || !(options->function_tolerance >= 0.0) || !(options->gradient_tolerance >= 0.0) ||
+        !(options->parameter_tolerance >= 0.0))
+        return fail(PVB_ERR_INVALID, "pvb_pnp_options: negative or NaN entry");
+    opt.max_num_iterations = options->max_num_iterations; opt.function_tolerance = options->function_tolerance;
+    opt.gradient_tolerance = options->gradient_tolerance; opt.parameter_tolerance = options->parameter_tolerance;
+    return PVB_OK;
 }
+
+} // namespace
 
 } // namespace pvb
+
+using namespace pvb;
+
+extern "C" {
+
+PVB_API int pvb_uncertainty_weights(const float *cov, float *weights, int32_t n, pvb_stream_t stream)
+{
+    if (n < 0) return fail(PVB_ERR_INVALID, "n < 0");
+    if (n && (!cov || !weights)) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (reinterpret_cast<uintptr_t>(cov) & 15u) return fail(PVB_ERR_INVALID, "cov must be 16-byte aligned");
+    if (n == 0) return PVB_OK;
+    pnp_weights_kernel<<<(n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(cov, weights, n);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "pnp weights kernel");
+}
+
+PVB_API int pvb_uncertainty_pnp(const double *pts2d, const double *pts3d, const double *wgt2d, const double *K,
+                                const double *init_rt, double *result_rt, int32_t *info, int32_t n, int32_t pn,
+                                int64_t pts3d_stride, int64_t k_stride, const pvb_pnp_options *options, pvb_stream_t stream)
+{
+    if (n < 0) return fail(PVB_ERR_INVALID, "n < 0");
+    if (pn < 1) return fail(PVB_ERR_INVALID, "pn must be >= 1 (got %d)", pn);
+    PnpArgs a = {};
+    if (int rc = pnp_check_inputs(n, pts2d && pts3d && wgt2d && K && init_rt && result_rt, pts3d_stride, k_stride)) return rc;
+    if (int rc = pnp_read_options(options, a.opt)) return rc;
+    if (n == 0) return PVB_OK;
+    a.pts2d = pts2d; a.wgt2d = wgt2d; a.pts3d = pts3d; a.K = K; a.init_rt = init_rt; a.result_rt = result_rt; a.info = info;
+    a.n = n; a.pn = pn; a.pts3d_stride = pts3d_stride; a.k_stride = k_stride;
+    pnp_batch_kernel<PnpInput::Fp64>
+        <<<(n + PNP_WARPS - 1) / PNP_WARPS, PNP_WARPS * 32, 0, static_cast<cudaStream_t>(stream)>>>(a);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "uncertainty pnp kernel");
+}
+
+PVB_API int pvb_uncertainty_pnp_from_votes(const float *kpt_2d, const float *cov, const float *weights, const double *pts3d,
+                                           const double *K, const double *init_rt, double *result_rt, double *init_out,
+                                           float *weights_out, int32_t *info, int32_t n, int32_t pn, int64_t pts3d_stride,
+                                           int64_t k_stride, const pvb_pnp_options *options, pvb_stream_t stream)
+{
+    if (n < 0) return fail(PVB_ERR_INVALID, "n < 0");
+    if (pn < 1 || pn > PNP_FUSED_MAX_PN) return fail(PVB_ERR_INVALID, "pn must be in [1,%d] (got %d)", PNP_FUSED_MAX_PN, pn);
+    if (!init_rt && pn < 4) return fail(PVB_ERR_INVALID, "the P3P initialisation needs pn >= 4 (got %d)", pn);
+    const bool given = kpt_2d && pts3d && K && result_rt;
+    // before pnp_check_inputs, but only once every required tensor is set: a caller keeps getting "NULL tensor" first,
+    // then this, then "negative stride"
+    if (n && given && ((cov == nullptr) == (weights == nullptr)))
+        return fail(PVB_ERR_INVALID, "pass exactly one of cov / weights");
+    PnpArgs a = {};
+    if (int rc = pnp_check_inputs(n, given, pts3d_stride, k_stride)) return rc;
+    if ((reinterpret_cast<uintptr_t>(kpt_2d) & 7u) || (reinterpret_cast<uintptr_t>(cov) & 15u))
+        return fail(PVB_ERR_INVALID, "kpt_2d must be 8-byte and cov 16-byte aligned");
+    if (int rc = pnp_read_options(options, a.opt)) return rc;
+    if (n == 0) return PVB_OK;
+    a.kpt2d = kpt_2d; a.cov = cov; a.weights = weights; a.weights_out = weights_out; a.pts3d = pts3d; a.K = K;
+    a.init_rt = init_rt; a.init_out = init_out; a.result_rt = result_rt; a.info = info;
+    a.n = n; a.pn = pn; a.pts3d_stride = pts3d_stride; a.k_stride = k_stride;
+    pnp_batch_kernel<PnpInput::Fp32Staged>
+        <<<(n + PNP_WARPS - 1) / PNP_WARPS, PNP_WARPS * 32, 0, static_cast<cudaStream_t>(stream)>>>(a);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "fused uncertainty pnp kernel");
+}
+
+PVB_API int pvb_uncertainty_pnp_init(const double *pts2d, const double *pts3d, const double *wgt2d, const double *K,
+                                     double *init_rt, int32_t n, int32_t pn, int64_t pts3d_stride, int64_t k_stride,
+                                     pvb_stream_t stream)
+{
+    if (n < 0) return fail(PVB_ERR_INVALID, "n < 0");
+    if (pn < 4) return fail(PVB_ERR_INVALID, "P3P needs pn >= 4 (got %d)", pn);
+    if (int rc = pnp_check_inputs(n, pts2d && pts3d && wgt2d && K && init_rt, pts3d_stride, k_stride)) return rc;
+    if (n == 0) return PVB_OK;
+    PnpArgs a = {};                    // no result_rt: the P3P start alone, written to init_out
+    a.pts2d = pts2d; a.wgt2d = wgt2d; a.pts3d = pts3d; a.K = K; a.init_out = init_rt;
+    a.n = n; a.pn = pn; a.pts3d_stride = pts3d_stride; a.k_stride = k_stride;
+    p3p_start_kernel<<<(n + 63) / 64, 64, 0, static_cast<cudaStream_t>(stream)>>>(a);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "p3p init kernel");
+}
+
+PVB_API int pvb_pnp_iterative(const double *pts2d, const double *pts3d, const double *K, double *pose, double *rt,
+                              int32_t *info, int32_t n, int32_t pn, int64_t pts3d_stride, int64_t k_stride,
+                              pvb_stream_t stream)
+{
+    if (n < 0) return fail(PVB_ERR_INVALID, "n < 0");
+    if (pn < 1) return fail(PVB_ERR_INVALID, "pn must be >= 1 (got %d)", pn);
+    if (int rc = pnp_check_inputs(n, pts2d && pts3d && K && pose, pts3d_stride, k_stride)) return rc;
+    if (n == 0) return PVB_OK;
+    PnpArgs a = {};
+    a.pts2d = pts2d; a.pts3d = pts3d; a.K = K; a.pose = pose; a.result_rt = rt; a.info = info;
+    a.n = n; a.pn = pn; a.pts3d_stride = pts3d_stride; a.k_stride = k_stride;
+    pnp_iter_kernel<<<(n + PNP_WARPS - 1) / PNP_WARPS, PNP_WARPS * 32, 0, static_cast<cudaStream_t>(stream)>>>(a);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "iterative pnp kernel");
+}
+
+} // extern "C"

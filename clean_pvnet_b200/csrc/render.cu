@@ -22,9 +22,23 @@
 // Depth is kept by atomicMin on the bits of the positive fp32 Z in an image filled with +inf, then +inf becomes 0; the
 // minimum does not depend on the order of the atomics, so the output is bit-identical run to run and each pose's image
 // depends on nothing else in the batch.
-#include "kernels.h"
+#include <algorithm>
+#include <cmath>
+#include <vector>
+#include "api.h"
 
 namespace pvb {
+
+struct VsdArgs {
+    const float *depth_test, *depth_est, *depth_gt;  // [B][H][W], [n_est][H][W], [n_gt][H][W]
+    const int *pairs;                                // [n][3]: est index, gt index, image index
+    const double *K;                                 // [3][3] per image at K + image * k_stride
+    long long k_stride;
+    int n, B, n_est, n_gt, est_base, gt_base, H, W;  // rows use est in [est_base, est_base + n_est), likewise gt
+    double delta, tau;
+    double *e;                                       // [n]: written only for rows within the windows
+};
+
 namespace {
 
 constexpr int RENDER_THREADS = 256;
@@ -331,6 +345,7 @@ __global__ void vsd_final_kernel(VsdArgs a, const VsdCounts *__restrict__ counts
 constexpr int MASK_THREADS = 256;
 constexpr int MASK_PPT = 8;                            // pixels per thread
 constexpr int MASK_PIXELS = MASK_THREADS * MASK_PPT;
+constexpr int MASK_MAX_INSTANCES = 2048;              // per image: their sums take 48 KB of shared memory
 
 // per-instance sums; the box is kept as maxima of W - x, x + 1, H - y, y + 1, which are all 0 for an empty mask, so the
 // sums start from a zero fill
@@ -427,79 +442,189 @@ __global__ void mask_finish_kernel(const MaskAcc *__restrict__ acc, int m, int H
 
 } // namespace
 
+// a queue counter, then the n * F queue entries
+// External linkage on purpose: nvcc names this file's anonymous namespace, and so its kernels, after the first
+// externally visible definition in the file.
 size_t render_workspace_bytes(int n, int F)
 {
     return 256 + (((size_t)n * (size_t)F * sizeof(unsigned) + 255) / 256) * 256;
 }
 
-cudaError_t launch_render_depth(const float *pts, int V, const int *faces, int F, const double *poses, int n,
-                                const double *K, long long k_stride, float *depth, int H, int W, double znear,
-                                double zfar, void *workspace, cudaStream_t st)
-{
-    unsigned *img = reinterpret_cast<unsigned *>(depth);
-    const long long total = (long long)n * H * W;
-    render_fill_kernel<<<stream_grid(total), RENDER_THREADS, 0, st>>>(img, total, RENDER_BG);
-    if (F > 0) {
-        unsigned *queue_len = static_cast<unsigned *>(workspace);
-        unsigned *queue = reinterpret_cast<unsigned *>(static_cast<char *>(workspace) + 256);
-        cudaError_t e = cudaMemsetAsync(queue_len, 0, sizeof(unsigned), st);
-        if (e != cudaSuccess) return e;
-        render_small_kernel<<<dim3((unsigned)((F + RENDER_THREADS - 1) / RENDER_THREADS), (unsigned)n), RENDER_THREADS,
-                              0, st>>>(pts, V, faces, F, poses, K, k_stride, H, W, znear, zfar, img, queue_len, queue);
-        const long long nq = (long long)n * F;
-        render_big_kernel<<<(unsigned)(nq < 132 * 8 ? nq : 132 * 8), RENDER_THREADS, 0, st>>>(
-            pts, V, faces, F, poses, K, k_stride, H, W, znear, zfar, img, queue_len, queue);
-    }
-    render_finish_kernel<<<stream_grid(total), RENDER_THREADS, 0, st>>>(img, total);
-    return cudaGetLastError();
-}
+namespace {
 
+// the integer counts of the n rows
 size_t vsd_workspace_bytes(int n)
 {
     return (((size_t)n * sizeof(VsdCounts) + 255) / 256) * 256;
 }
 
-cudaError_t launch_vsd(const VsdArgs &a, void *workspace, cudaStream_t st)
-{
-    VsdCounts *counts = static_cast<VsdCounts *>(workspace);
-    cudaError_t e = cudaMemsetAsync(counts, 0, (size_t)a.n * sizeof(VsdCounts), st);
-    if (e != cudaSuccess) return e;
-    const int chunks = (a.H * a.W + VSD_PIXELS - 1) / VSD_PIXELS;
-    if (chunks > 0)
-        vsd_count_kernel<<<dim3((unsigned)chunks, (unsigned)(a.n < 65535 ? a.n : 65535)), VSD_THREADS, 0, st>>>(a, counts);
-    vsd_final_kernel<<<(unsigned)((a.n + 255) / 256), 256, 0, st>>>(a, counts);
-    return cudaGetLastError();
-}
-
-namespace {
 size_t mask_table_bytes(int B, int m)
 {
     return (((size_t)B + 1 + 2 * (size_t)m) * sizeof(int) + 255) / 256 * 256;
 }
-} // namespace
 
+// the table, then the integer sums of the m instances
 size_t instance_masks_workspace_bytes(int B, int m)
 {
     return mask_table_bytes(B, m) + ((size_t)m * sizeof(MaskAcc) + 255) / 256 * 256;
 }
 
-cudaError_t launch_instance_masks(const float *depth, const int *table, int B, int m, int max_m, int H, int W,
-                                  short *label, long long *a_out, long long *p_out, int *box_out, void *workspace,
-                                  cudaStream_t st)
-{
-    int *d_table = static_cast<int *>(workspace);
-    MaskAcc *acc = reinterpret_cast<MaskAcc *>(static_cast<char *>(workspace) + mask_table_bytes(B, m));
-    // the table is pageable host memory: the copy stages it before returning, so the caller may free it at once
-    cudaError_t e = cudaMemcpyAsync(d_table, table, ((size_t)B + 1 + 2 * (size_t)m) * sizeof(int), cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) return e;
-    e = cudaMemsetAsync(acc, 0, (size_t)m * sizeof(MaskAcc), st);
-    if (e != cudaSuccess) return e;
-    const int chunks = (H * W + MASK_PIXELS - 1) / MASK_PIXELS;
-    if (chunks > 0)
-        mask_compose_kernel<<<dim3((unsigned)chunks, (unsigned)B), MASK_THREADS, (size_t)max_m * sizeof(MaskAcc), st>>>(
-            depth, d_table, B, m, H, W, label, acc);
-    mask_finish_kernel<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(acc, m, H, W, a_out, p_out, box_out);
-    return cudaGetLastError();
-}
+} // namespace
 
 } // namespace pvb
+
+using namespace pvb;
+
+extern "C" {
+
+PVB_API size_t pvb_render_depth_workspace_bytes(int32_t n, int32_t F)
+{
+    if (n <= 0 || F <= 0 || (long long)n * F > 0x7fffffffll) return 0;
+    return render_workspace_bytes(n, F);
+}
+
+PVB_API int pvb_render_depth(const float *pts, int32_t V, const int32_t *faces, int32_t F, const double *poses, int32_t n,
+                             const double *K, int64_t k_stride, float *depth, int32_t H, int32_t W, double clip_near,
+                             double clip_far, void *workspace, size_t workspace_bytes, pvb_stream_t stream)
+{
+    if (n < 0 || V < 0 || F < 0 || H < 0 || W < 0)
+        return fail(PVB_ERR_INVALID, "negative size (n=%d V=%d F=%d H=%d W=%d)", n, V, F, H, W);
+    if (!(clip_near > 0.0) || !(clip_far >= clip_near) || !std::isfinite(clip_far))
+        return fail(PVB_ERR_INVALID, "need 0 < near <= far < inf (got %g, %g)", clip_near, clip_far);
+    if ((long long)H * W > 0x7fffffffll) return fail(PVB_ERR_INVALID, "image too large (H*W >= 2^31)");
+    if ((long long)n * F > 0x7fffffffll) return fail(PVB_ERR_INVALID, "n * F too large (>= 2^31)");
+    if (n > 65535) return fail(PVB_ERR_INVALID, "n must be <= 65535 (got %d)", n);
+    if (n == 0 || (long long)H * W == 0) return PVB_OK;
+    if (!poses || !K || !depth || (F > 0 && (!faces || (V > 0 && !pts)))) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (k_stride < 0) return fail(PVB_ERR_INVALID, "negative stride");
+    if (F > 0)
+        if (int rc = check_workspace(render_workspace_bytes(n, F), workspace, workspace_bytes)) return rc;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    unsigned *img = reinterpret_cast<unsigned *>(depth);
+    const long long total = (long long)n * H * W;
+    render_fill_kernel<<<stream_grid(total), RENDER_THREADS, 0, st>>>(img, total, RENDER_BG);
+    cudaError_t e = cudaSuccess;
+    if (F > 0) {
+        unsigned *queue_len = static_cast<unsigned *>(workspace);
+        unsigned *queue = reinterpret_cast<unsigned *>(static_cast<char *>(workspace) + 256);
+        e = cudaMemsetAsync(queue_len, 0, sizeof(unsigned), st);
+        if (e == cudaSuccess) {
+            render_small_kernel<<<dim3((unsigned)((F + RENDER_THREADS - 1) / RENDER_THREADS), (unsigned)n), RENDER_THREADS,
+                                  0, st>>>(pts, V, faces, F, poses, K, k_stride, H, W, clip_near, clip_far, img, queue_len,
+                                           queue);
+            const long long nq = (long long)n * F;
+            render_big_kernel<<<(unsigned)(nq < 132 * 8 ? nq : 132 * 8), RENDER_THREADS, 0, st>>>(
+                pts, V, faces, F, poses, K, k_stride, H, W, clip_near, clip_far, img, queue_len, queue);
+        }
+    }
+    if (e == cudaSuccess) {
+        render_finish_kernel<<<stream_grid(total), RENDER_THREADS, 0, st>>>(img, total);
+        e = cudaGetLastError();
+    }
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "depth render kernels");
+}
+
+PVB_API size_t pvb_vsd_workspace_bytes(int32_t n)
+{
+    if (n <= 0) return 0;
+    return vsd_workspace_bytes(n);
+}
+
+PVB_API int pvb_vsd(const float *depth_test, int32_t B, const float *depth_est, int32_t n_est, int32_t est_base,
+                    const float *depth_gt, int32_t n_gt, int32_t gt_base, const int32_t *pairs, int32_t n, const double *K,
+                    int64_t k_stride, int32_t H, int32_t W, double delta, double tau, double *e, void *workspace,
+                    size_t workspace_bytes, pvb_stream_t stream)
+{
+    if (n < 0 || B < 0 || n_est < 0 || n_gt < 0 || H < 0 || W < 0)
+        return fail(PVB_ERR_INVALID, "negative size (n=%d B=%d n_est=%d n_gt=%d H=%d W=%d)", n, B, n_est, n_gt, H, W);
+    if ((long long)H * W > 0x7fffffffll) return fail(PVB_ERR_INVALID, "image too large (H*W >= 2^31)");
+    if (std::isnan(delta) || std::isnan(tau)) return fail(PVB_ERR_INVALID, "delta and tau must not be NaN");
+    if (n == 0) return PVB_OK;
+    const bool px = (long long)H * W > 0;
+    if (!pairs || !e || !K || (px && ((B > 0 && !depth_test) || (n_est > 0 && !depth_est) || (n_gt > 0 && !depth_gt))))
+        return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (k_stride < 0) return fail(PVB_ERR_INVALID, "negative stride");
+    if (int rc = check_workspace(vsd_workspace_bytes(n), workspace, workspace_bytes)) return rc;
+    VsdArgs a;
+    a.depth_test = depth_test; a.depth_est = depth_est; a.depth_gt = depth_gt; a.pairs = pairs; a.K = K;
+    a.k_stride = k_stride; a.n = n; a.B = B; a.n_est = n_est; a.n_gt = n_gt; a.est_base = est_base; a.gt_base = gt_base;
+    a.H = H; a.W = W; a.delta = delta; a.tau = tau; a.e = e;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    VsdCounts *counts = static_cast<VsdCounts *>(workspace);
+    cudaError_t err = cudaMemsetAsync(counts, 0, (size_t)n * sizeof(VsdCounts), st);
+    if (err == cudaSuccess) {
+        const int chunks = (H * W + VSD_PIXELS - 1) / VSD_PIXELS;
+        if (chunks > 0)
+            vsd_count_kernel<<<dim3((unsigned)chunks, (unsigned)(n < 65535 ? n : 65535)), VSD_THREADS, 0, st>>>(a, counts);
+        vsd_final_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, counts);
+        err = cudaGetLastError();
+    }
+    return err == cudaSuccess ? PVB_OK : cuda_fail(err, "vsd kernels");
+}
+
+PVB_API size_t pvb_instance_masks_workspace_bytes(int32_t B, int32_t m)
+{
+    if (B <= 0 || m <= 0) return 0;
+    return instance_masks_workspace_bytes(B, m);
+}
+
+PVB_API int pvb_instance_masks(const float *depth, int32_t n_depth, const int32_t *slot, const int32_t *obj_id, int32_t n,
+                               const int32_t *image_first, int32_t B, int32_t H, int32_t W, int16_t *label,
+                               int64_t *a_pixel_num, int64_t *pixel_num, int32_t *bbox, void *workspace,
+                               size_t workspace_bytes, pvb_stream_t stream)
+{
+    if (n_depth < 0 || n < 0 || B < 0 || H < 0 || W < 0)
+        return fail(PVB_ERR_INVALID, "negative size (n_depth=%d n=%d B=%d H=%d W=%d)", n_depth, n, B, H, W);
+    if ((long long)H * W > 0x7fffffffll) return fail(PVB_ERR_INVALID, "image too large (H*W >= 2^31)");
+    if (B > 65535) return fail(PVB_ERR_INVALID, "B must be <= 65535 (got %d)", B);
+    if (B == 0) return PVB_OK;
+    if (!image_first || !slot || !obj_id) return fail(PVB_ERR_INVALID, "NULL host table");
+    const bool px = (long long)H * W > 0;
+    if (!a_pixel_num || !pixel_num || !bbox || (px && (!depth || !label))) return fail(PVB_ERR_INVALID, "NULL tensor");
+    const int32_t i0 = image_first[0];
+    if (i0 < 0) return fail(PVB_ERR_INVALID, "image 0's instances start at %d", i0);
+    int max_m = 0;
+    for (int32_t b = 0; b < B; ++b) {
+        const int32_t lo = image_first[b], hi = image_first[b + 1];
+        if (hi <= lo || hi > n)
+            return fail(PVB_ERR_INVALID, "image %d's instance range [%d, %d) is empty or outside [0, %d)", b, lo, hi, n);
+        if (hi - lo > MASK_MAX_INSTANCES)
+            return fail(PVB_ERR_INVALID, "image %d has %d instances (at most %d)", b, hi - lo, MASK_MAX_INSTANCES);
+        max_m = std::max(max_m, hi - lo);
+    }
+    // the kernels' table: image b's instances are [table[b], table[b+1]) (table[0] == 0), then the depth slot of each of
+    // the m instances, then its label
+    const int32_t m = image_first[B] - i0;
+    std::vector<int32_t> table((size_t)B + 1 + 2 * (size_t)m);
+    for (int32_t b = 0; b <= B; ++b) table[b] = image_first[b] - i0;
+    for (int32_t b = 0; b < B; ++b)
+        for (int32_t i = image_first[b]; i < image_first[b + 1]; ++i) {
+            if (slot[i] < 0 || slot[i] >= n_depth)
+                return fail(PVB_ERR_INVALID, "instance %d reads depth slot %d (outside [0, %d))", i, slot[i], n_depth);
+            const long long lab = (long long)obj_id[i] * 1000 + (i - image_first[b]);
+            if (lab < -32768 || lab > 32767)
+                return fail(PVB_ERR_INVALID, "instance %d's label %lld (obj_id * 1000 + instance_id) does not fit int16", i, lab);
+            table[B + 1 + (i - i0)] = slot[i];
+            table[B + 1 + m + (i - i0)] = (int32_t)lab;
+        }
+    if (int rc = check_workspace(instance_masks_workspace_bytes(B, m), workspace, workspace_bytes)) return rc;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int *d_table = static_cast<int *>(workspace);
+    MaskAcc *acc = reinterpret_cast<MaskAcc *>(static_cast<char *>(workspace) + mask_table_bytes(B, m));
+    // the table is pageable host memory: the copy stages it before returning, so it may go out of scope at once
+    cudaError_t e = cudaMemcpyAsync(d_table, table.data(), table.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(acc, 0, (size_t)m * sizeof(MaskAcc), st);
+    if (e == cudaSuccess) {
+        const int chunks = (H * W + MASK_PIXELS - 1) / MASK_PIXELS;
+        if (chunks > 0)
+            mask_compose_kernel<<<dim3((unsigned)chunks, (unsigned)B), MASK_THREADS, (size_t)max_m * sizeof(MaskAcc), st>>>(
+                depth, d_table, B, m, H, W, reinterpret_cast<short *>(label), acc);
+        mask_finish_kernel<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(
+            acc, m, H, W, reinterpret_cast<long long *>(a_pixel_num) + i0, reinterpret_cast<long long *>(pixel_num) + i0,
+            bbox + 4ll * i0);
+        e = cudaGetLastError();
+    }
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "instance mask kernels");
+}
+
+} // extern "C"

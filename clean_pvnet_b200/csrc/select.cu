@@ -17,6 +17,7 @@
 //
 // The evaluator's mask_iou (mask_iou_kernel, at the end) streams a predicted and a ground-truth mask with the same loads.
 #include <atomic>
+#include "api.h"
 #include "common.cuh"
 #include "kernels.h"
 
@@ -539,6 +540,8 @@ mask_iou_kernel(const TP *__restrict__ pred, long long psb, long long psy, long 
     }
 }
 
+namespace {
+
 template <typename TP, typename TG>
 void launch_mask_iou_typed(const void *pred, const long long *ps, const void *gt, const long long *gs, long long *inter,
                            long long *uni, int B, int H, int W, cudaStream_t st)
@@ -564,23 +567,49 @@ bool launch_mask_iou_gt(const void *pred, const long long *ps, const void *gt, i
     }
 }
 
-cudaError_t launch_mask_iou(const void *pred, int pred_dtype, const long long *ps, const void *gt, int gt_dtype,
-                            const long long *gs, long long *inter, long long *uni, int B, int H, int W, cudaStream_t st)
-{
-    if (B <= 0) return cudaSuccess;
-    cudaError_t e = cudaMemsetAsync(inter, 0, (size_t)B * sizeof(long long), st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(uni, 0, (size_t)B * sizeof(long long), st);
-    if (e != cudaSuccess || (long long)H * W == 0) return e;
-    bool ok = false;
-    switch (pred_dtype) {
-    case PVB_MASK_U8: ok = launch_mask_iou_gt<uint8_t>(pred, ps, gt, gt_dtype, gs, inter, uni, B, H, W, st); break;
-    case PVB_MASK_I8: ok = launch_mask_iou_gt<int8_t>(pred, ps, gt, gt_dtype, gs, inter, uni, B, H, W, st); break;
-    case PVB_MASK_I16: ok = launch_mask_iou_gt<int16_t>(pred, ps, gt, gt_dtype, gs, inter, uni, B, H, W, st); break;
-    case PVB_MASK_I32: ok = launch_mask_iou_gt<int32_t>(pred, ps, gt, gt_dtype, gs, inter, uni, B, H, W, st); break;
-    case PVB_MASK_I64: ok = launch_mask_iou_gt<long long>(pred, ps, gt, gt_dtype, gs, inter, uni, B, H, W, st); break;
-    default: break;
-    }
-    return ok ? cudaGetLastError() : cudaErrorInvalidValue;
-}
+} // namespace
 
 } // namespace pvb
+
+using namespace pvb;
+
+extern "C" {
+
+PVB_API int pvb_mask_iou(const void *pred, int32_t pred_dtype, const int64_t *pred_stride, const void *gt, int32_t gt_dtype,
+                         const int64_t *gt_stride, int64_t *inter, int64_t *uni, int32_t B, int32_t H, int32_t W,
+                         pvb_stream_t stream)
+{
+    if (B < 0 || H < 0 || W < 0) return fail(PVB_ERR_INVALID, "negative size (B=%d H=%d W=%d)", B, H, W);
+    for (int32_t dt : {pred_dtype, gt_dtype})
+        if (dt < PVB_MASK_U8 || dt > PVB_MASK_I64)
+            return fail(PVB_ERR_INVALID, "mask dtypes must be integer pvb_mask_dtypes (U8..I64), got %d and %d", pred_dtype,
+                        gt_dtype);
+    if (B == 0) return PVB_OK;
+    if (!pred_stride || !gt_stride) return fail(PVB_ERR_INVALID, "NULL stride array");
+    const long long HW = (long long)H * W;
+    if (!inter || !uni || (HW > 0 && (!pred || !gt))) return fail(PVB_ERR_INVALID, "NULL tensor");
+    if (HW > 0x7fffffffll) return fail(PVB_ERR_INVALID, "image too large (H*W >= 2^31)");
+    for (int i = 0; i < 3; ++i)
+        if (pred_stride[i] < 0 || gt_stride[i] < 0) return fail(PVB_ERR_INVALID, "negative stride");
+    const long long ps[3] = {pred_stride[0], pred_stride[1], pred_stride[2]};
+    const long long gs[3] = {gt_stride[0], gt_stride[1], gt_stride[2]};
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    long long *in = reinterpret_cast<long long *>(inter), *un = reinterpret_cast<long long *>(uni);
+    cudaError_t e = cudaMemsetAsync(in, 0, (size_t)B * sizeof(long long), st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(un, 0, (size_t)B * sizeof(long long), st);
+    if (e == cudaSuccess && HW > 0) {
+        bool ok = false;
+        switch (pred_dtype) {
+        case PVB_MASK_U8: ok = launch_mask_iou_gt<uint8_t>(pred, ps, gt, gt_dtype, gs, in, un, B, H, W, st); break;
+        case PVB_MASK_I8: ok = launch_mask_iou_gt<int8_t>(pred, ps, gt, gt_dtype, gs, in, un, B, H, W, st); break;
+        case PVB_MASK_I16: ok = launch_mask_iou_gt<int16_t>(pred, ps, gt, gt_dtype, gs, in, un, B, H, W, st); break;
+        case PVB_MASK_I32: ok = launch_mask_iou_gt<int32_t>(pred, ps, gt, gt_dtype, gs, in, un, B, H, W, st); break;
+        case PVB_MASK_I64: ok = launch_mask_iou_gt<long long>(pred, ps, gt, gt_dtype, gs, in, un, B, H, W, st); break;
+        default: break;
+        }
+        e = ok ? cudaGetLastError() : cudaErrorInvalidValue;
+    }
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "mask iou kernel");
+}
+
+} // extern "C"
