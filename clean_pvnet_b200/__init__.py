@@ -23,6 +23,8 @@ Public surface (same names/signatures as the reference):
     warp_affine_batch (cv2.warpAffine INTER_LINEAR for n rows), install_crop_as_reference (the cascade's crop)
     dcn.dcn_v2_conv / DCNv2 / DCN (twins of lib/networks/dcn_v2.py, the detector's deformable convolution, forward and
     backward), install_dcn_as_reference_module (call it before anything imports lib.networks.ct*)
+    dcn_pool.dcn_v2_pooling / DCNv2Pooling / DCNPooling (twins of the deformable PSROI pooling of the same module,
+    forward and backward; dcn_pool is what install_dcn_as_reference_module binds as lib.networks.dcn_v2)
     ct_loss.ct_focal_loss (the CenterNet trainer's heatmap focal loss and its gradient from the boxes), ct_target_batch
     (twin of the datasets' draw_umich_gaussian heatmap), ct_radius, CtNetworkWrapper (twin of lib/train/trainers/ct.py),
     install_ct_loss_as_reference
@@ -52,6 +54,8 @@ from . import crop  # noqa: F401
 from .crop import crop_inputs, uncrop_keypoints, warp_affine_batch, install_crop_as_reference  # noqa: F401
 from . import dcn  # noqa: F401
 from .dcn import dcn_v2_conv, DCNv2, DCN, install_dcn_as_reference_module  # noqa: F401
+from . import dcn_pool  # noqa: F401
+from .dcn_pool import dcn_v2_pooling, DCNv2Pooling, DCNPooling  # noqa: F401
 from .vote_loss import vote_loss, vote_target_batch, NetworkWrapper, install_vote_loss_as_reference  # noqa: F401
 from . import ct_loss  # noqa: F401
 from .ct_loss import (ct_focal_loss, ct_target_batch, ct_radius, CtNetworkWrapper,  # noqa: F401
@@ -80,6 +84,7 @@ __all__ = [
     "instance_masks_batch", "instance_masks_from_depth", "install_tless_renderer_as_reference",
     "crop", "crop_inputs", "uncrop_keypoints", "warp_affine_batch", "install_crop_as_reference",
     "dcn", "dcn_v2_conv", "DCNv2", "DCN", "install_dcn_as_reference_module",
+    "dcn_pool", "dcn_v2_pooling", "DCNv2Pooling", "DCNPooling",
     "ct_loss", "ct_focal_loss", "ct_target_batch", "ct_radius", "CtNetworkWrapper", "install_ct_loss_as_reference",
     "ct_decode", "decode_detections", "detection_boxes", "install_ct_decode_as_reference",
     "fps", "farthest_point_sampling", "farthest_point_sampling_batch", "install_fps_as_reference_module",

@@ -54,6 +54,13 @@ class PvbDcnDesc(ctypes.Structure):
                                              "pad_w", "dilation_h", "dilation_w", "deformable_groups")]
 
 
+class PvbDcnPoolDesc(ctypes.Structure):
+    """== struct pvb_dcn_pool_desc (include/pvnet_vote_b200.h)"""
+    _fields_ = [(n, ctypes.c_int32) for n in ("B", "C", "H", "W", "n_roi", "output_dim", "pooled_size", "part_size",
+                                             "sample_per_part", "group_size", "num_classes", "no_trans")] + [
+        ("spatial_scale", ctypes.c_float), ("trans_std", ctypes.c_float)]
+
+
 # every symbol include/pvnet_vote_b200.h declares: name -> (restype, argtypes)
 _vp, _i32, _sz, _f = ctypes.c_void_p, ctypes.c_int32, ctypes.c_size_t, ctypes.c_float
 _dp, _lp = ctypes.POINTER(PvbDesc), ctypes.POINTER(PvbLayout)
@@ -116,6 +123,8 @@ SIGNATURES = {
     "pvb_dcn_backward_workspace_bytes": (_sz, [ctypes.POINTER(PvbDcnDesc), _i32]),
     "pvb_dcn_backward": (ctypes.c_int, [ctypes.POINTER(PvbDcnDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                         _i32, _vp, _sz, _vp]),
+    "pvb_dcn_pool_forward": (ctypes.c_int, [ctypes.POINTER(PvbDcnPoolDesc), _vp, _vp, _vp, _vp, _vp, _vp]),
+    "pvb_dcn_pool_backward": (ctypes.c_int, [ctypes.POINTER(PvbDcnPoolDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "pvb_read_status": (ctypes.c_int, [_dp, _vp, _vp]),
     "pvb_host_scratch_bytes": (_sz, [_dp, _i32]),
     "pvb_ransac_voting_v3_host": (ctypes.c_int, [_dp, _vp, _vp, _vp, _i32, ctypes.c_uint32, _vp, _sz, _vp]),

@@ -5,7 +5,8 @@ CenterNet detector, lib/networks/ct/dla_dcn.py) on the device kernels of csrc/dc
                                       the autograd Function, same positional signature as the reference's
     DCNv2(in, out, kernel_size, stride, padding, dilation=1, deformable_groups=1)
     DCN(...)                          the same module, with its own conv_offset_mask (what dla_dcn.py builds)
-    install_dcn_as_reference_module() `from lib.networks.dcn_v2 import DCN` binds this module
+    install_dcn_as_reference_module() `from lib.networks.dcn_v2 import DCN` binds these names (and the pooling's, from
+                                      dcn_pool.py, the twin of the rest of lib/networks/dcn_v2.py)
 
 The reference's extension, lib/csrc/dcn_v2, is written against THC and does not build on current torch, so
 `import lib.networks.ct.dla_dcn` fails there; with install_dcn_as_reference_module() called first it imports and runs
@@ -194,15 +195,17 @@ class DCN(DCNv2):
 
 
 def install_dcn_as_reference_module():
-    """Makes `from lib.networks.dcn_v2 import DCN` (lib/networks/ct/dla_dcn.py:16) bind this module, so the detector
-    imports and runs without the THC extension `lib.csrc.dcn_v2._ext` ever being built or imported.  Only the leaf
-    `lib.networks.dcn_v2` is replaced; `lib` and `lib.networks` stay the real packages whenever they import.
+    """Makes `lib.networks.dcn_v2` (imported by lib/networks/ct/dla_dcn.py:16 and by lib/csrc/dcn_v2/test.py) bind this
+    package's twin of the whole module, clean_pvnet_b200.dcn_pool: the convolution (dcn_v2_conv, DCNv2, DCN) and the
+    deformable PSROI pooling (dcn_v2_pooling, DCNv2Pooling, DCNPooling).  The detector then imports and runs without
+    the THC extension `lib.csrc.dcn_v2._ext` ever being built or imported.  Only the leaf `lib.networks.dcn_v2` is
+    replaced; `lib` and `lib.networks` stay the real packages whenever they import.
 
     Call it BEFORE anything imports `lib.networks.ct*` (for the cascade: before install_crop_as_reference()).  Unlike
     the other drop-ins it cannot be installed afterwards: without it that import fails on the extension.  Idempotent."""
     from ._dropin import reference_package
-    this = sys.modules[__name__]
+    from . import dcn_pool
     parent = reference_package("lib.networks")
-    sys.modules["lib.networks.dcn_v2"] = this
-    parent.dcn_v2 = this
-    return this
+    sys.modules["lib.networks.dcn_v2"] = dcn_pool
+    parent.dcn_v2 = dcn_pool
+    return dcn_pool

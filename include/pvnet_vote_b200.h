@@ -627,6 +627,40 @@ PVB_API int pvb_dcn_backward(const pvb_dcn_desc *d, const float *input, const fl
                              float *grad_mask, float *grad_weight, float *grad_bias, int32_t chunk, void *workspace,
                              size_t workspace_bytes, pvb_stream_t stream);
 
+/* ---- DCNv2's deformable PSROI pooling (DESIGN.md section 8m) -------------------------------------------------------
+ * The other half of lib/csrc/dcn_v2 (dcn_v2_psroi_pooling_cuda.cu), behind DCNv2Pooling / DCNPooling.  Shapes: input
+ * [B,C,H,W], rois [n_roi,5] = (batch, x1, y1, x2, y2), trans [n_roi, 2*num_classes, part_size, part_size] ((x, y)
+ * offsets of class k at channels 2k and 2k + 1; unread with no_trans), out and count [n_roi, C, P, P], P = pooled_size;
+ * all device fp32, contiguous.  Output channel c belongs to class c / (C / num_classes).  Bin (ph, pw) of ROI n averages
+ * sample_per_part^2 bilinear samples, shifted by trans * trans_std * (ROI width, height) of part cell
+ * (floor(ph / P * part_size), floor(pw / P * part_size)); count is the number of samples inside the map.  The rounding
+ * is the reference kernel's as its sm_90a build runs it; DESIGN.md 8m tabulates it.
+ * Requirements: B, n_roi >= 0, C, H, W, pooled_size, part_size >= 1, output_dim == C, group_size == 1,
+ * 1 <= sample_per_part <= 32, num_classes >= 1 dividing C (num_classes is taken as 1 with no_trans),
+ * n_roi*C*P^2, B*C*H*W and n_roi*2*num_classes*part_size^2 < 2^31.  A tensor may be NULL only when it is empty or
+ * unread.  A bad descriptor or a NULL tensor returns PVB_ERR_INVALID before any CUDA call.
+ * Defined where the reference reads out of bounds: a ROI whose batch index (float -> int truncation, NaN -> 0) is
+ * outside [0, B) gives output 0, count 0 and no gradient; group_size != 1 and a class count that does not divide C are
+ * rejected.  No entry synchronises with the host or allocates; both can be captured in a CUDA graph. */
+typedef struct pvb_dcn_pool_desc {
+    int32_t B, C, H, W, n_roi, output_dim, pooled_size, part_size, sample_per_part, group_size, num_classes, no_trans;
+    float spatial_scale, trans_std;
+} pvb_dcn_pool_desc;
+
+/* Replaces dcn_v2_psroi_pooling_cuda_forward (dcn_v2_psroi_pooling_cuda.cu:272): out, and count unless it is NULL,
+ * bit-equal to the reference kernel's.  Each CTA computes the sample geometry of its ROI, class and bins once for all
+ * the class's channels.  n_roi == 0 is a no-op. */
+PVB_API int pvb_dcn_pool_forward(const pvb_dcn_pool_desc *d, const float *input, const float *rois, const float *trans,
+                                 float *out, float *count, pvb_stream_t stream);
+
+/* Replaces dcn_v2_psroi_pooling_cuda_backward (dcn_v2_psroi_pooling_cuda.cu:344) and needs no saved count: grad_input
+ * [B,C,H,W] is zeroed and then receives each valid sample's bilinear weights times grad_out / count through float
+ * atomics, as in the reference; grad_trans (shaped like trans; may be NULL with no_trans) is fully written, each part
+ * cell summed in a fixed order, so it is bit-identical run to run and per ROI.  rois get no gradient. */
+PVB_API int pvb_dcn_pool_backward(const pvb_dcn_pool_desc *d, const float *input, const float *rois,
+                                  const float *trans, const float *grad_out, float *grad_input, float *grad_trans,
+                                  pvb_stream_t stream);
+
 /* Reads the sticky status word of a workspace (synchronises `stream`). */
 PVB_API int pvb_read_status(const pvb_desc *d, const void *workspace, pvb_stream_t stream);
 
