@@ -16,6 +16,7 @@ PVB_IPC_HANDLE_BYTES = 64
 PVB_SELECT_BYTE, PVB_SELECT_EQ1 = 0, 1
 PVB_CROP_MASK_TO_BOX, PVB_CROP_CENTER_F64 = 1, 2
 (PVB_PNP_OK, PVB_PNP_ITERATION_LIMIT, PVB_PNP_TOO_FEW_POINTS, PVB_PNP_PLANAR, PVB_PNP_DEGENERATE) = range(5)
+PVB_DCN_F16, PVB_DCN_BF16 = 1, 2
 
 
 class PvbDesc(ctypes.Structure):
@@ -120,6 +121,7 @@ SIGNATURES = {
     "pvb_ct_decode": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int64), _vp, ctypes.POINTER(ctypes.c_int64), _i32, _i32,
                                      _i32, _i32, _i32, _i32, _vp, _vp, _vp, _sz, _vp]),
     "pvb_dcn_forward": (ctypes.c_int, [ctypes.POINTER(PvbDcnDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "pvb_dcn_forward_half": (ctypes.c_int, [ctypes.POINTER(PvbDcnDesc), _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "pvb_dcn_backward_workspace_bytes": (_sz, [ctypes.POINTER(PvbDcnDesc), _i32]),
     "pvb_dcn_backward": (ctypes.c_int, [ctypes.POINTER(PvbDcnDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                         _i32, _vp, _sz, _vp]),

@@ -9,11 +9,20 @@
 // split-K partials reduced in a fixed order, and a fixed-order grad_bias.  Everything but grad_input is bitwise
 // reproducible.  All arithmetic is FP32 FFMA (no TF32, no tensor cores).
 //
+// The half-precision forward (fp16 or bf16 operands, DESIGN.md section 8n) is a second implicit-GEMM kernel on the
+// tensor cores: the same sampler, fed the up-cast inputs, fills bf16 / fp16 B tiles in shared memory; the weight
+// tiles arrive by cp.async; mma.sync m16n8k16 accumulates in fp32.  It has no backward of its own: the Python layer
+// runs the fp32 backward on up-cast copies of the operands the forward used.
+//
 // A sample point of (pixel, tap, deformable group) has four corner offsets and four bilinear weights that do not depend
 // on the channel: they are computed once per tile and reused over the group's channels.  The sampled value is the
 // reference kernel's bit for bit: nvcc contracts its `w1*v1 + w2*v2 + w3*v3 + w4*v4` (dcn_v2_im2col_cuda.cu:52) into
 // fma(w4,v4, fma(w3,v3, fma(w1,v1, w2*v2))) at sm_90a (read off the reference build's SASS), written out below with
 // explicit intrinsics; the mask multiplies after the bilinear sum.
+#include <cooperative_groups.h>
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
 #include "api.h"
 
 namespace pvb {
@@ -59,23 +68,31 @@ __device__ __forceinline__ Corners sample_point(float h, float w, int H, int W)
     return s;
 }
 
-__device__ __forceinline__ float bilinear(const float *plane, const int off[4], const float wt[4])
+// one element read as fp32: fp16 and bf16 up-cast exactly, so the sampler sees the value the fp32 path would
+__device__ __forceinline__ float ld_f32(const float *p) { return __ldg(p); }
+__device__ __forceinline__ float ld_f32(const __half *p) { return __half2float(__ldg(p)); }
+__device__ __forceinline__ float ld_f32(const __nv_bfloat16 *p) { return __bfloat162float(__ldg(p)); }
+
+template <typename T>
+__device__ __forceinline__ float bilinear(const T *plane, const int off[4], const float wt[4])
 {
-    const float v1 = off[0] >= 0 ? __ldg(plane + off[0]) : 0.f;
-    const float v2 = off[1] >= 0 ? __ldg(plane + off[1]) : 0.f;
-    const float v3 = off[2] >= 0 ? __ldg(plane + off[2]) : 0.f;
-    const float v4 = off[3] >= 0 ? __ldg(plane + off[3]) : 0.f;
+    const float v1 = off[0] >= 0 ? ld_f32(plane + off[0]) : 0.f;
+    const float v2 = off[1] >= 0 ? ld_f32(plane + off[1]) : 0.f;
+    const float v3 = off[2] >= 0 ? ld_f32(plane + off[2]) : 0.f;
+    const float v4 = off[3] >= 0 ? ld_f32(plane + off[3]) : 0.f;
     return __fmaf_rn(wt[3], v4, __fmaf_rn(wt[2], v3, __fmaf_rn(wt[0], v1, __fmul_rn(wt[1], v2))));
 }
 
 // the sample coordinate of output pixel p at tap (i, j): float(ho*s - p + i*d) + offset, rounded once
-__device__ __forceinline__ void sample_coord(const DcnArgs &a, long long ob, int tap, int p, float &h, float &w)
+template <typename T>
+__device__ __forceinline__ void sample_coord(const DcnArgs &a, const T *offset, long long ob, int tap, int p, float &h,
+                                             float &w)
 {
     const int ho = p / a.Wo, wo = p - (p / a.Wo) * a.Wo;
     const int i = tap / a.kw, j = tap - (tap / a.kw) * a.kw;
     const long long P = (long long)a.Ho * a.Wo;
-    const float dy = __ldg(a.offset + ob + (2ll * tap) * P + p);
-    const float dx = __ldg(a.offset + ob + (2ll * tap + 1) * P + p);
+    const float dy = ld_f32(offset + ob + (2ll * tap) * P + p);
+    const float dx = ld_f32(offset + ob + (2ll * tap + 1) * P + p);
     h = __fadd_rn((float)(ho * a.sh - a.ph + i * a.dh), dy);
     w = __fadd_rn((float)(wo * a.sw - a.pw + j * a.dw), dx);
 }
@@ -146,7 +163,7 @@ __global__ void __launch_bounds__(NT) dcn_forward_kernel(DcnArgs a)
                 const int p = p0 + tid;
                 if (p < P) {
                     float h, w;
-                    sample_coord(a, ob, tap, p, h, w);
+                    sample_coord(a, a.offset, ob, tap, p, h, w);
                     store_sample(st, tid, sample_point(h, w, a.H, a.W), __ldg(a.mask + mb + (long long)tap * P + p));
                 } else {
                     Corners z;
@@ -236,7 +253,7 @@ __global__ void __launch_bounds__(256) dcn_grad_coord_kernel(DcnArgs a, int b0)
     const long long HW = (long long)a.H * a.W, K = (long long)a.C * T;
     const long long ob = ((long long)b * a.dg + g) * 2 * T * P, mb = ((long long)b * a.dg + g) * T * P;
     float h, w;
-    sample_coord(a, ob, tap, p, h, w);
+    sample_coord(a, a.offset, ob, tap, p, h, w);
     const float m = __ldg(a.mask + mb + (long long)tap * P + p);
     float gy = 0.f, gx = 0.f, gm = 0.f;
     // a point with h <= -1, w <= -1, h >= H or w >= W contributes nothing (the reference's predicate: NaN passes it)
@@ -279,7 +296,7 @@ __global__ void __launch_bounds__(256) dcn_grad_input_kernel(DcnArgs a, int b0)
     const long long HW = (long long)a.H * a.W, K = (long long)a.C * T;
     const long long ob = ((long long)b * a.dg + g) * 2 * T * P, mb = ((long long)b * a.dg + g) * T * P;
     float h, w;
-    sample_coord(a, ob, tap, p, h, w);
+    sample_coord(a, a.offset, ob, tap, p, h, w);
     if (!(h > -1.f && w > -1.f && h < (float)a.H && w < (float)a.W)) return;
     const float m = __ldg(a.mask + mb + (long long)tap * P + p);
     const int hl = (int)floorf(h), wl = (int)floorf(w);
@@ -328,7 +345,7 @@ __global__ void __launch_bounds__(NT) dcn_grad_weight_kernel(DcnArgs a, long lon
             if (q < q1) {
                 b = (int)(q / P); p = (int)(q - (long long)b * P);
                 float h, w;
-                sample_coord(a, ((long long)b * a.dg + g) * 2 * T * P, tap, p, h, w);
+                sample_coord(a, a.offset, ((long long)b * a.dg + g) * 2 * T * P, tap, p, h, w);
                 s = sample_point(h, w, a.H, a.W);
                 m = __ldg(a.mask + ((long long)b * a.dg + g) * T * P + (long long)tap * P + p);
             } else {
@@ -400,6 +417,199 @@ __global__ void __launch_bounds__(256) dcn_grad_bias_kernel(DcnArgs a)
     }
 }
 
+// ---- the half-precision forward: fp16 / bf16 operands on the tensor cores ----------------------------------------
+// CTA tile HBM output channels x HBN pixels, K in chunks of HBK channels of one (group, tap); 8 warps as 4 (rows) x 2
+// (pixels) of 32 x 32, each an array of 2 x 4 m16n8k16 MMAs.  Tiles are stored [row][k] with a pitch of HKP halves, so
+// the eight 16-byte rows an ldmatrix phase reads fall in distinct banks.
+constexpr int HBM = 128, HBN = 64, HBK = 32, HKP = HBK + 8;
+// split-K: a layer whose tiles would not fill two CTAs per H100 SM splits its K chunks over a cluster of up to
+// H_MAX_SPLIT CTAs (each keeping at least H_MIN_CHUNKS chunks), which add their partials through distributed shared
+// memory in rank order.  Chosen from the per-image shape only, so an image's output does not depend on the batch.
+constexpr int H_TARGET_CTAS = 264, H_MAX_SPLIT = 8, H_MIN_CHUNKS = 4;
+
+template <typename T> struct DcnHalfPtrs {
+    const T *input, *offset, *mask;
+    const T *weight;          // tap-major [Co][kh][kw][C]: a (tap, channel chunk) row is contiguous
+    const T *bias;
+    T *out;
+};
+
+template <typename T> struct HalfSmem {
+    union {
+        struct { T A[2][HBM][HKP]; T B[2][HBN][HKP]; } t;   // double-buffered weight and column tiles
+        float red[HBM][HBN + 4];                           // the fp32 accumulator tile, after the K loop
+    };
+};
+
+__device__ __forceinline__ uint32_t pack2(__half, float x, float y)
+{
+    const __half2 h = __floats2half2_rn(x, y);
+    return *reinterpret_cast<const uint32_t *>(&h);
+}
+__device__ __forceinline__ uint32_t pack2(__nv_bfloat16, float x, float y)
+{
+    const __nv_bfloat162 h = __floats2bfloat162_rn(x, y);
+    return *reinterpret_cast<const uint32_t *>(&h);
+}
+// round to nearest even; beyond the format's range the result is +-inf, never the largest finite value
+__device__ __forceinline__ __half to_lp(__half, float x) { return __float2half_rn(x); }
+__device__ __forceinline__ __nv_bfloat16 to_lp(__nv_bfloat16, float x) { return __float2bfloat16_rn(x); }
+
+__device__ __forceinline__ void cp_async16(void *dst, const void *src, bool valid)   // zero-fills when !valid
+{
+    const unsigned s = (unsigned)__cvta_generic_to_shared(dst);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(src), "r"(valid ? 16 : 0));
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
+
+__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], const void *p)
+{
+    const unsigned s = (unsigned)__cvta_generic_to_shared(p);
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(s));
+}
+
+__device__ __forceinline__ void mma16816(__half, float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1)
+{
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
+                 "{%0,%1,%2,%3};\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void mma16816(__nv_bfloat16, float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1)
+{
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
+                 "{%0,%1,%2,%3};\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+// out[b][o][p] = RN_T(bias[o] + sum over (g, tap, c in group g) of W[o][c*T + tap] * RN_T(cols[b][c*T + tap][p])),
+// the sum in fp32 on the tensor cores.  grid (ceil(P / HBN) * S, ceil(Co / HBM), B), clusters of (S, 1, 1) when S > 1;
+// CTA rank r of a cluster runs K chunks [r*n/S, (r+1)*n/S) of the n = dg * T * ceil(Cg / HBK).
+template <typename T>
+__global__ void __launch_bounds__(NT, 2) dcn_forward_half_kernel(DcnArgs a, DcnHalfPtrs<T> t, int S)
+{
+    __shared__ __align__(16) HalfSmem<T> sm;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wm = warp >> 1, wn = warp & 1;
+    const int split = blockIdx.x % S, P = a.Ho * a.Wo, p0 = (int)(blockIdx.x / S) * HBN, o0 = blockIdx.y * HBM;
+    const int b = blockIdx.z, T_ = a.kh * a.kw, Cg = a.C / a.dg, nct = (Cg + HBK - 1) / HBK, nchunk = a.dg * T_ * nct;
+    const int kb = (int)((long long)split * nchunk / S), ke = (int)((long long)(split + 1) * nchunk / S);
+    const long long HW = (long long)a.H * a.W, K = (long long)a.C * T_;
+    // every 8-channel run of a weight row is 16-byte aligned, so the weight tile arrives by 16-byte cp.async
+    const bool vec = ((a.C | Cg) & 7) == 0 && (reinterpret_cast<uintptr_t>(t.weight) & 15) == 0;
+    const bool live = o0 + wm * 32 < a.Co;       // this warp's rows hold at least one output channel
+    // the sampler's share of a B tile: pixel sn, channels sk .. sk + 7 of the chunk
+    const int sn = tid % HBN, sk = (tid / HBN) * 8, sp = p0 + sn;
+
+    float acc[2][4][4];
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+            const int o = o0 + wm * 32 + mt * 16 + hf * 8 + lane / 4;
+            const float bv = (split == 0 && o < a.Co) ? ld_f32(t.bias + o) : 0.f;
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt) acc[mt][nt][2 * hf] = acc[mt][nt][2 * hf + 1] = bv;
+        }
+
+    // the sample point of pixel sp at the current tap: computed once per tap, reused over the group's channels
+    Corners s = {};
+    float m = 0.f;
+
+    auto stage = [&](int it, int buf) {
+        const int g = it / (T_ * nct), tap = (it / nct) % T_, c0 = (it % nct) * HBK;
+        if (c0 == 0 || it == kb) {
+            if (sp < P) {
+                float h, w;
+                sample_coord(a, t.offset, ((long long)b * a.dg + g) * 2 * T_ * P, tap, sp, h, w);
+                s = sample_point(h, w, a.H, a.W);
+                m = ld_f32(t.mask + ((long long)b * a.dg + g) * T_ * P + (long long)tap * P + sp);
+            }
+        }
+#pragma unroll
+        for (int r = 0; r < HBM * HBK / 8 / NT; ++r) {     // the weight tile, 8 channels per copy
+            const int e = tid + r * NT, row = e / (HBK / 8), v = (e % (HBK / 8)) * 8;
+            const int o = o0 + row, c = c0 + v;
+            T *dst = &sm.t.A[buf][row][v];
+            const T *src = t.weight + (long long)o * K + (long long)tap * a.C + (long long)g * Cg + c;
+            if (vec) {
+                const bool ok = o < a.Co && c < Cg;
+                cp_async16(dst, ok ? src : t.weight, ok);
+            } else {
+#pragma unroll
+                for (int q = 0; q < 8; ++q) dst[q] = (o < a.Co && c + q < Cg) ? src[q] : to_lp(T{}, 0.f);
+            }
+        }
+        cp_async_commit();
+        float v[8];
+        const T *plane = t.input + ((long long)b * a.C + (long long)g * Cg + c0 + sk) * HW;
+#pragma unroll
+        for (int q = 0; q < 8; ++q)
+            v[q] = (sp < P && c0 + sk + q < Cg) ? __fmul_rn(m, bilinear(plane + q * HW, s.off, s.wt)) : 0.f;
+        uint4 pk;
+        pk.x = pack2(T{}, v[0], v[1]); pk.y = pack2(T{}, v[2], v[3]);
+        pk.z = pack2(T{}, v[4], v[5]); pk.w = pack2(T{}, v[6], v[7]);
+        *reinterpret_cast<uint4 *>(&sm.t.B[buf][sn][sk]) = pk;
+    };
+
+    stage(kb, 0);
+    cp_async_wait_all();
+    __syncthreads();
+    for (int it = kb; it < ke; ++it) {
+        const int buf = (it - kb) & 1;
+        if (it + 1 < ke) stage(it + 1, buf ^ 1);           // the next chunk's tiles load while this one multiplies
+        if (live) {
+#pragma unroll
+            for (int ks = 0; ks < HBK; ks += 16) {
+                uint32_t af[2][4], bf[2][4];
+#pragma unroll
+                for (int mt = 0; mt < 2; ++mt)
+                    ldmatrix_x4(af[mt], &sm.t.A[buf][wm * 32 + mt * 16 + (lane & 15)][ks + (lane >> 4) * 8]);
+#pragma unroll
+                for (int np = 0; np < 2; ++np)
+                    ldmatrix_x4(bf[np], &sm.t.B[buf][wn * 32 + np * 16 + (lane & 7) + (lane >> 4) * 8]
+                                                    [ks + ((lane >> 3) & 1) * 8]);
+#pragma unroll
+                for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+                    for (int nt = 0; nt < 4; ++nt)
+                        mma16816(T{}, acc[mt][nt], af[mt], bf[nt >> 1][(nt & 1) * 2], bf[nt >> 1][(nt & 1) * 2 + 1]);
+            }
+        }
+        cp_async_wait_all();
+        __syncthreads();
+    }
+
+    // the loop ended on a barrier: the tiles are consumed and the accumulator tile may take their place
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+            for (int hf = 0; hf < 2; ++hf) {
+                const int row = wm * 32 + mt * 16 + hf * 8 + lane / 4, col = wn * 32 + nt * 8 + (lane % 4) * 2;
+                sm.red[row][col] = acc[mt][nt][2 * hf];
+                sm.red[row][col + 1] = acc[mt][nt][2 * hf + 1];
+            }
+    namespace cg = cooperative_groups;
+    if (S > 1) cg::this_cluster().sync(); else __syncthreads();
+    // rank `split` stores rows [split*HBM/S, (split+1)*HBM/S) of the tile, adding the ranks' partials in rank order
+    const int r0 = split * HBM / S, r1 = (split + 1) * HBM / S;
+    for (int e = r0 * HBN + tid; e < r1 * HBN; e += NT) {
+        const int row = e / HBN, col = e % HBN, o = o0 + row, p = p0 + col;
+        if (o >= a.Co || p >= P) continue;
+        float v = sm.red[row][col];
+        if (S > 1) {
+            v = cg::this_cluster().map_shared_rank(&sm.red[row][col], 0)[0];
+            for (int q = 1; q < S; ++q) v = __fadd_rn(v, cg::this_cluster().map_shared_rank(&sm.red[row][col], q)[0]);
+        }
+        t.out[((long long)b * a.Co + o) * P + p] = to_lp(T{}, v);
+    }
+    if (S > 1) cg::this_cluster().sync();                  // no CTA leaves while another reads its partials
+}
+
 } // namespace
 
 // backward plan: images per grad_cols chunk, and grad_weight's split of the (image, pixel) reduction into `splits`
@@ -462,6 +672,43 @@ int dcn_args(const pvb_dcn_desc *d, DcnArgs &a)
     return PVB_OK;
 }
 
+// the split-K factor of the half-precision forward: a function of the per-image shape only
+int dcn_half_splits(const DcnArgs &a)
+{
+    const int T = a.kh * a.kw, Cg = a.C / a.dg;
+    const long long nchunk = (long long)a.dg * T * ((Cg + HBK - 1) / HBK);
+    const long long tiles = ((long long)a.Ho * a.Wo + HBN - 1) / HBN * ((a.Co + HBM - 1) / HBM);
+    long long S = (H_TARGET_CTAS + tiles - 1) / tiles;
+    if (S > H_MAX_SPLIT) S = H_MAX_SPLIT;
+    if (S > nchunk / H_MIN_CHUNKS) S = nchunk / H_MIN_CHUNKS;
+    return S < 1 ? 1 : (int)S;
+}
+
+template <typename T>
+int launch_dcn_forward_half(const DcnArgs &a, const DcnHalfPtrs<T> &t, cudaStream_t stream)
+{
+    const int S = dcn_half_splits(a);
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)(((long long)a.Ho * a.Wo + HBN - 1) / HBN * S), (a.Co + HBM - 1) / HBM, a.B);
+    cfg.blockDim = dim3(NT);
+    cfg.stream = stream;
+    cudaLaunchAttribute cluster;
+    cluster.id = cudaLaunchAttributeClusterDimension;
+    cluster.val.clusterDim.x = S; cluster.val.clusterDim.y = 1; cluster.val.clusterDim.z = 1;
+    cfg.attrs = &cluster;
+    cfg.numAttrs = S > 1 ? 1 : 0;
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, dcn_forward_half_kernel<T>, a, t, S);
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "dcn half forward kernel");
+}
+
+template <typename T>
+DcnHalfPtrs<T> half_ptrs(const void *input, const void *offset, const void *mask, const void *weight, const void *bias,
+                         void *output)
+{
+    return DcnHalfPtrs<T>{static_cast<const T *>(input), static_cast<const T *>(offset), static_cast<const T *>(mask),
+                          static_cast<const T *>(weight), static_cast<const T *>(bias), static_cast<T *>(output)};
+}
+
 } // namespace
 
 } // namespace pvb
@@ -482,6 +729,23 @@ PVB_API int pvb_dcn_forward(const pvb_dcn_desc *d, const float *input, const flo
     dcn_forward_kernel<<<grid, NT, 0, static_cast<cudaStream_t>(stream)>>>(a);
     cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? PVB_OK : cuda_fail(e, "dcn forward kernel");
+}
+
+PVB_API int pvb_dcn_forward_half(const pvb_dcn_desc *d, int32_t dtype, const void *input, const void *offset,
+                                 const void *mask, const void *weight, const void *bias, void *output,
+                                 pvb_stream_t stream)
+{
+    if (dtype != PVB_DCN_F16 && dtype != PVB_DCN_BF16)
+        return fail(PVB_ERR_INVALID, "dtype=%d must be PVB_DCN_F16 (%d) or PVB_DCN_BF16 (%d)", dtype, PVB_DCN_F16,
+                    PVB_DCN_BF16);
+    DcnArgs a;
+    if (int rc = dcn_args(d, a)) return rc;
+    if (a.B == 0) return PVB_OK;
+    if (!input || !offset || !mask || !weight || !bias || !output) return fail(PVB_ERR_INVALID, "NULL tensor");
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return dtype == PVB_DCN_F16
+               ? launch_dcn_forward_half(a, half_ptrs<__half>(input, offset, mask, weight, bias, output), st)
+               : launch_dcn_forward_half(a, half_ptrs<__nv_bfloat16>(input, offset, mask, weight, bias, output), st);
 }
 
 PVB_API size_t pvb_dcn_backward_workspace_bytes(const pvb_dcn_desc *d, int32_t chunk)

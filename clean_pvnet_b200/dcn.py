@@ -10,8 +10,14 @@ CenterNet detector, lib/networks/ct/dla_dcn.py) on the device kernels of csrc/dc
 
 The reference's extension, lib/csrc/dcn_v2, is written against THC and does not build on current torch, so
 `import lib.networks.ct.dla_dcn` fails there; with install_dcn_as_reference_module() called first it imports and runs
-on these kernels, and net_utils.load_network loads a trained detector unchanged (same parameter names).  fp32 CUDA
+on these kernels, and net_utils.load_network loads a trained detector unchanged (same parameter names).  CUDA
 tensors only; there is no CPU implementation behind them.
+
+The compute dtype is the input's.  An fp32 input needs every tensor fp32 and runs the FP32-FFMA kernels.  An fp16 or
+bf16 input (what the DLA-34's convolutions emit under torch.autocast, or a .half() / .bfloat16() model) casts offset,
+mask, weight and bias to its dtype, round to nearest, and runs the tensor-core forward (DESIGN.md section 8n); the
+backward is the fp32 one on exact up-casts of those operands, and each gradient comes back in its tensor's dtype, so an
+fp32 parameter gets an fp32 gradient.  The dispatch does not look at the autocast state.
 """
 import ctypes
 import math
@@ -28,6 +34,9 @@ from . import _lib
 # grad_cols, the backward's only stored column matrix ([chunk, C*kh*kw, Ho*Wo] fp32), is planned in image chunks of at
 # most this many bytes (one image always fits); the other outputs do not depend on the chunking.
 MAX_COLUMN_BYTES = 1 << 28
+
+# the half-precision compute dtypes and their code in pvb_dcn_forward_half
+HALF = {torch.float16: _lib.PVB_DCN_F16, torch.bfloat16: _lib.PVB_DCN_BF16}
 
 
 def _desc(input, weight, stride, padding, dilation, deformable_groups):
@@ -47,13 +56,32 @@ def _out_hw(d):
     return ho, wo
 
 
+def _operands(input, offset, mask, weight, bias):
+    """(offset, mask, weight, bias) in the compute dtype: cast to an fp16 / bf16 input's dtype (round to nearest) from
+    fp32, fp16 or bf16; left as they are for any other input, which _check then holds to fp32."""
+    if not isinstance(input, torch.Tensor) or input.dtype not in HALF:
+        return offset, mask, weight, bias
+    ts = dict(offset=offset, mask=mask, weight=weight, bias=bias)
+    for name, t in ts.items():
+        if isinstance(t, torch.Tensor) and t.dtype not in (torch.float32, torch.float16, torch.bfloat16):
+            raise RuntimeError(f"dcn_v2_conv: {name} must be float32, float16 or bfloat16 with a {input.dtype} input, "
+                               f"got {t.dtype}")
+    return tuple(t.to(input.dtype) if isinstance(t, torch.Tensor) else t for t in ts.values())
+
+
 def _check(input, offset, mask, weight, bias, d):
     ts = dict(input=input, offset=offset, mask=mask, weight=weight, bias=bias)
     for name, t in ts.items():
-        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+        if not isinstance(t, torch.Tensor):
             raise RuntimeError(f"dcn_v2_conv: {name} must be a CUDA tensor")
-        if t.dtype != torch.float32:
-            raise RuntimeError(f"dcn_v2_conv: {name} must be float32, got {t.dtype} (the kernels are fp32 only)")
+    want = input.dtype if input.dtype in HALF else torch.float32
+    for name, t in ts.items():
+        if t.dtype != want:
+            raise RuntimeError(f"dcn_v2_conv: {name} must be {want}, got {t.dtype} (the kernels take float32 throughout, "
+                               f"or a float16 / bfloat16 input with the other tensors cast to its dtype)")
+    for name, t in ts.items():
+        if not t.is_cuda:
+            raise RuntimeError(f"dcn_v2_conv: {name} must be a CUDA tensor")
         if t.device != input.device:
             raise RuntimeError(f"dcn_v2_conv: {name} is on {t.device}, input on {input.device}")
     if input.dim() != 4 or weight.dim() != 4 or weight.shape[1] != input.shape[1]:
@@ -74,14 +102,20 @@ def _call(entry, dev, *args):
 
 
 def dcn_forward(input, offset, mask, weight, bias, stride, padding, dilation, deformable_groups):
-    """The forward of dcn_v2_conv without autograd: output [B,C_out,Ho,Wo] on input's device; no host sync."""
+    """The forward of dcn_v2_conv without autograd: output [B,C_out,Ho,Wo] in the compute dtype on input's device; no
+    host sync."""
+    offset, mask, weight, bias = _operands(input, offset, mask, weight, bias)
     d = _desc(input, weight, stride, padding, dilation, deformable_groups)
     _check(input, offset, mask, weight, bias, d)
     ho, wo = _out_hw(d)
-    out = torch.empty((d.B, d.C_out, ho, wo), dtype=torch.float32, device=input.device)
-    if d.B:
+    out = torch.empty((d.B, d.C_out, ho, wo), dtype=input.dtype, device=input.device)
+    if d.B and input.dtype == torch.float32:
         c = [t.contiguous() for t in (input, offset, mask, weight, bias)]
         _call("pvb_dcn_forward", input.device, ctypes.byref(d), *c, out)
+    elif d.B:
+        x, off, m, b = (t.contiguous() for t in (input, offset, mask, bias))
+        w = weight.permute(0, 2, 3, 1).contiguous()          # tap-major [C_out, kh, kw, C], as the kernel reads it
+        _call("pvb_dcn_forward_half", input.device, ctypes.byref(d), HALF[input.dtype], x, off, m, w, b, out)
     return out
 
 
@@ -119,19 +153,23 @@ class _DCNv2(Function):
         ctx.dilation = _pair(dilation)
         ctx.kernel_size = _pair(weight.shape[2:4])
         ctx.deformable_groups = deformable_groups
-        output = dcn_forward(input, offset, mask, weight, bias, ctx.stride, ctx.padding, ctx.dilation,
-                             deformable_groups)
-        ctx.save_for_backward(input, offset, mask, weight, bias)
+        ops = _operands(input, offset, mask, weight, bias)
+        output = dcn_forward(input, *ops, ctx.stride, ctx.padding, ctx.dilation, deformable_groups)
+        ctx.dtypes = tuple(t.dtype for t in (input, offset, mask, weight, bias))
+        ctx.save_for_backward(input, *ops)
         return output
 
     @staticmethod
     @once_differentiable
     def backward(ctx, grad_output):
         input, offset, mask, weight, bias = ctx.saved_tensors
-        grad_input, grad_offset, grad_mask, grad_weight, grad_bias = dcn_backward(
-            input, offset, mask, weight, bias, grad_output.contiguous(), ctx.stride, ctx.padding, ctx.dilation,
-            ctx.deformable_groups)
-        return grad_input, grad_offset, grad_mask, grad_weight, grad_bias, None, None, None, None
+        grad_output = grad_output.contiguous()
+        if input.dtype != torch.float32:     # the fp32 backward on the operands the forward used, up-cast exactly
+            input, offset, mask, weight, bias, grad_output = (
+                t.float() for t in (input, offset, mask, weight, bias, grad_output))
+        grads = dcn_backward(input, offset, mask, weight, bias, grad_output, ctx.stride, ctx.padding, ctx.dilation,
+                             ctx.deformable_groups)
+        return tuple(g.to(dt) for g, dt in zip(grads, ctx.dtypes)) + (None, None, None, None)
 
 
 dcn_v2_conv = _DCNv2.apply

@@ -613,6 +613,20 @@ typedef struct pvb_dcn_desc {
 PVB_API int pvb_dcn_forward(const pvb_dcn_desc *d, const float *input, const float *offset, const float *mask,
                             const float *weight, const float *bias, float *output, pvb_stream_t stream);
 
+/* The same forward in half precision (DESIGN.md section 8n), for torch.autocast and half models: every tensor is
+ * `dtype` (PVB_DCN_F16 = IEEE fp16, PVB_DCN_BF16 = bfloat16), shaped as above except that the weight is tap-major,
+ * [C_out][kh][kw][C] (weight.permute(0, 2, 3, 1)), so that a (tap, channel chunk) tile of it is contiguous.  Each
+ * column entry is the fp32 forward's, computed from the up-cast inputs and rounded once to `dtype`; output =
+ * RN_dtype(bias + weight . cols) with the sum in fp32 on the tensor cores, +-inf where it overflows.  Same descriptor
+ * checks, limits and guarantees as pvb_dcn_forward (bit-identical run to run, an image independent of the batch, no
+ * host synchronisation, no allocation); an unknown dtype returns PVB_ERR_INVALID before any CUDA call.  There is no
+ * half-precision backward: run pvb_dcn_backward on fp32 copies of the operands this call used. */
+#define PVB_DCN_F16  1
+#define PVB_DCN_BF16 2
+PVB_API int pvb_dcn_forward_half(const pvb_dcn_desc *d, int32_t dtype, const void *input, const void *offset,
+                                 const void *mask, const void *weight, const void *bias, void *output,
+                                 pvb_stream_t stream);
+
 /* Replaces dcn_v2_cuda_backward (dcn_v2_cuda.cu:206) for the whole batch: grad_cols = weight^T . grad_output goes to the
  * workspace `chunk` images at a time (the only column matrix stored); grad_offset / grad_mask (the reference's
  * col2im_coord: grad_mask = sum grad_col * value, grad_offset = sum d(value)/d(h, w) * grad_col * mask, 0 for a point
