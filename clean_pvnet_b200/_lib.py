@@ -122,6 +122,7 @@ SIGNATURES = {
                                      _i32, _i32, _i32, _i32, _vp, _vp, _vp, _sz, _vp]),
     "pvb_dcn_forward": (ctypes.c_int, [ctypes.POINTER(PvbDcnDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "pvb_dcn_forward_half": (ctypes.c_int, [ctypes.POINTER(PvbDcnDesc), _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "pvb_dcn_forward_half_nhwc": (ctypes.c_int, [ctypes.POINTER(PvbDcnDesc), _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "pvb_dcn_backward_workspace_bytes": (_sz, [ctypes.POINTER(PvbDcnDesc), _i32]),
     "pvb_dcn_backward": (ctypes.c_int, [ctypes.POINTER(PvbDcnDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                         _i32, _vp, _sz, _vp]),

@@ -11,8 +11,9 @@
 //
 // The half-precision forward (fp16 or bf16 operands, DESIGN.md section 8n) is a second implicit-GEMM kernel on the
 // tensor cores: the same sampler, fed the up-cast inputs, fills bf16 / fp16 B tiles in shared memory; the weight
-// tiles arrive by cp.async; mma.sync m16n8k16 accumulates in fp32.  It has no backward of its own: the Python layer
-// runs the fp32 backward on up-cast copies of the operands the forward used.
+// tiles arrive by cp.async; mma.sync m16n8k16 accumulates in fp32.  Its NHWC (channels_last) twin (section 8o) shares
+// that body and differs only in where it reads and writes, so its output is the NCHW kernel's bit for bit.  Neither
+// has a backward of its own: the Python layer runs the fp32 backward on up-cast copies of the operands the forward used.
 //
 // A sample point of (pixel, tap, deformable group) has four corner offsets and four bilinear weights that do not depend
 // on the channel: they are computed once per tile and reused over the group's channels.  The sampled value is the
@@ -73,6 +74,12 @@ __device__ __forceinline__ float ld_f32(const float *p) { return __ldg(p); }
 __device__ __forceinline__ float ld_f32(const __half *p) { return __half2float(__ldg(p)); }
 __device__ __forceinline__ float ld_f32(const __nv_bfloat16 *p) { return __bfloat162float(__ldg(p)); }
 
+// the bilinear sum of the four corner values v1..v4 (0 for a corner outside the image), in the reference's order
+__device__ __forceinline__ float blend(const float wt[4], float v1, float v2, float v3, float v4)
+{
+    return __fmaf_rn(wt[3], v4, __fmaf_rn(wt[2], v3, __fmaf_rn(wt[0], v1, __fmul_rn(wt[1], v2))));
+}
+
 template <typename T>
 __device__ __forceinline__ float bilinear(const T *plane, const int off[4], const float wt[4])
 {
@@ -80,7 +87,7 @@ __device__ __forceinline__ float bilinear(const T *plane, const int off[4], cons
     const float v2 = off[1] >= 0 ? ld_f32(plane + off[1]) : 0.f;
     const float v3 = off[2] >= 0 ? ld_f32(plane + off[2]) : 0.f;
     const float v4 = off[3] >= 0 ? ld_f32(plane + off[3]) : 0.f;
-    return __fmaf_rn(wt[3], v4, __fmaf_rn(wt[2], v3, __fmaf_rn(wt[0], v1, __fmul_rn(wt[1], v2))));
+    return blend(wt, v1, v2, v3, v4);
 }
 
 // the sample coordinate of output pixel p at tap (i, j): float(ho*s - p + i*d) + offset, rounded once
@@ -95,6 +102,17 @@ __device__ __forceinline__ void sample_coord(const DcnArgs &a, const T *offset, 
     const float dx = ld_f32(offset + ob + (2ll * tap + 1) * P + p);
     h = __fadd_rn((float)(ho * a.sh - a.ph + i * a.dh), dy);
     w = __fadd_rn((float)(wo * a.sw - a.pw + j * a.dw), dx);
+}
+
+// the same on an NHWC offset [B][Ho][Wo][dg*2*kh*kw]: op points at the pixel's (dy, dx) of the tap.  Kept apart from
+// sample_coord, whose sharing it would reschedule the fp32 kernels.
+template <typename T>
+__device__ __forceinline__ void sample_coord_nhwc(const DcnArgs &a, const T *op, int tap, int p, float &h, float &w)
+{
+    const int ho = p / a.Wo, wo = p - (p / a.Wo) * a.Wo;
+    const int i = tap / a.kw, j = tap - (tap / a.kw) * a.kw;
+    h = __fadd_rn((float)(ho * a.sh - a.ph + i * a.dh), ld_f32(op));
+    w = __fadd_rn((float)(wo * a.sw - a.pw + j * a.dw), ld_f32(op + 1));
 }
 
 // shared-memory sample table of one tile: corners, weights and mask of up to BN sample points
@@ -427,6 +445,7 @@ constexpr int HBM = 128, HBN = 64, HBK = 32, HKP = HBK + 8;
 // memory in rank order.  Chosen from the per-image shape only, so an image's output does not depend on the batch.
 constexpr int H_TARGET_CTAS = 264, H_MAX_SPLIT = 8, H_MIN_CHUNKS = 4;
 
+// input, offset, mask and out are NCHW for dcn_forward_half_kernel and NHWC (channels_last) for dcn_forward_nhwc_kernel
 template <typename T> struct DcnHalfPtrs {
     const T *input, *offset, *mask;
     const T *weight;          // tap-major [Co][kh][kw][C]: a (tap, channel chunk) row is contiguous
@@ -437,7 +456,8 @@ template <typename T> struct DcnHalfPtrs {
 template <typename T> struct HalfSmem {
     union {
         struct { T A[2][HBM][HKP]; T B[2][HBN][HKP]; } t;   // double-buffered weight and column tiles
-        float red[HBM][HBN + 4];                           // the fp32 accumulator tile, after the K loop
+        float red[HBM][HBN + 4];                           // the fp32 accumulator tile, after the K loop (NCHW)
+        float red_t[HBN][HBM + 4];                         // the same, pixel-major (NHWC)
     };
 };
 
@@ -454,6 +474,51 @@ __device__ __forceinline__ uint32_t pack2(__nv_bfloat16, float x, float y)
 // round to nearest even; beyond the format's range the result is +-inf, never the largest finite value
 __device__ __forceinline__ __half to_lp(__half, float x) { return __float2half_rn(x); }
 __device__ __forceinline__ __nv_bfloat16 to_lp(__nv_bfloat16, float x) { return __float2bfloat16_rn(x); }
+
+__device__ __forceinline__ float to_f32(__half x) { return __half2float(x); }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 x) { return __bfloat162float(x); }
+
+// NHWC sampler: the column entries of channels ch .. ch + 7 at one sample point, px pointing at channel ch of pixel 0
+// of the image.  Each corner's 8 channels arrive in one 16-byte load (px 16-byte aligned, C % 8 == 0); the values are
+// bilinear()'s on the same up-cast inputs.
+template <typename T>
+__device__ __forceinline__ void bilinear8(const T *px, long long C, const Corners &s, float m, float (&v)[8])
+{
+    uint4 r[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+        r[q] = s.off[q] >= 0 ? __ldg(reinterpret_cast<const uint4 *>(px + s.off[q] * C)) : make_uint4(0, 0, 0, 0);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        float c[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) c[q] = to_f32(reinterpret_cast<const T *>(&r[q])[k]);
+        v[k] = __fmul_rn(m, blend(s.wt, c[0], c[1], c[2], c[3]));
+    }
+}
+
+// NHWC sampler, one channel: px points at the channel in pixel 0 of the image
+template <typename T>
+__device__ __forceinline__ float bilinear_nhwc(const T *px, long long C, const Corners &s)
+{
+    const float v1 = s.off[0] >= 0 ? ld_f32(px + s.off[0] * C) : 0.f;
+    const float v2 = s.off[1] >= 0 ? ld_f32(px + s.off[1] * C) : 0.f;
+    const float v3 = s.off[2] >= 0 ? ld_f32(px + s.off[2] * C) : 0.f;
+    const float v4 = s.off[3] >= 0 ? ld_f32(px + s.off[3] * C) : 0.f;
+    return blend(s.wt, v1, v2, v3, v4);
+}
+
+// the rank-ordered sum over a cluster of S CTAs of the partial at x (each CTA's own copy when S == 1)
+__device__ __forceinline__ float rank_sum(float *x, int S)
+{
+    namespace cg = cooperative_groups;
+    float v = *x;
+    if (S > 1) {
+        v = cg::this_cluster().map_shared_rank(x, 0)[0];
+        for (int q = 1; q < S; ++q) v = __fadd_rn(v, cg::this_cluster().map_shared_rank(x, q)[0]);
+    }
+    return v;
+}
 
 __device__ __forceinline__ void cp_async16(void *dst, const void *src, bool valid)   // zero-fills when !valid
 {
@@ -488,10 +553,11 @@ __device__ __forceinline__ void mma16816(__nv_bfloat16, float (&d)[4], const uin
 // out[b][o][p] = RN_T(bias[o] + sum over (g, tap, c in group g) of W[o][c*T + tap] * RN_T(cols[b][c*T + tap][p])),
 // the sum in fp32 on the tensor cores.  grid (ceil(P / HBN) * S, ceil(Co / HBM), B), clusters of (S, 1, 1) when S > 1;
 // CTA rank r of a cluster runs K chunks [r*n/S, (r+1)*n/S) of the n = dg * T * ceil(Cg / HBK).
-template <typename T>
-__global__ void __launch_bounds__(NT, 2) dcn_forward_half_kernel(DcnArgs a, DcnHalfPtrs<T> t, int S)
+// NHWC (DESIGN.md section 8o) changes only where the sampler reads a corner's channels and the offset and mask, and
+// how the epilogue stores the tile; the tiles, the MMA sequence and the split are the same, so is every output bit.
+template <typename T, bool NHWC>
+__device__ __forceinline__ void forward_half_body(const DcnArgs &a, const DcnHalfPtrs<T> &t, int S, HalfSmem<T> &sm)
 {
-    __shared__ __align__(16) HalfSmem<T> sm;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wm = warp >> 1, wn = warp & 1;
     const int split = blockIdx.x % S, P = a.Ho * a.Wo, p0 = (int)(blockIdx.x / S) * HBN, o0 = blockIdx.y * HBM;
     const int b = blockIdx.z, T_ = a.kh * a.kw, Cg = a.C / a.dg, nct = (Cg + HBK - 1) / HBK, nchunk = a.dg * T_ * nct;
@@ -500,8 +566,11 @@ __global__ void __launch_bounds__(NT, 2) dcn_forward_half_kernel(DcnArgs a, DcnH
     // every 8-channel run of a weight row is 16-byte aligned, so the weight tile arrives by 16-byte cp.async
     const bool vec = ((a.C | Cg) & 7) == 0 && (reinterpret_cast<uintptr_t>(t.weight) & 15) == 0;
     const bool live = o0 + wm * 32 < a.Co;       // this warp's rows hold at least one output channel
-    // the sampler's share of a B tile: pixel sn, channels sk .. sk + 7 of the chunk
-    const int sn = tid % HBN, sk = (tid / HBN) * 8, sp = p0 + sn;
+    // the sampler's share of a B tile: pixel sn, channels sk .. sk + 7 of the chunk.  NCHW: a warp reads one channel
+    // plane at 32 pixels; NHWC: 4 lanes read a pixel's 32 channels, one 64-byte run per corner
+    const int sn = NHWC ? tid / (HBK / 8) : tid % HBN, sk = NHWC ? (tid % (HBK / 8)) * 8 : (tid / HBN) * 8;
+    const int sp = p0 + sn;
+    const bool vin = NHWC && ((a.C | Cg) & 7) == 0 && (reinterpret_cast<uintptr_t>(t.input) & 15) == 0;
 
     float acc[2][4][4];
 #pragma unroll
@@ -523,9 +592,17 @@ __global__ void __launch_bounds__(NT, 2) dcn_forward_half_kernel(DcnArgs a, DcnH
         if (c0 == 0 || it == kb) {
             if (sp < P) {
                 float h, w;
-                sample_coord(a, t.offset, ((long long)b * a.dg + g) * 2 * T_ * P, tap, sp, h, w);
-                s = sample_point(h, w, a.H, a.W);
-                m = ld_f32(t.mask + ((long long)b * a.dg + g) * T_ * P + (long long)tap * P + sp);
+                if constexpr (NHWC) {      // offset [B][Ho][Wo][dg*2*T], mask [B][Ho][Wo][dg*T]
+                    const long long px = (long long)b * P + sp;
+                    const T *op = t.offset + px * (2 * a.dg * T_) + 2 * (g * T_ + tap);
+                    sample_coord_nhwc(a, op, tap, sp, h, w);
+                    s = sample_point(h, w, a.H, a.W);
+                    m = ld_f32(t.mask + px * (a.dg * T_) + g * T_ + tap);
+                } else {
+                    sample_coord(a, t.offset, ((long long)b * a.dg + g) * 2 * T_ * P, tap, sp, h, w);
+                    s = sample_point(h, w, a.H, a.W);
+                    m = ld_f32(t.mask + ((long long)b * a.dg + g) * T_ * P + (long long)tap * P + sp);
+                }
             }
         }
 #pragma unroll
@@ -544,10 +621,21 @@ __global__ void __launch_bounds__(NT, 2) dcn_forward_half_kernel(DcnArgs a, DcnH
         }
         cp_async_commit();
         float v[8];
-        const T *plane = t.input + ((long long)b * a.C + (long long)g * Cg + c0 + sk) * HW;
+        if constexpr (NHWC) {
+            const T *px = t.input + (long long)b * HW * a.C + (long long)g * Cg + c0 + sk;
+            if (vin && sp < P && c0 + sk < Cg) {
+                bilinear8(px, a.C, s, m, v);
+            } else {
 #pragma unroll
-        for (int q = 0; q < 8; ++q)
-            v[q] = (sp < P && c0 + sk + q < Cg) ? __fmul_rn(m, bilinear(plane + q * HW, s.off, s.wt)) : 0.f;
+                for (int q = 0; q < 8; ++q)
+                    v[q] = (sp < P && c0 + sk + q < Cg) ? __fmul_rn(m, bilinear_nhwc(px + q, a.C, s)) : 0.f;
+            }
+        } else {
+            const T *plane = t.input + ((long long)b * a.C + (long long)g * Cg + c0 + sk) * HW;
+#pragma unroll
+            for (int q = 0; q < 8; ++q)
+                v[q] = (sp < P && c0 + sk + q < Cg) ? __fmul_rn(m, bilinear(plane + q * HW, s.off, s.wt)) : 0.f;
+        }
         uint4 pk;
         pk.x = pack2(T{}, v[0], v[1]); pk.y = pack2(T{}, v[2], v[3]);
         pk.z = pack2(T{}, v[4], v[5]); pk.w = pack2(T{}, v[6], v[7]);
@@ -590,24 +678,49 @@ __global__ void __launch_bounds__(NT, 2) dcn_forward_half_kernel(DcnArgs a, DcnH
 #pragma unroll
             for (int hf = 0; hf < 2; ++hf) {
                 const int row = wm * 32 + mt * 16 + hf * 8 + lane / 4, col = wn * 32 + nt * 8 + (lane % 4) * 2;
-                sm.red[row][col] = acc[mt][nt][2 * hf];
-                sm.red[row][col + 1] = acc[mt][nt][2 * hf + 1];
+                if constexpr (NHWC) {
+                    sm.red_t[col][row] = acc[mt][nt][2 * hf];
+                    sm.red_t[col + 1][row] = acc[mt][nt][2 * hf + 1];
+                } else {
+                    sm.red[row][col] = acc[mt][nt][2 * hf];
+                    sm.red[row][col + 1] = acc[mt][nt][2 * hf + 1];
+                }
             }
     namespace cg = cooperative_groups;
     if (S > 1) cg::this_cluster().sync(); else __syncthreads();
     // rank `split` stores rows [split*HBM/S, (split+1)*HBM/S) of the tile, adding the ranks' partials in rank order
     const int r0 = split * HBM / S, r1 = (split + 1) * HBM / S;
-    for (int e = r0 * HBN + tid; e < r1 * HBN; e += NT) {
-        const int row = e / HBN, col = e % HBN, o = o0 + row, p = p0 + col;
-        if (o >= a.Co || p >= P) continue;
-        float v = sm.red[row][col];
-        if (S > 1) {
-            v = cg::this_cluster().map_shared_rank(&sm.red[row][col], 0)[0];
-            for (int q = 1; q < S; ++q) v = __fadd_rn(v, cg::this_cluster().map_shared_rank(&sm.red[row][col], q)[0]);
+    if constexpr (NHWC) {                                  // output channels fastest: a warp stores a contiguous run
+        const int nr = r1 - r0;
+        for (int e = tid; e < nr * HBN; e += NT) {
+            const int col = e / nr, row = r0 + e % nr, o = o0 + row, p = p0 + col;
+            if (o >= a.Co || p >= P) continue;
+            t.out[((long long)b * P + p) * a.Co + o] = to_lp(T{}, rank_sum(&sm.red_t[col][row], S));
         }
-        t.out[((long long)b * a.Co + o) * P + p] = to_lp(T{}, v);
+    } else {
+        for (int e = r0 * HBN + tid; e < r1 * HBN; e += NT) {
+            const int row = e / HBN, col = e % HBN, o = o0 + row, p = p0 + col;
+            if (o >= a.Co || p >= P) continue;
+            t.out[((long long)b * a.Co + o) * P + p] = to_lp(T{}, rank_sum(&sm.red[row][col], S));
+        }
     }
     if (S > 1) cg::this_cluster().sync();                  // no CTA leaves while another reads its partials
+}
+
+template <typename T>
+__global__ void __launch_bounds__(NT, 2) dcn_forward_half_kernel(DcnArgs a, DcnHalfPtrs<T> t, int S)
+{
+    __shared__ __align__(16) HalfSmem<T> sm;
+    forward_half_body<T, false>(a, t, S, sm);
+}
+
+// the same forward on NHWC input, offset, mask and output (the name leaves out "forward_half" on purpose: the register
+// test counts the NCHW kernels by it)
+template <typename T>
+__global__ void __launch_bounds__(NT, 2) dcn_forward_nhwc_kernel(DcnArgs a, DcnHalfPtrs<T> t, int S)
+{
+    __shared__ __align__(16) HalfSmem<T> sm;
+    forward_half_body<T, true>(a, t, S, sm);
 }
 
 } // namespace
@@ -685,7 +798,7 @@ int dcn_half_splits(const DcnArgs &a)
 }
 
 template <typename T>
-int launch_dcn_forward_half(const DcnArgs &a, const DcnHalfPtrs<T> &t, cudaStream_t stream)
+int launch_dcn_forward_half(const DcnArgs &a, const DcnHalfPtrs<T> &t, bool nhwc, cudaStream_t stream)
 {
     const int S = dcn_half_splits(a);
     cudaLaunchConfig_t cfg = {};
@@ -697,8 +810,8 @@ int launch_dcn_forward_half(const DcnArgs &a, const DcnHalfPtrs<T> &t, cudaStrea
     cluster.val.clusterDim.x = S; cluster.val.clusterDim.y = 1; cluster.val.clusterDim.z = 1;
     cfg.attrs = &cluster;
     cfg.numAttrs = S > 1 ? 1 : 0;
-    const cudaError_t e = cudaLaunchKernelEx(&cfg, dcn_forward_half_kernel<T>, a, t, S);
-    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "dcn half forward kernel");
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, nhwc ? dcn_forward_nhwc_kernel<T> : dcn_forward_half_kernel<T>, a, t, S);
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, nhwc ? "dcn nhwc forward kernel" : "dcn half forward kernel");
 }
 
 template <typename T>
@@ -707,6 +820,24 @@ DcnHalfPtrs<T> half_ptrs(const void *input, const void *offset, const void *mask
 {
     return DcnHalfPtrs<T>{static_cast<const T *>(input), static_cast<const T *>(offset), static_cast<const T *>(mask),
                           static_cast<const T *>(weight), static_cast<const T *>(bias), static_cast<T *>(output)};
+}
+
+// the checks and launch of pvb_dcn_forward_half (nhwc false) and pvb_dcn_forward_half_nhwc (true)
+int dcn_forward_half(const pvb_dcn_desc *d, int32_t dtype, const void *input, const void *offset, const void *mask,
+                     const void *weight, const void *bias, void *output, bool nhwc, pvb_stream_t stream)
+{
+    if (dtype != PVB_DCN_F16 && dtype != PVB_DCN_BF16)
+        return fail(PVB_ERR_INVALID, "dtype=%d must be PVB_DCN_F16 (%d) or PVB_DCN_BF16 (%d)", dtype, PVB_DCN_F16,
+                    PVB_DCN_BF16);
+    DcnArgs a;
+    if (int rc = dcn_args(d, a)) return rc;
+    if (a.B == 0) return PVB_OK;
+    if (!input || !offset || !mask || !weight || !bias || !output) return fail(PVB_ERR_INVALID, "NULL tensor");
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return dtype == PVB_DCN_F16
+               ? launch_dcn_forward_half(a, half_ptrs<__half>(input, offset, mask, weight, bias, output), nhwc, st)
+               : launch_dcn_forward_half(a, half_ptrs<__nv_bfloat16>(input, offset, mask, weight, bias, output), nhwc,
+                                         st);
 }
 
 } // namespace
@@ -735,17 +866,14 @@ PVB_API int pvb_dcn_forward_half(const pvb_dcn_desc *d, int32_t dtype, const voi
                                  const void *mask, const void *weight, const void *bias, void *output,
                                  pvb_stream_t stream)
 {
-    if (dtype != PVB_DCN_F16 && dtype != PVB_DCN_BF16)
-        return fail(PVB_ERR_INVALID, "dtype=%d must be PVB_DCN_F16 (%d) or PVB_DCN_BF16 (%d)", dtype, PVB_DCN_F16,
-                    PVB_DCN_BF16);
-    DcnArgs a;
-    if (int rc = dcn_args(d, a)) return rc;
-    if (a.B == 0) return PVB_OK;
-    if (!input || !offset || !mask || !weight || !bias || !output) return fail(PVB_ERR_INVALID, "NULL tensor");
-    const cudaStream_t st = static_cast<cudaStream_t>(stream);
-    return dtype == PVB_DCN_F16
-               ? launch_dcn_forward_half(a, half_ptrs<__half>(input, offset, mask, weight, bias, output), st)
-               : launch_dcn_forward_half(a, half_ptrs<__nv_bfloat16>(input, offset, mask, weight, bias, output), st);
+    return dcn_forward_half(d, dtype, input, offset, mask, weight, bias, output, false, stream);
+}
+
+PVB_API int pvb_dcn_forward_half_nhwc(const pvb_dcn_desc *d, int32_t dtype, const void *input, const void *offset,
+                                      const void *mask, const void *weight, const void *bias, void *output,
+                                      pvb_stream_t stream)
+{
+    return dcn_forward_half(d, dtype, input, offset, mask, weight, bias, output, true, stream);
 }
 
 PVB_API size_t pvb_dcn_backward_workspace_bytes(const pvb_dcn_desc *d, int32_t chunk)

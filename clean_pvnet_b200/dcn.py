@@ -18,6 +18,13 @@ bf16 input (what the DLA-34's convolutions emit under torch.autocast, or a .half
 mask, weight and bias to its dtype, round to nearest, and runs the tensor-core forward (DESIGN.md section 8n); the
 backward is the fp32 one on exact up-casts of those operands, and each gradient comes back in its tensor's dtype, so an
 fp32 parameter gets an fp32 gradient.  The dispatch does not look at the autocast state.
+
+The layout is the input's.  An fp16 / bf16 input that is channels_last and not NCHW-contiguous (what a model moved to
+torch.channels_last feeds its DCN layers) runs the NHWC twin of the tensor-core forward (DESIGN.md section 8o) with no
+copy of the input; offset and mask are brought to channels_last (a no-op for the ones DCN builds from a channels_last
+input), and the output is channels_last with the values the NCHW call returns, bit for bit.  Every other input (fp32 in
+any layout, NCHW, or contiguous in both layouts) is made NCHW-contiguous and returns NCHW, as before.  The backward is
+the same in both layouts: NCHW fp32, so a channels_last call's gradients equal the NCHW call's.
 """
 import ctypes
 import math
@@ -95,6 +102,17 @@ def _check(input, offset, mask, weight, bias, d):
             raise RuntimeError(f"dcn_v2_conv: {name} must be {shape}, got {list(ts[name].shape)}")
 
 
+def _nhwc(input):
+    """Whether a forward runs the NHWC kernel: an fp16 / bf16 input that is channels_last-contiguous and not
+    NCHW-contiguous.  An empty batch is contiguous in both layouts whatever its strides, so there the strides decide."""
+    if input.dtype not in HALF:
+        return False
+    B, C, H, W = input.shape
+    if B == 0:
+        return C > 1 and H * W > 1 and input.stride() == (H * W * C, 1, W * C, C)
+    return input.is_contiguous(memory_format=torch.channels_last) and not input.is_contiguous()
+
+
 def _call(entry, dev, *args):
     args = [ctypes.c_void_p(a.data_ptr()) if isinstance(a, torch.Tensor) else a for a in args]
     with torch.cuda.device(dev):
@@ -102,16 +120,23 @@ def _call(entry, dev, *args):
 
 
 def dcn_forward(input, offset, mask, weight, bias, stride, padding, dilation, deformable_groups):
-    """The forward of dcn_v2_conv without autograd: output [B,C_out,Ho,Wo] in the compute dtype on input's device; no
-    host sync."""
+    """The forward of dcn_v2_conv without autograd: output [B,C_out,Ho,Wo] in the compute dtype on input's device,
+    channels_last when the input takes the NHWC path (see _nhwc); no host sync."""
     offset, mask, weight, bias = _operands(input, offset, mask, weight, bias)
     d = _desc(input, weight, stride, padding, dilation, deformable_groups)
     _check(input, offset, mask, weight, bias, d)
     ho, wo = _out_hw(d)
-    out = torch.empty((d.B, d.C_out, ho, wo), dtype=input.dtype, device=input.device)
+    nhwc = _nhwc(input)
+    layout = torch.channels_last if nhwc else torch.contiguous_format
+    out = torch.empty((d.B, d.C_out, ho, wo), dtype=input.dtype, device=input.device, memory_format=layout)
     if d.B and input.dtype == torch.float32:
         c = [t.contiguous() for t in (input, offset, mask, weight, bias)]
         _call("pvb_dcn_forward", input.device, ctypes.byref(d), *c, out)
+    elif d.B and nhwc:
+        off, m = (t.contiguous(memory_format=torch.channels_last) for t in (offset, mask))
+        w = weight.permute(0, 2, 3, 1).contiguous()          # tap-major [C_out, kh, kw, C], as the kernel reads it
+        _call("pvb_dcn_forward_half_nhwc", input.device, ctypes.byref(d), HALF[input.dtype], input, off, m, w,
+              bias.contiguous(), out)
     elif d.B:
         x, off, m, b = (t.contiguous() for t in (input, offset, mask, bias))
         w = weight.permute(0, 2, 3, 1).contiguous()          # tap-major [C_out, kh, kw, C], as the kernel reads it

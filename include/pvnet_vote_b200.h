@@ -627,6 +627,18 @@ PVB_API int pvb_dcn_forward_half(const pvb_dcn_desc *d, int32_t dtype, const voi
                                  const void *mask, const void *weight, const void *bias, void *output,
                                  pvb_stream_t stream);
 
+/* Replaces dcn_v2_cuda_forward (dcn_v2_cuda.cu:43) for channels_last models (DESIGN.md section 8o): pvb_dcn_forward_half
+ * on NHWC tensors.  input [B][H][W][C], offset [B][Ho][Wo][dg*2*kh*kw], mask [B][Ho][Wo][dg*kh*kw] and output
+ * [B][Ho][Wo][C_out] are dense in that order (torch's channels_last layout of the shapes above); weight (tap-major) and
+ * bias are as in pvb_dcn_forward_half.  The output's values are pvb_dcn_forward_half's on the same values in NCHW, bit
+ * for bit: the columns, the K order, the tensor-core sequence and the split are the same.  When C and C/dg are
+ * multiples of 8 and input is 16-byte aligned, each corner's 8 channels arrive in one 16-byte load.  Same checks,
+ * refusals (unknown dtype, malformed descriptor, NULL tensor, all before any CUDA call) and guarantees as
+ * pvb_dcn_forward_half; B == 0 is a no-op.  The backward is pvb_dcn_backward on NCHW fp32 copies, as for the NCHW call. */
+PVB_API int pvb_dcn_forward_half_nhwc(const pvb_dcn_desc *d, int32_t dtype, const void *input, const void *offset,
+                                      const void *mask, const void *weight, const void *bias, void *output,
+                                      pvb_stream_t stream);
+
 /* Replaces dcn_v2_cuda_backward (dcn_v2_cuda.cu:206) for the whole batch: grad_cols = weight^T . grad_output goes to the
  * workspace `chunk` images at a time (the only column matrix stored); grad_offset / grad_mask (the reference's
  * col2im_coord: grad_mask = sum grad_col * value, grad_offset = sum d(value)/d(h, w) * grad_col * mask, 0 for a point
