@@ -126,6 +126,9 @@ SIGNATURES = {
     "pvb_dcn_backward_workspace_bytes": (_sz, [ctypes.POINTER(PvbDcnDesc), _i32]),
     "pvb_dcn_backward": (ctypes.c_int, [ctypes.POINTER(PvbDcnDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                         _i32, _vp, _sz, _vp]),
+    "pvb_dcn_forward_tf32": (ctypes.c_int, [ctypes.POINTER(PvbDcnDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "pvb_dcn_backward_tf32": (ctypes.c_int, [ctypes.POINTER(PvbDcnDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                             _vp, _i32, _vp, _sz, _vp]),
     "pvb_dcn_pool_forward": (ctypes.c_int, [ctypes.POINTER(PvbDcnPoolDesc), _vp, _vp, _vp, _vp, _vp, _vp]),
     "pvb_dcn_pool_backward": (ctypes.c_int, [ctypes.POINTER(PvbDcnPoolDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "pvb_read_status": (ctypes.c_int, [_dp, _vp, _vp]),

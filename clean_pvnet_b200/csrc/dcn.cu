@@ -9,6 +9,11 @@
 // split-K partials reduced in a fixed order, and a fixed-order grad_bias.  Everything but grad_input is bitwise
 // reproducible.  All arithmetic is FP32 FFMA (no TF32, no tensor cores).
 //
+// The TF32 path (DESIGN.md section 8p), which the Python layer takes for fp32 inputs when torch allows TF32 matmuls,
+// is a third forward kernel and TF32 twins of the backward's two products, grad_cols and grad_weight: the same sampler
+// and tiles, each operand rounded once to TF32 (cvt.rna) and multiplied by mma.sync m16n8k8 with fp32 accumulation.
+// The backward's other kernels, its plan and its workspace are shared.
+//
 // The half-precision forward (fp16 or bf16 operands, DESIGN.md section 8n) is a second implicit-GEMM kernel on the
 // tensor cores: the same sampler, fed the up-cast inputs, fills bf16 / fp16 B tiles in shared memory; the weight
 // tiles arrive by cp.async; mma.sync m16n8k16 accumulates in fp32.  Its NHWC (channels_last) twin (section 8o) shares
@@ -840,6 +845,385 @@ int dcn_forward_half(const pvb_dcn_desc *d, int32_t dtype, const void *input, co
                                          st);
 }
 
+// ---- the TF32 path: fp32 operands rounded once to TF32 on the tensor cores (DESIGN.md section 8p) -------------------
+// The forward and the backward's two products multiply TF_BM x TF_BN tiles over TF_BK-deep steps (the FFMA kernels'
+// 64 x 128 x 16, so the backward plan is dcn_plan's) with 8 warps as 2 (rows) x 4 (columns) of 32 x 32, each an array of
+// 2 x 4 mma.sync m16n8k8.  Operand tiles are fp32 in shared memory, double-buffered, and rounded to TF32 (cvt.rna) as
+// the fragments are loaded.  A tile is stored row-major, [row][k] with a pitch of TF_BK + 4 floats, or k-major,
+// [k][row] with a pitch of rows + 8, whichever its global layout fills coalesced; either pitch puts the 32 lanes of a
+// fragment load in 32 distinct banks.
+constexpr int TF_BM = 64, TF_BN = 128, TF_BK = 16;
+// the forward's split-K, chosen as the half-precision forward's: a cluster of up to TF_MAX_SPLIT CTAs, each keeping at
+// least TF_MIN_CHUNKS K chunks, when the tiles would not fill two CTAs per H100 SM; a function of the per-image shape
+constexpr int TF_TARGET_CTAS = 264, TF_MAX_SPLIT = 8, TF_MIN_CHUNKS = 4;
+
+template <int ROWS, bool KMAJOR> struct TfTile {
+    static constexpr int PITCH = KMAJOR ? ROWS + 8 : TF_BK + 4;
+    static constexpr int SIZE = KMAJOR ? TF_BK * PITCH : ROWS * PITCH;
+    __device__ static __forceinline__ int at(int row, int k) { return KMAJOR ? k * PITCH + row : row * PITCH + k; }
+};
+
+// round to the nearest TF32 value (10-bit mantissa), ties away from zero; the result is an fp32 bit pattern
+__device__ __forceinline__ uint32_t tf32_rna(float x)
+{
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;\n" : "=r"(r) : "f"(x));
+    return r;
+}
+
+__device__ __forceinline__ void mma1688(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1)
+{
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
+                 "{%0,%1,%2,%3};\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+// acc[mt][nt] += A B^T over one TF_BK-deep step of the tiles A (TF_BM rows) and B (TF_BN rows), for the warp at
+// rows wm*32 + mt*16 .., columns wn*32 + nt*8 ..; the m16n8k8 fragments: A (row r, k) at lane 4*(r % 8) + k % 4, B and
+// the accumulator alike (PTX ISA, "Matrix Fragments for mma.m16n8k8" with .tf32)
+template <typename LA, typename LB>
+__device__ __forceinline__ void tf32_step(const float *A, const float *B, float (&acc)[2][4][4], int wm, int wn, int lane)
+{
+    const int gr = lane >> 2, tg = lane & 3;
+#pragma unroll
+    for (int ks = 0; ks < TF_BK; ks += 8) {
+        uint32_t af[2][4], bf[4][2];
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) {
+            const int r = wm * 32 + mt * 16 + gr;
+            af[mt][0] = tf32_rna(A[LA::at(r, ks + tg)]);
+            af[mt][1] = tf32_rna(A[LA::at(r + 8, ks + tg)]);
+            af[mt][2] = tf32_rna(A[LA::at(r, ks + tg + 4)]);
+            af[mt][3] = tf32_rna(A[LA::at(r + 8, ks + tg + 4)]);
+        }
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) {
+            const int n = wn * 32 + nt * 8 + gr;
+            bf[nt][0] = tf32_rna(B[LB::at(n, ks + tg)]);
+            bf[nt][1] = tf32_rna(B[LB::at(n, ks + tg + 4)]);
+        }
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt) mma1688(acc[mt][nt], af[mt], bf[nt][0], bf[nt][1]);
+    }
+}
+
+using FwA = TfTile<TF_BM, false>;   // forward: weight [o][c]
+using FwB = TfTile<TF_BN, false>;   //          columns [p][c]
+using GcA = TfTile<TF_BM, true>;    // grad_cols: weight [o][k], k-major
+using GcB = TfTile<TF_BN, true>;    //            grad_out [o][p], k-major
+using GwA = TfTile<TF_BM, false>;   // grad_weight: grad_out [o][pixel]
+using GwB = TfTile<TF_BN, false>;   //              columns [c][pixel]
+
+struct TfFwdSmem {
+    union {
+        struct { float A[2][FwA::SIZE]; float B[2][FwB::SIZE]; } t;   // double-buffered weight and column tiles
+        float red[TF_BM][TF_BN + 8];                                  // the fp32 accumulator tile, after the K loop
+    };
+};
+
+// out[b][o][p] = bias[o] + sum over (g, tap, c in group g) of RN_tf32(W[o][c*T + tap]) * RN_tf32(cols[b][c*T + tap][p]),
+// the sum in fp32 on the tensor cores, from the bias.  a.weight is tap-major, [Co][kh][kw][C].  grid
+// (ceil(P / TF_BN) * S, ceil(Co / TF_BM), B), clusters of (S, 1, 1) when S > 1; CTA rank r runs K chunks
+// [r*n/S, (r+1)*n/S) of the n = dg * T * ceil(Cg / TF_BK), and the ranks add their partials in rank order.
+__global__ void __launch_bounds__(NT, 2) dcn_forward_tf32_kernel(DcnArgs a, int S)
+{
+    __shared__ __align__(16) TfFwdSmem sm;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wm = warp >> 2, wn = warp & 3;
+    const int split = blockIdx.x % S, P = a.Ho * a.Wo, p0 = (int)(blockIdx.x / S) * TF_BN, o0 = blockIdx.y * TF_BM;
+    const int b = blockIdx.z, T = a.kh * a.kw, Cg = a.C / a.dg, nct = (Cg + TF_BK - 1) / TF_BK, nchunk = a.dg * T * nct;
+    const int kb = (int)((long long)split * nchunk / S), ke = (int)((long long)(split + 1) * nchunk / S);
+    const long long HW = (long long)a.H * a.W, K = (long long)a.C * T;
+    // every 4-channel run of a weight row is 16-byte aligned, so the weight tile arrives by 16-byte cp.async
+    const bool vec = ((a.C | Cg) & 3) == 0 && (reinterpret_cast<uintptr_t>(a.weight) & 15) == 0;
+    const bool live = o0 + wm * 32 < a.Co;       // this warp's rows hold at least one output channel
+    // the sampler's share of a B tile: pixel sn, channels sk .. sk + 7 of the chunk; a warp reads one plane at 32 pixels
+    const int sn = tid % TF_BN, sk = (tid / TF_BN) * 8, sp = p0 + sn;
+
+    float acc[2][4][4];
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+            const int o = o0 + wm * 32 + mt * 16 + hf * 8 + lane / 4;
+            const float bv = (split == 0 && o < a.Co) ? __ldg(a.bias + o) : 0.f;
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt) acc[mt][nt][2 * hf] = acc[mt][nt][2 * hf + 1] = bv;
+        }
+
+    // the sample point of pixel sp at the current tap: computed once per tap, reused over the group's channels
+    Corners s = {};
+    float m = 0.f;
+
+    auto stage = [&](int it, int buf) {
+        const int g = it / (T * nct), tap = (it / nct) % T, c0 = (it % nct) * TF_BK;
+        if ((c0 == 0 || it == kb) && sp < P) {
+            float h, w;
+            sample_coord(a, a.offset, ((long long)b * a.dg + g) * 2 * T * P, tap, sp, h, w);
+            s = sample_point(h, w, a.H, a.W);
+            m = __ldg(a.mask + ((long long)b * a.dg + g) * T * P + (long long)tap * P + sp);
+        }
+        {                                                  // the weight tile, 4 channels per thread
+            const int row = tid / (TF_BK / 4), v = (tid % (TF_BK / 4)) * 4, o = o0 + row, c = c0 + v;
+            float *dst = &sm.t.A[buf][FwA::at(row, v)];
+            const float *src = a.weight + (long long)o * K + (long long)tap * a.C + (long long)g * Cg + c;
+            if (vec) {
+                const bool ok = o < a.Co && c < Cg;
+                cp_async16(dst, ok ? src : a.weight, ok);
+            } else {
+#pragma unroll
+                for (int q = 0; q < 4; ++q) dst[q] = (o < a.Co && c + q < Cg) ? __ldg(src + q) : 0.f;
+            }
+        }
+        cp_async_commit();
+        const float *plane = a.input + ((long long)b * a.C + (long long)g * Cg + c0 + sk) * HW;
+        float v[8];
+#pragma unroll
+        for (int q = 0; q < 8; ++q)
+            v[q] = (sp < P && c0 + sk + q < Cg) ? __fmul_rn(m, bilinear(plane + q * HW, s.off, s.wt)) : 0.f;
+        float4 *dst = reinterpret_cast<float4 *>(&sm.t.B[buf][FwB::at(sn, sk)]);
+        dst[0] = make_float4(v[0], v[1], v[2], v[3]);
+        dst[1] = make_float4(v[4], v[5], v[6], v[7]);
+    };
+
+    stage(kb, 0);
+    cp_async_wait_all();
+    __syncthreads();
+    for (int it = kb; it < ke; ++it) {
+        const int buf = (it - kb) & 1;
+        if (it + 1 < ke) stage(it + 1, buf ^ 1);           // the next chunk's tiles load while this one multiplies
+        if (live) tf32_step<FwA, FwB>(sm.t.A[buf], sm.t.B[buf], acc, wm, wn, lane);
+        cp_async_wait_all();
+        __syncthreads();
+    }
+
+    // the loop ended on a barrier: the tiles are consumed and the accumulator tile may take their place
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+            for (int hf = 0; hf < 2; ++hf) {
+                const int row = wm * 32 + mt * 16 + hf * 8 + lane / 4, col = wn * 32 + nt * 8 + (lane % 4) * 2;
+                *reinterpret_cast<float2 *>(&sm.red[row][col]) = make_float2(acc[mt][nt][2 * hf], acc[mt][nt][2 * hf + 1]);
+            }
+    namespace cg = cooperative_groups;
+    if (S > 1) cg::this_cluster().sync(); else __syncthreads();
+    // rank `split` stores rows [split*TF_BM/S, (split+1)*TF_BM/S) of the tile, adding the ranks' partials in rank order
+    const int r0 = split * TF_BM / S, r1 = (split + 1) * TF_BM / S;
+    for (int e = r0 * TF_BN + tid; e < r1 * TF_BN; e += NT) {
+        const int row = e / TF_BN, col = e % TF_BN, o = o0 + row, p = p0 + col;
+        if (o >= a.Co || p >= P) continue;
+        a.out[((long long)b * a.Co + o) * P + p] = rank_sum(&sm.red[row][col], S);
+    }
+    if (S > 1) cg::this_cluster().sync();                  // no CTA leaves while another reads its partials
+}
+
+// grad_cols[bl][k][p] = sum over o of RN_tf32(W[o][k]) * RN_tf32(grad_out[b0 + bl][o][p]) on the tensor cores, in
+// TF_BK-deep steps of o.  grid (ceil(P / TF_BN), ceil(K / TF_BM), nb)
+__global__ void __launch_bounds__(NT, 2) dcn_grad_cols_tf32_kernel(DcnArgs a, int b0)
+{
+    __shared__ __align__(16) float As[2][GcA::SIZE];
+    __shared__ __align__(16) float Bs[2][GcB::SIZE];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wm = warp >> 2, wn = warp & 3;
+    const int P = a.Ho * a.Wo, p0 = blockIdx.x * TF_BN, k0 = blockIdx.y * TF_BM, bl = blockIdx.z;
+    const long long K = (long long)a.C * a.kh * a.kw;
+    const float *go = a.grad_out + (long long)(b0 + bl) * a.Co * P;
+    float acc[2][4][4] = {};
+    float ra[TF_BK * TF_BM / NT], rb[TF_BK * TF_BN / NT];  // the next step's tiles, loaded while this one multiplies
+    auto fetch = [&](int o0) {
+#pragma unroll
+        for (int r = 0; r < TF_BK * TF_BM / NT; ++r) {
+            const int e = tid + r * NT, kk = e / TF_BM, m = e % TF_BM;
+            ra[r] = (o0 + kk < a.Co && k0 + m < K) ? __ldg(a.weight + (long long)(o0 + kk) * K + k0 + m) : 0.f;
+        }
+#pragma unroll
+        for (int r = 0; r < TF_BK * TF_BN / NT; ++r) {
+            const int e = tid + r * NT, kk = e / TF_BN, n = e % TF_BN;
+            rb[r] = (o0 + kk < a.Co && p0 + n < P) ? __ldg(go + (long long)(o0 + kk) * P + p0 + n) : 0.f;
+        }
+    };
+    auto put = [&](int buf) {
+#pragma unroll
+        for (int r = 0; r < TF_BK * TF_BM / NT; ++r) {
+            const int e = tid + r * NT;
+            As[buf][GcA::at(e % TF_BM, e / TF_BM)] = ra[r];
+        }
+#pragma unroll
+        for (int r = 0; r < TF_BK * TF_BN / NT; ++r) {
+            const int e = tid + r * NT;
+            Bs[buf][GcB::at(e % TF_BN, e / TF_BN)] = rb[r];
+        }
+    };
+    const int n = (a.Co + TF_BK - 1) / TF_BK;
+    fetch(0);
+    put(0);
+    __syncthreads();
+    for (int i = 0; i < n; ++i) {
+        const int buf = i & 1;
+        if (i + 1 < n) fetch((i + 1) * TF_BK);
+        tf32_step<GcA, GcB>(As[buf], Bs[buf], acc, wm, wn, lane);
+        if (i + 1 < n) put(buf ^ 1);
+        __syncthreads();
+    }
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+            const long long k = k0 + wm * 32 + mt * 16 + hf * 8 + lane / 4;
+            if (k >= K) continue;
+            float *dst = a.cols + ((long long)bl * K + k) * P;
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt) {
+                const int p = p0 + wn * 32 + nt * 8 + (lane % 4) * 2;
+                if (p < P) dst[p] = acc[mt][nt][2 * hf];
+                if (p + 1 < P) dst[p + 1] = acc[mt][nt][2 * hf + 1];
+            }
+        }
+}
+
+// split s of grad_weight: part[s][o][c*T + tap] = sum over the split's (image, pixel) range, in TF_BK-pixel steps, of
+// RN_tf32(grad_out[b][o][p]) * RN_tf32(cols[b][c*T + tap][p]), the columns re-sampled like the forward.
+// grid (ntile_n, ceil(Co / TF_BM), S) of dcn_plan; tile n covers channels cb .. cb + TF_BN - 1 of group g at tap
+__global__ void __launch_bounds__(NT, 2) dcn_grad_weight_tf32_kernel(DcnArgs a, long long span, float *part)
+{
+    __shared__ __align__(16) float As[2][GwA::SIZE];
+    __shared__ __align__(16) float Bs[2][GwB::SIZE];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wm = warp >> 2, wn = warp & 3;
+    const int T = a.kh * a.kw, Cg = a.C / a.dg, nct = (Cg + TF_BN - 1) / TF_BN;
+    const int g = blockIdx.x / (T * nct), tap = (blockIdx.x / nct) % T, cb = (blockIdx.x % nct) * TF_BN;
+    const int o0 = blockIdx.y * TF_BM, P = a.Ho * a.Wo;
+    const long long K = (long long)a.C * T, HW = (long long)a.H * a.W, Q = (long long)a.B * P;
+    const long long q0 = (long long)blockIdx.z * span, q1 = min(Q, q0 + span);
+    // this thread's pixel of a step, and its first row (output channel) and column (channel); rows and columns go by 16
+    const int kk = tid % TF_BK, rn = tid / TF_BK;
+    float acc[2][4][4] = {};
+    float ra[TF_BM / 16], rb[TF_BN / 16];                  // the next step's tiles, loaded while this one multiplies
+    auto fetch = [&](long long qs) {
+        const long long q = qs + kk;
+        if (q < q1) {
+            const int b = (int)(q / P), p = (int)(q - (long long)b * P);
+            float h, w;
+            sample_coord(a, a.offset, ((long long)b * a.dg + g) * 2 * T * P, tap, p, h, w);
+            const Corners s = sample_point(h, w, a.H, a.W);
+            const float m = __ldg(a.mask + ((long long)b * a.dg + g) * T * P + (long long)tap * P + p);
+#pragma unroll
+            for (int r = 0; r < TF_BM / 16; ++r) {
+                const int o = o0 + rn + 16 * r;
+                ra[r] = o < a.Co ? __ldg(a.grad_out + ((long long)b * a.Co + o) * P + p) : 0.f;
+            }
+#pragma unroll
+            for (int r = 0; r < TF_BN / 16; ++r) {
+                const int c = cb + rn + 16 * r;
+                rb[r] = c < Cg ? __fmul_rn(m, bilinear(a.input + ((long long)b * a.C + g * Cg + c) * HW, s.off, s.wt))
+                               : 0.f;
+            }
+        } else {
+#pragma unroll
+            for (int r = 0; r < TF_BM / 16; ++r) ra[r] = 0.f;
+#pragma unroll
+            for (int r = 0; r < TF_BN / 16; ++r) rb[r] = 0.f;
+        }
+    };
+    auto put = [&](int buf) {
+#pragma unroll
+        for (int r = 0; r < TF_BM / 16; ++r) As[buf][GwA::at(rn + 16 * r, kk)] = ra[r];
+#pragma unroll
+        for (int r = 0; r < TF_BN / 16; ++r) Bs[buf][GwB::at(rn + 16 * r, kk)] = rb[r];
+    };
+    const long long n = (q1 - q0 + TF_BK - 1) / TF_BK;
+    fetch(q0);
+    put(0);
+    __syncthreads();
+    for (long long i = 0; i < n; ++i) {
+        const int buf = (int)(i & 1);
+        if (i + 1 < n) fetch(q0 + (i + 1) * TF_BK);
+        tf32_step<GwA, GwB>(As[buf], Bs[buf], acc, wm, wn, lane);
+        if (i + 1 < n) put(buf ^ 1);
+        __syncthreads();
+    }
+    float *dst = part + (long long)blockIdx.z * a.Co * K;
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+            const int o = o0 + wm * 32 + mt * 16 + hf * 8 + lane / 4;
+            if (o >= a.Co) continue;
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+                for (int j = 0; j < 2; ++j) {
+                    const int ch = cb + wn * 32 + nt * 8 + (lane % 4) * 2 + j;
+                    if (ch < Cg) dst[(long long)o * K + (long long)(g * Cg + ch) * T + tap] = acc[mt][nt][2 * hf + j];
+                }
+        }
+}
+
+// the split-K factor of the TF32 forward: a function of the per-image shape only
+int dcn_tf32_splits(const DcnArgs &a)
+{
+    const int T = a.kh * a.kw, Cg = a.C / a.dg;
+    const long long nchunk = (long long)a.dg * T * ((Cg + TF_BK - 1) / TF_BK);
+    const long long tiles = ((long long)a.Ho * a.Wo + TF_BN - 1) / TF_BN * ((a.Co + TF_BM - 1) / TF_BM);
+    long long S = (TF_TARGET_CTAS + tiles - 1) / tiles;
+    if (S > TF_MAX_SPLIT) S = TF_MAX_SPLIT;
+    if (S > nchunk / TF_MIN_CHUNKS) S = nchunk / TF_MIN_CHUNKS;
+    return S < 1 ? 1 : (int)S;
+}
+
+// the checks and launches of pvb_dcn_backward (tf32 false: FFMA products) and pvb_dcn_backward_tf32 (true: grad_cols
+// and grad_weight on the tensor cores); the plan, and every other kernel, is the same
+int dcn_backward(const pvb_dcn_desc *d, const float *input, const float *offset, const float *mask, const float *weight,
+                 const float *grad_output, float *grad_input, float *grad_offset, float *grad_mask, float *grad_weight,
+                 float *grad_bias, int32_t chunk, void *workspace, size_t workspace_bytes, bool tf32,
+                 pvb_stream_t stream)
+{
+    DcnArgs a;
+    if (int rc = dcn_args(d, a)) return rc;
+    if (a.B == 0) return PVB_OK;
+    if (!input || !offset || !mask || !weight || !grad_output || !grad_input || !grad_offset || !grad_mask ||
+        !grad_weight || !grad_bias)
+        return fail(PVB_ERR_INVALID, "NULL tensor");
+    const DcnPlan pl = dcn_plan(a, chunk);
+    if (int rc = check_workspace(dcn_workspace_bytes(pl), workspace, workspace_bytes)) return rc;
+    a.input = input; a.offset = offset; a.mask = mask; a.weight = weight; a.grad_out = grad_output;
+    a.grad_input = grad_input; a.grad_offset = grad_offset; a.grad_mask = grad_mask; a.grad_weight = grad_weight;
+    a.grad_bias = grad_bias;
+    a.cols = static_cast<float *>(workspace);
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int P = a.Ho * a.Wo, T = a.kh * a.kw;
+    const long long K = (long long)a.C * T;
+    float *part = pl.splits > 1 ? reinterpret_cast<float *>(static_cast<char *>(workspace) + pl.cols_bytes) : a.grad_weight;
+    cudaError_t e = cudaMemsetAsync(a.grad_input, 0, (size_t)a.B * a.C * a.H * a.W * sizeof(float), st);
+    if (e != cudaSuccess) return cuda_fail(e, "dcn backward kernels");
+    for (int b0 = 0; b0 < a.B; b0 += pl.chunk) {
+        const int nb = a.B - b0 < pl.chunk ? a.B - b0 : pl.chunk;
+        const dim3 grid((P + BN - 1) / BN, (unsigned)((K + BM - 1) / BM), nb);
+        if (tf32)
+            dcn_grad_cols_tf32_kernel<<<grid, NT, 0, st>>>(a, b0);
+        else
+            dcn_grad_cols_kernel<<<grid, NT, 0, st>>>(a, b0);
+        dcn_grad_coord_kernel<<<dim3((P + 255) / 256, a.dg * T, nb), 256, 0, st>>>(a, b0);
+        dcn_grad_input_kernel<<<dim3((P + 255) / 256, a.dg * T, nb), 256, 0, st>>>(a, b0);
+    }
+    const dim3 gw_grid((unsigned)pl.ntile_n, (a.Co + BM - 1) / BM, pl.splits);
+    if (tf32)
+        dcn_grad_weight_tf32_kernel<<<gw_grid, NT, 0, st>>>(a, pl.span, part);
+    else
+        dcn_grad_weight_kernel<<<gw_grid, NT, 0, st>>>(a, pl.span, part);
+    if (pl.splits > 1) {
+        const long long n = (long long)a.Co * K;
+        dcn_reduce_splits_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(part, a.grad_weight, n, pl.splits);
+    }
+    dcn_grad_bias_kernel<<<a.Co, 256, 0, st>>>(a);
+    e = cudaGetLastError();
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "dcn backward kernels");
+}
+
+static_assert(TF_BM == BM && TF_BN == BN && TF_BK == BK, "the TF32 backward kernels run on dcn_plan's tiles");
+
 } // namespace
 
 } // namespace pvb
@@ -888,38 +1272,39 @@ PVB_API int pvb_dcn_backward(const pvb_dcn_desc *d, const float *input, const fl
                              float *grad_mask, float *grad_weight, float *grad_bias, int32_t chunk, void *workspace,
                              size_t workspace_bytes, pvb_stream_t stream)
 {
+    return dcn_backward(d, input, offset, mask, weight, grad_output, grad_input, grad_offset, grad_mask, grad_weight,
+                        grad_bias, chunk, workspace, workspace_bytes, false, stream);
+}
+
+PVB_API int pvb_dcn_forward_tf32(const pvb_dcn_desc *d, const float *input, const float *offset, const float *mask,
+                                 const float *weight, const float *bias, float *output, pvb_stream_t stream)
+{
     DcnArgs a;
     if (int rc = dcn_args(d, a)) return rc;
     if (a.B == 0) return PVB_OK;
-    if (!input || !offset || !mask || !weight || !grad_output || !grad_input || !grad_offset || !grad_mask ||
-        !grad_weight || !grad_bias)
-        return fail(PVB_ERR_INVALID, "NULL tensor");
-    const DcnPlan pl = dcn_plan(a, chunk);
-    if (int rc = check_workspace(dcn_workspace_bytes(pl), workspace, workspace_bytes)) return rc;
-    a.input = input; a.offset = offset; a.mask = mask; a.weight = weight; a.grad_out = grad_output;
-    a.grad_input = grad_input; a.grad_offset = grad_offset; a.grad_mask = grad_mask; a.grad_weight = grad_weight;
-    a.grad_bias = grad_bias;
-    a.cols = static_cast<float *>(workspace);
-    const cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int P = a.Ho * a.Wo, T = a.kh * a.kw;
-    const long long K = (long long)a.C * T;
-    float *part = pl.splits > 1 ? reinterpret_cast<float *>(static_cast<char *>(workspace) + pl.cols_bytes) : a.grad_weight;
-    cudaError_t e = cudaMemsetAsync(a.grad_input, 0, (size_t)a.B * a.C * a.H * a.W * sizeof(float), st);
-    if (e != cudaSuccess) return cuda_fail(e, "dcn backward kernels");
-    for (int b0 = 0; b0 < a.B; b0 += pl.chunk) {
-        const int nb = a.B - b0 < pl.chunk ? a.B - b0 : pl.chunk;
-        dcn_grad_cols_kernel<<<dim3((P + BN - 1) / BN, (unsigned)((K + BM - 1) / BM), nb), NT, 0, st>>>(a, b0);
-        dcn_grad_coord_kernel<<<dim3((P + 255) / 256, a.dg * T, nb), 256, 0, st>>>(a, b0);
-        dcn_grad_input_kernel<<<dim3((P + 255) / 256, a.dg * T, nb), 256, 0, st>>>(a, b0);
-    }
-    dcn_grad_weight_kernel<<<dim3((unsigned)pl.ntile_n, (a.Co + BM - 1) / BM, pl.splits), NT, 0, st>>>(a, pl.span, part);
-    if (pl.splits > 1) {
-        const long long n = (long long)a.Co * K;
-        dcn_reduce_splits_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(part, a.grad_weight, n, pl.splits);
-    }
-    dcn_grad_bias_kernel<<<a.Co, 256, 0, st>>>(a);
-    e = cudaGetLastError();
-    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "dcn backward kernels");
+    if (!input || !offset || !mask || !weight || !bias || !output) return fail(PVB_ERR_INVALID, "NULL tensor");
+    a.input = input; a.offset = offset; a.mask = mask; a.weight = weight; a.bias = bias; a.out = output;
+    const int S = dcn_tf32_splits(a);
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)(((long long)a.Ho * a.Wo + TF_BN - 1) / TF_BN * S), (a.Co + TF_BM - 1) / TF_BM, a.B);
+    cfg.blockDim = dim3(NT);
+    cfg.stream = static_cast<cudaStream_t>(stream);
+    cudaLaunchAttribute cluster;
+    cluster.id = cudaLaunchAttributeClusterDimension;
+    cluster.val.clusterDim.x = S; cluster.val.clusterDim.y = 1; cluster.val.clusterDim.z = 1;
+    cfg.attrs = &cluster;
+    cfg.numAttrs = S > 1 ? 1 : 0;
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, dcn_forward_tf32_kernel, a, S);
+    return e == cudaSuccess ? PVB_OK : cuda_fail(e, "dcn tf32 forward kernel");
+}
+
+PVB_API int pvb_dcn_backward_tf32(const pvb_dcn_desc *d, const float *input, const float *offset, const float *mask,
+                                  const float *weight, const float *grad_output, float *grad_input, float *grad_offset,
+                                  float *grad_mask, float *grad_weight, float *grad_bias, int32_t chunk, void *workspace,
+                                  size_t workspace_bytes, pvb_stream_t stream)
+{
+    return dcn_backward(d, input, offset, mask, weight, grad_output, grad_input, grad_offset, grad_mask, grad_weight,
+                        grad_bias, chunk, workspace, workspace_bytes, true, stream);
 }
 
 } // extern "C"

@@ -25,6 +25,15 @@ copy of the input; offset and mask are brought to channels_last (a no-op for the
 input), and the output is channels_last with the values the NCHW call returns, bit for bit.  Every other input (fp32 in
 any layout, NCHW, or contiguous in both layouts) is made NCHW-contiguous and returns NCHW, as before.  The backward is
 the same in both layouts: NCHW fp32, so a channels_last call's gradients equal the NCHW call's.
+
+TF32 follows torch's matmul switch, read on every call as torch.matmul reads it (tf32_enabled):
+torch.backends.cuda.matmul.fp32_precision == "tf32", which torch.set_float32_matmul_precision("high" / "medium"),
+torch.backends.cuda.matmul.allow_tf32 = True and torch.backends.fp32_precision = "tf32" all set.  When it is on, an fp32
+forward runs pvb_dcn_forward_tf32 and every backward (fp32, or the one on the up-cast operands of an fp16 / bf16
+forward) runs pvb_dcn_backward_tf32: the same columns, with each product's operands rounded once to TF32 and summed in
+fp32 on the tensor cores (DESIGN.md section 8p).  The fp16 / bf16 forward is the same with the switch on or off.  When
+it is off (torch's default), nothing here differs from the FP32-FFMA path.  torch.backends.cudnn.allow_tf32 is not
+followed: DCN's product is a GEMM, and it defaults to True.
 """
 import ctypes
 import math
@@ -113,6 +122,18 @@ def _nhwc(input):
     return input.is_contiguous(memory_format=torch.channels_last) and not input.is_contiguous()
 
 
+def tf32_enabled():
+    """Whether fp32 products may round their operands to TF32: torch's matmul flag.  matmul.fp32_precision is readable
+    whichever API set it ("tf32" on; "none", the default, or "ieee" off); reading allow_tf32 or
+    get_float32_matmul_precision() raises once the new API is in use, so they are read only on a torch without it."""
+    matmul = torch.backends.cuda.matmul
+    try:
+        precision = matmul.fp32_precision
+    except AttributeError:                                   # torch < 2.9
+        return bool(matmul.allow_tf32)
+    return precision == "tf32"
+
+
 def _call(entry, dev, *args):
     args = [ctypes.c_void_p(a.data_ptr()) if isinstance(a, torch.Tensor) else a for a in args]
     with torch.cuda.device(dev):
@@ -129,7 +150,11 @@ def dcn_forward(input, offset, mask, weight, bias, stride, padding, dilation, de
     nhwc = _nhwc(input)
     layout = torch.channels_last if nhwc else torch.contiguous_format
     out = torch.empty((d.B, d.C_out, ho, wo), dtype=input.dtype, device=input.device, memory_format=layout)
-    if d.B and input.dtype == torch.float32:
+    if d.B and input.dtype == torch.float32 and tf32_enabled():
+        x, off, m, b = (t.contiguous() for t in (input, offset, mask, bias))
+        w = weight.permute(0, 2, 3, 1).contiguous()          # tap-major [C_out, kh, kw, C], as the kernel reads it
+        _call("pvb_dcn_forward_tf32", input.device, ctypes.byref(d), x, off, m, w, b, out)
+    elif d.B and input.dtype == torch.float32:
         c = [t.contiguous() for t in (input, offset, mask, weight, bias)]
         _call("pvb_dcn_forward", input.device, ctypes.byref(d), *c, out)
     elif d.B and nhwc:
@@ -147,7 +172,8 @@ def dcn_forward(input, offset, mask, weight, bias, stride, padding, dilation, de
 def dcn_backward(input, offset, mask, weight, bias, grad_output, stride, padding, dilation, deformable_groups,
                  max_column_bytes=None):
     """(grad_input, grad_offset, grad_mask, grad_weight, grad_bias) of dcn_v2_conv for grad_output; no host sync.
-    grad_cols goes through a workspace of at most max_column_bytes (default MAX_COLUMN_BYTES) per image chunk."""
+    grad_cols goes through a workspace of at most max_column_bytes (default MAX_COLUMN_BYTES) per image chunk.  Runs
+    pvb_dcn_backward_tf32 when tf32_enabled() holds at the call, pvb_dcn_backward otherwise."""
     d = _desc(input, weight, stride, padding, dilation, deformable_groups)
     _check(input, offset, mask, weight, bias, d)
     ho, wo = _out_hw(d)
@@ -166,7 +192,8 @@ def dcn_backward(input, offset, mask, weight, bias, grad_output, stride, padding
     lib = _lib.load()
     nbytes = lib.pvb_dcn_backward_workspace_bytes(ctypes.byref(d), chunk)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=input.device)
-    _call("pvb_dcn_backward", input.device, ctypes.byref(d), *c, *grads, chunk, ws, nbytes)
+    entry = "pvb_dcn_backward_tf32" if tf32_enabled() else "pvb_dcn_backward"
+    _call(entry, input.device, ctypes.byref(d), *c, *grads, chunk, ws, nbytes)
     return tuple(grads)
 
 

@@ -653,6 +653,23 @@ PVB_API int pvb_dcn_backward(const pvb_dcn_desc *d, const float *input, const fl
                              float *grad_mask, float *grad_weight, float *grad_bias, int32_t chunk, void *workspace,
                              size_t workspace_bytes, pvb_stream_t stream);
 
+/* The fp32 convolution on TF32 tensor cores (DESIGN.md section 8p), what dcn_v2_conv runs for fp32 inputs when torch
+ * allows TF32 matmuls.  pvb_dcn_forward_tf32 takes pvb_dcn_forward's tensors except that the weight is tap-major,
+ * [C_out][kh][kw][C] (weight.permute(0, 2, 3, 1)), as pvb_dcn_forward_half's; the column entries are pvb_dcn_forward's
+ * bit for bit, and output = bias + sum RN_tf32(weight) * RN_tf32(cols) in fp32 on the tensor cores, each operand
+ * rounded once (cvt.rna: to nearest, ties away from zero).  pvb_dcn_backward_tf32 takes pvb_dcn_backward's arguments
+ * and workspace (pvb_dcn_backward_workspace_bytes: the plan is the same) and runs its kernels, except that grad_cols
+ * = RN_tf32(weight)^T . RN_tf32(grad_output) and grad_weight = RN_tf32(grad_output) . RN_tf32(cols)^T run on the
+ * tensor cores; grad_bias is pvb_dcn_backward's bit for bit.  Same checks, refusals, limits and guarantees as the
+ * fp32 entries: bit-identical run to run (every backward output but grad_input), an image's output independent of the
+ * batch, the backward independent of `chunk`, B == 0 a no-op, no host synchronisation, no allocation. */
+PVB_API int pvb_dcn_forward_tf32(const pvb_dcn_desc *d, const float *input, const float *offset, const float *mask,
+                                 const float *weight, const float *bias, float *output, pvb_stream_t stream);
+PVB_API int pvb_dcn_backward_tf32(const pvb_dcn_desc *d, const float *input, const float *offset, const float *mask,
+                                  const float *weight, const float *grad_output, float *grad_input, float *grad_offset,
+                                  float *grad_mask, float *grad_weight, float *grad_bias, int32_t chunk, void *workspace,
+                                  size_t workspace_bytes, pvb_stream_t stream);
+
 /* ---- DCNv2's deformable PSROI pooling (DESIGN.md section 8m) -------------------------------------------------------
  * The other half of lib/csrc/dcn_v2 (dcn_v2_psroi_pooling_cuda.cu), behind DCNv2Pooling / DCNPooling.  Shapes: input
  * [B,C,H,W], rois [n_roi,5] = (batch, x1, y1, x2, y2), trans [n_roi, 2*num_classes, part_size, part_size] ((x, y)
